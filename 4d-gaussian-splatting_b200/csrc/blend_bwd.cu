@@ -40,6 +40,25 @@ __device__ __forceinline__ float ex2_approx(float x) {
     return y;
 }
 
+// Per-pixel background image (BlendBwdParams::bg_image): the colour behind the last Gaussian becomes bg + bg_image[pix],
+// which only changes the background term of dL/dalpha.  dL/dbg_image = (1 - alpha) dL/dpix with alpha = 1 - T_final,
+// rounded as PyTorch rounds that expression; it is written here, before the tile loop, so that the pixels of tiles
+// with an empty list get theirs too.
+__device__ __forceinline__ void background_image_terms(const BlendBwdParams& p, int pix_id, int HW, float T_final, float gp0,
+                                                       float gp1, float gp2, float& bg0, float& bg1, float& bg2) {
+    if (p.bg_image) {
+        bg0 += p.bg_image[0 * HW + pix_id];
+        bg1 += p.bg_image[1 * HW + pix_id];
+        bg2 += p.bg_image[2 * HW + pix_id];
+    }
+    if (p.dL_dbg_image) {
+        const float w = __fsub_rn(1.0f, __fsub_rn(1.0f, T_final));
+        p.dL_dbg_image[0 * HW + pix_id] = __fmul_rn(w, gp0);
+        p.dL_dbg_image[1 * HW + pix_id] = __fmul_rn(w, gp1);
+        p.dL_dbg_image[2 * HW + pix_id] = __fmul_rn(w, gp2);
+    }
+}
+
 template <bool AUX>
 __global__ void __launch_bounds__(BB_THREADS, AUX ? 3 : 4) blend_bwd_kernel(const BlendBwdParams p) {
     __shared__ BlendBwdSmem sm;
@@ -99,8 +118,10 @@ __global__ void __launch_bounds__(BB_THREADS, AUX ? 3 : 4) blend_bwd_kernel(cons
             if (p.dL_masks) gm = p.dL_masks[pix_id];
         }
     }
+    float bg0 = p.background[0], bg1 = p.background[1], bg2 = p.background[2];
+    if (inside) background_image_terms(p, pix_id, HW, T_final, gp0, gp1, gp2, bg0, bg1, bg2);
     // background term of dL_dalpha, backward.cu:1110-1113:  (-T_final / (1 - alpha)) * (bg . dL_dpixel)
-    const float tb = -T_final * (p.background[0] * gp0 + p.background[1] * gp1 + p.background[2] * gp2);
+    const float tb = -T_final * (bg0 * gp0 + bg1 * gp1 + bg2 * gp2);
 
     // Reduce-scatter targets.  AUX: 12 values { dcolor r,g,b | dmean2D x,y,depth | dconic x,y,w |
     // dflow x,y, dopacity }, value 6*b4 + 3*b3 + (b1 ? 2 : b2) ends on the even lanes (b_k = bit k of
@@ -440,7 +461,9 @@ __global__ void __launch_bounds__(B2_THREADS, (ACOL_SMEM && !AUX) ? 4 : 3) blend
             if (p.dL_masks) gm = p.dL_masks[pix_id];
         }
     }
-    const float tb = -T_final * (p.background[0] * gp0 + p.background[1] * gp1 + p.background[2] * gp2);
+    float bg0 = p.background[0], bg1 = p.background[1], bg2 = p.background[2];
+    if (inside) background_image_terms(p, pix_id, HW, T_final, gp0, gp1, gp2, bg0, bg1, bg2);
+    const float tb = -T_final * (bg0 * gp0 + bg1 * gp1 + bg2 * gp2);
 
     // ---- constant A fragments (m16n8k8: a0 = A[g][t], a2 = A[g][t + 4], g = lane / 4, t = lane % 4; k = pixel) ----
     // colour tile: rows 0..2 = hi part of the colour gradient of pixel k, rows 4..6 = its lo part

@@ -168,9 +168,18 @@ __global__ void __launch_bounds__(BF_THREADS) blend_fwd_kernel(const BlendFwdPar
         p.final_T[pix_id] = T;
         p.out_T[pix_id] = T;
         p.n_contrib[pix_id] = last_contributor;
-        p.out_color[0 * HW + pix_id] = ffma(T, p.background[0], C0);
-        p.out_color[1 * HW + pix_id] = ffma(T, p.background[1], C1);
-        p.out_color[2 * HW + pix_id] = ffma(T, p.background[2], C2);
+        float o0 = ffma(T, p.background[0], C0), o1 = ffma(T, p.background[1], C1), o2 = ffma(T, p.background[2], C2);
+        if (p.bg_image) {
+            // out + (1 - alpha) * bg_image with alpha = 1 - T, rounded step by step exactly as PyTorch evaluates that
+            // expression on the returned images (no contraction into an FMA)
+            const float w = __fsub_rn(1.0f, __fsub_rn(1.0f, T));
+            o0 = __fadd_rn(o0, __fmul_rn(w, p.bg_image[0 * HW + pix_id]));
+            o1 = __fadd_rn(o1, __fmul_rn(w, p.bg_image[1 * HW + pix_id]));
+            o2 = __fadd_rn(o2, __fmul_rn(w, p.bg_image[2 * HW + pix_id]));
+        }
+        p.out_color[0 * HW + pix_id] = o0;
+        p.out_color[1 * HW + pix_id] = o1;
+        p.out_color[2 * HW + pix_id] = o2;
         p.out_flow[0 * HW + pix_id] = F0;
         p.out_flow[1 * HW + pix_id] = F1;
         p.out_depth[pix_id] = Dp;

@@ -208,8 +208,12 @@ size_t fdgs_geom_bytes(int P) { return GeomState::carve(nullptr, P).bytes + 128;
 size_t fdgs_image_bytes(int width, int height) { return ImageState::carve(nullptr, width, height).bytes + 128; }
 size_t fdgs_binning_bytes(int num_rendered, int, int) { return BinningState::carve(nullptr, num_rendered).bytes + 128; }
 
-int fdgs_forward(const fdgs_forward_args* a, fdgs_alloc_fn geom_alloc, void* geom_ctx, fdgs_alloc_fn binning_alloc,
-                 void* binning_ctx, fdgs_alloc_fn image_alloc, void* image_ctx, void* stream_v,
+}  // extern "C"
+
+namespace {
+
+int forward_impl(const fdgs_forward_args* a, const float* bg_image, fdgs_alloc_fn geom_alloc, void* geom_ctx,
+                 fdgs_alloc_fn binning_alloc, void* binning_ctx, fdgs_alloc_fn image_alloc, void* image_ctx, void* stream_v,
                  fdgs_forward_result* res) {
     g_last_error.clear();
     if (!a || !res || !geom_alloc || !binning_alloc || !image_alloc) return fail(FDGS_ERR_INVALID_ARG, "null argument");
@@ -330,19 +334,34 @@ int fdgs_forward(const fdgs_forward_args* a, fdgs_alloc_fn geom_alloc, void* geo
     bp.ranges = img.ranges; bp.recs = bin.recs; bp.background = a->background;
     bp.final_T = img.final_T; bp.n_contrib = img.n_contrib;
     bp.out_color = a->out_color; bp.out_flow = a->out_flow; bp.out_depth = a->out_depth; bp.out_T = a->out_T;
+    bp.bg_image = bg_image;
     (void)N;
     FDGS_STAGE(5, 1, fdgs::launch_blend_fwd(bp, stream), "blend_fwd");
     return FDGS_OK;
 }
 
-int fdgs_backward(const fdgs_backward_args* a, void* stream_v) {
+int backward_impl(const fdgs_backward_args* a, const float* bg_image, float* dL_dbg_image, void* stream_v) {
     g_last_error.clear();
     if (!a) return fail(FDGS_ERR_INVALID_ARG, "null argument");
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
     const bool debug = a->debug != 0;
     const int P = a->P, W = a->width, H = a->height, R = a->R;
-    if (P <= 0) return FDGS_OK;
+    if (P <= 0 && !dL_dbg_image) return FDGS_OK;
     if (W <= 0 || H <= 0 || R < 0) return fail(FDGS_ERR_INVALID_ARG, "bad width / height / R");
+    if (P <= 0) {
+        // nothing was rendered: the background image takes the whole colour gradient (the blend kernel walks empty
+        // tile lists and writes dL_dbg_image only)
+        if (!a->image_buffer || !a->dL_dpix || !a->background)
+            return fail(FDGS_ERR_INVALID_ARG, "image buffer / colour image gradient / background required");
+        ImageState img = ImageState::carve(align128(const_cast<char*>(a->image_buffer)), W, H);
+        fdgs::BlendBwdParams bp;
+        memset(&bp, 0, sizeof(bp));
+        bp.W = W; bp.H = H; bp.grid_x = (W + fdgs::TILE_X - 1) / fdgs::TILE_X; bp.grid_y = (H + fdgs::TILE_Y - 1) / fdgs::TILE_Y;
+        bp.ranges = img.ranges; bp.background = a->background; bp.final_T = img.final_T; bp.n_contrib = img.n_contrib;
+        bp.dL_dpix = a->dL_dpix; bp.bg_image = bg_image; bp.dL_dbg_image = dL_dbg_image;
+        FDGS_STAGE(6, 1, fdgs::launch_blend_bwd(bp, stream), "blend_bwd");
+        return FDGS_OK;
+    }
     if (!a->geom_buffer || !a->image_buffer || (R > 0 && !a->binning_buffer))
         return fail(FDGS_ERR_INVALID_ARG, "scratch buffers of the forward pass required");
     // dL_depths / dL_masks / dL_dpix_flow may be NULL: no upstream gradient for that image
@@ -359,7 +378,8 @@ int fdgs_backward(const fdgs_backward_args* a, void* stream_v) {
     BinningState bin = BinningState::carve(a->binning_buffer ? align128(const_cast<char*>(a->binning_buffer)) : nullptr, R);
 
     bool blend_raw = false;
-    if (R > 0) {
+    // with no instance at all the blend only has dL_dbg_image to write
+    if (R > 0 || dL_dbg_image) {
         fdgs::BlendBwdParams bp;
         bp.W = W; bp.H = H; bp.grid_x = grid_x; bp.grid_y = grid_y;
         bp.ranges = img.ranges; bp.recs = bin.recs; bp.background = a->background;
@@ -367,7 +387,8 @@ int fdgs_backward(const fdgs_backward_args* a, void* stream_v) {
         bp.dL_dpix = a->dL_dpix; bp.dL_depths = a->dL_depths; bp.dL_masks = a->dL_masks; bp.dL_dpix_flow = a->dL_dpix_flow;
         bp.dL_dmean2D = a->dL_dmean2D; bp.dL_dconic = a->dL_dconic; bp.dL_dopacity = a->dL_dopacity;
         bp.dL_dcolor = a->dL_dcolor; bp.dL_dflows = a->dL_dflows;
-        blend_raw = fdgs::blend_bwd_is_raw(bp);
+        bp.bg_image = bg_image; bp.dL_dbg_image = dL_dbg_image;
+        blend_raw = R > 0 && fdgs::blend_bwd_is_raw(bp);
         FDGS_STAGE(6, 1, fdgs::launch_blend_bwd(bp, stream), "blend_bwd");
     }
     fdgs::PreprocessBwdParams pb;
@@ -399,6 +420,63 @@ int fdgs_backward(const fdgs_backward_args* a, void* stream_v) {
     if (pb.has_scales && pb.rot_4d && (!a->rotations_r || !a->scales_t || !a->ts || !a->opacities))
         return fail(FDGS_ERR_INVALID_ARG, "rot_4d backward needs rotations_r, scales_t, ts, opacities");
     FDGS_STAGE(7, fdgs::preprocess_bwd_kernel_count(pb), fdgs::launch_preprocess_bwd(pb, stream), "preprocess_bwd");
+    return FDGS_OK;
+}
+
+int check_sky_args(const fdgs_sky_args* a) {
+    if (!a) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    if (!a->env_map || !a->c2w || !a->campos) return fail(FDGS_ERR_INVALID_ARG, "env_map / c2w / campos required");
+    if (a->env_height <= 0 || a->env_width <= 0 || a->env_width > 65000 || a->width <= 0 || a->height <= 0)
+        return fail(FDGS_ERR_INVALID_ARG, "bad environment map / image size");
+    if (!(a->radius > 0.0f)) return fail(FDGS_ERR_INVALID_ARG, "sky radius must be positive");
+    return FDGS_OK;
+}
+
+fdgs::SkyParams sky_params(const fdgs_sky_args* a) {
+    fdgs::SkyParams p;
+    p.env_map = a->env_map; p.env_height = a->env_height; p.env_width = a->env_width;
+    p.c2w = a->c2w; p.campos = a->campos;
+    p.fl_x = a->fl_x; p.fl_y = a->fl_y; p.cx = a->cx; p.cy = a->cy; p.radius = a->radius;
+    p.W = a->width; p.H = a->height;
+    return p;
+}
+
+}  // namespace
+
+extern "C" {
+
+int fdgs_forward(const fdgs_forward_args* a, fdgs_alloc_fn geom_alloc, void* geom_ctx, fdgs_alloc_fn binning_alloc,
+                 void* binning_ctx, fdgs_alloc_fn image_alloc, void* image_ctx, void* stream, fdgs_forward_result* res) {
+    return forward_impl(a, nullptr, geom_alloc, geom_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, stream, res);
+}
+
+int fdgs_forward_bg(const fdgs_forward_args* a, const float* bg_image, fdgs_alloc_fn geom_alloc, void* geom_ctx,
+                    fdgs_alloc_fn binning_alloc, void* binning_ctx, fdgs_alloc_fn image_alloc, void* image_ctx, void* stream,
+                    fdgs_forward_result* res) {
+    return forward_impl(a, bg_image, geom_alloc, geom_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, stream, res);
+}
+
+int fdgs_backward(const fdgs_backward_args* a, void* stream) { return backward_impl(a, nullptr, nullptr, stream); }
+
+int fdgs_backward_bg(const fdgs_backward_args* a, const float* bg_image, float* dL_dbg_image, void* stream) {
+    return backward_impl(a, bg_image, dL_dbg_image, stream);
+}
+
+int fdgs_sky_forward(const fdgs_sky_args* a, float* out_sky, int* miss_flag, void* stream_v) {
+    g_last_error.clear();
+    if (int rc = check_sky_args(a)) return rc;
+    if (!out_sky) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    FDGS_CUDA(fdgs::launch_sky_fwd(sky_params(a), out_sky, miss_flag, reinterpret_cast<cudaStream_t>(stream_v)), "sky_forward");
+    g_kernel_launches += 1;
+    return FDGS_OK;
+}
+
+int fdgs_sky_backward(const fdgs_sky_args* a, const float* dL_dsky, float* dL_denv, void* stream_v) {
+    g_last_error.clear();
+    if (int rc = check_sky_args(a)) return rc;
+    if (!dL_dsky || !dL_denv) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    FDGS_CUDA(fdgs::launch_sky_bwd(sky_params(a), dL_dsky, dL_denv, reinterpret_cast<cudaStream_t>(stream_v)), "sky_backward");
+    g_kernel_launches += 1;
     return FDGS_OK;
 }
 

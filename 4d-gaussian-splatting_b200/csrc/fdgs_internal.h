@@ -103,6 +103,7 @@ struct BlendFwdParams {
     float* out_flow;       // [2,H,W]
     float* out_depth;      // [H,W]
     float* out_T;          // [H,W]
+    const float* bg_image; // [3,H,W] per-pixel background behind the Gaussians, or NULL
 };
 cudaError_t launch_blend_fwd(const BlendFwdParams& p, cudaStream_t stream);
 
@@ -122,6 +123,8 @@ struct BlendBwdParams {
     float* dL_dopacity;   // [P]
     float* dL_dcolor;     // [P,3]
     float* dL_dflows;     // [P,2]
+    const float* bg_image;   // [3,H,W] or NULL (BlendFwdParams::bg_image)
+    float* dL_dbg_image;     // [3,H,W] overwritten for every pixel, or NULL
 };
 cudaError_t launch_blend_bwd(const BlendBwdParams& p, cudaStream_t stream);
 // true when launch_blend_bwd(p) leaves RAW moment sums (W10, W01 | W20, W11, W02 | W00 of w = G dL/dalpha
@@ -228,5 +231,19 @@ cudaError_t launch_knn_bruteforce(int n, int k, const float* xyz, int* idx, floa
 
 cudaError_t launch_mark_visible(int P, const float* means3D, const float* viewmatrix, unsigned char* present,
                                 cudaStream_t stream);
+
+// ---- environment-map sky (sky.cu) ------------------------------------------------------------------
+struct SkyParams {
+    const float* env_map;   // [3,Hm,Wm]
+    int env_height, env_width;
+    const float* c2w;       // [16] row-major camera-to-world
+    const float* campos;    // [3]
+    float fl_x, fl_y, cx, cy, radius;
+    int W, H;
+};
+// out_sky [3,H,W]; miss_flag[0] = 1 if a ray misses the sphere (may be NULL)
+cudaError_t launch_sky_fwd(const SkyParams& p, float* out_sky, int* miss_flag, cudaStream_t stream);
+// dL_denv [3,Hm,Wm] += the bilinear taps' share of dL_dsky [3,H,W]
+cudaError_t launch_sky_bwd(const SkyParams& p, const float* dL_dsky, float* dL_denv, cudaStream_t stream);
 
 }  // namespace fdgs

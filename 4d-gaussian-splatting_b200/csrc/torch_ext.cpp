@@ -43,6 +43,16 @@ const float* fptr(const torch::Tensor& t) {
 
 torch::Tensor contig(const torch::Tensor& t) { return (t.defined() && t.numel() > 0) ? t.contiguous() : t; }
 
+// the per-pixel background image of a call, checked against the image size (undefined / empty = none)
+torch::Tensor background_image(const torch::Tensor& bg_image, const torch::Tensor& like, int H, int W) {
+    if (!bg_image.defined() || bg_image.numel() == 0) return torch::Tensor();
+    TORCH_CHECK(bg_image.is_cuda() && bg_image.device() == like.device(), "fdgs: bg_image must be on the device of means3D");
+    TORCH_CHECK(bg_image.scalar_type() == torch::kFloat32, "fdgs: bg_image must be float32");
+    TORCH_CHECK(bg_image.dim() == 3 && bg_image.size(0) == 3 && bg_image.size(1) == H && bg_image.size(2) == W,
+                "fdgs: bg_image must be [3, image_height, image_width]");
+    return bg_image.contiguous();
+}
+
 void check(int rc, const char* where) {
     if (rc != FDGS_OK) throw std::runtime_error(std::string("fdgs ") + where + " failed: " + fdgs_last_error());
 }
@@ -68,7 +78,7 @@ using ForwardOut = std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, 
 
 // sh_rest (possibly empty) / raw_params: the raw-parameter entry of include/fdgs.h (fdgs_forward_args.raw_params)
 static ForwardOut
-forward_impl(const torch::Tensor& sh_rest, const bool raw_params,
+forward_impl(const torch::Tensor& bg_image, const torch::Tensor& sh_rest, const bool raw_params,
                        const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors,
                        const torch::Tensor& flows, const torch::Tensor& opacity, const torch::Tensor& ts,
                        const torch::Tensor& scales, const torch::Tensor& scales_t, const torch::Tensor& rotations,
@@ -131,8 +141,10 @@ forward_impl(const torch::Tensor& sh_rest, const bool raw_params,
     a.out_flow = out_flow.data_ptr<float>(); a.out_depth = out_depth.data_ptr<float>();
     a.out_T = out_T.data_ptr<float>(); a.radii = radii.data_ptr<int>();
 
+    const auto bgi_c = background_image(bg_image, means3D, H, W);
     fdgs_forward_result r;
-    check(fdgs_forward(&a, resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer, (void*)stream, &r),
+    check(fdgs_forward_bg(&a, fptr(bgi_c), resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer,
+                          (void*)stream, &r),
           "forward");
 
     torch::Tensor covs3D_com;
@@ -147,24 +159,35 @@ forward_impl(const torch::Tensor& sh_rest, const bool raw_params,
 }
 
 // the reference's entry point: 30 positional arguments, 11-tuple (rasterize_points.h:18-49)
-ForwardOut RasterizeGaussiansCUDA(FDGS_FWD_PARAMS) { return forward_impl(torch::Tensor(), false, FDGS_FWD_ARGS); }
+ForwardOut RasterizeGaussiansCUDA(FDGS_FWD_PARAMS) { return forward_impl(torch::Tensor(), torch::Tensor(), false, FDGS_FWD_ARGS); }
+
+// the same + a per-pixel background image bg_image [3,H,W] (include/fdgs.h: fdgs_forward_bg; empty = none)
+ForwardOut RasterizeGaussiansBg(FDGS_FWD_PARAMS, const torch::Tensor& bg_image) {
+    return forward_impl(bg_image, torch::Tensor(), false, FDGS_FWD_ARGS);
+}
 
 // raw-parameter entry: the same 30 arguments (scales = log-scales, rotations un-normalised, opacity = logits when
 // raw_params) + the second SH tensor (sh = features_dc [P,1,3], sh_rest = features_rest [P,M-1,3]; may be empty)
 ForwardOut RasterizeGaussiansRaw(FDGS_FWD_PARAMS, const torch::Tensor& sh_rest, const bool raw_params) {
-    return forward_impl(sh_rest, raw_params, FDGS_FWD_ARGS);
+    return forward_impl(torch::Tensor(), sh_rest, raw_params, FDGS_FWD_ARGS);
+}
+
+ForwardOut RasterizeGaussiansRawBg(FDGS_FWD_PARAMS, const torch::Tensor& sh_rest, const bool raw_params,
+                                   const torch::Tensor& bg_image) {
+    return forward_impl(bg_image, sh_rest, raw_params, FDGS_FWD_ARGS);
 }
 
 namespace {
 struct BackwardOut {
     torch::Tensor dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dflows, dL_dts, dL_dscales,
-        dL_dscales_t, dL_drotations, dL_drotations_r, sh_factors, dL_dsh_rest;
+        dL_dscales_t, dL_drotations, dL_drotations_r, sh_factors, dL_dsh_rest, dL_dbg_image;
 };
 }  // namespace
 
 // sh_factor_mode: view-parallel mode -- no dL_dsh rows, the [P,3] colour factors instead (include/fdgs.h: sh_factors)
 static BackwardOut
-backward_impl(const bool sh_factor_mode, const torch::Tensor& sh_rest, const bool raw_params,
+backward_impl(const torch::Tensor& bg_image, const bool want_dbg, const bool sh_factor_mode, const torch::Tensor& sh_rest,
+                               const bool raw_params,
                                const torch::Tensor& background, const torch::Tensor& means3D,
                                const torch::Tensor& out_means3D, const torch::Tensor& radii, const torch::Tensor& colors,
                                const torch::Tensor& flows_2d, const torch::Tensor& opacities, const torch::Tensor& ts,
@@ -207,8 +230,11 @@ backward_impl(const bool sh_factor_mode, const torch::Tensor& sh_rest, const boo
     torch::Tensor dL_dscales_t = torch::empty({P, 1}, opts);
     torch::Tensor dL_drotations = torch::empty({P, 4}, opts);
     torch::Tensor dL_drotations_r = torch::empty({P, 4}, opts);
+    // overwritten for every pixel by the blend backward
+    torch::Tensor dL_dbg_image = want_dbg ? torch::empty({3, H, W}, opts) : torch::empty({0}, opts);
+    const auto bgi_c = background_image(bg_image, means3D, H, W);
 
-    if (P != 0) {
+    if (P != 0 || want_dbg) {
         const auto bg_c = contig(background), om_c = contig(out_means3D), rad_c = contig(radii), col_c = contig(colors),
                    flow_c = contig(flows_2d), op_c = contig(opacities), ts_c = contig(ts), sc_c = contig(scales),
                    sct_c = contig(scales_t), rot_c = contig(rotations), rotr_c = contig(rotations_r),
@@ -227,8 +253,8 @@ backward_impl(const bool sh_factor_mode, const torch::Tensor& sh_rest, const boo
         a.viewmatrix = fptr(view_c); a.projmatrix = fptr(proj_c); a.campos = fptr(cam_c);
         a.timestamp = timestamp; a.time_duration = time_duration; a.rot_4d = rot_4d; a.gaussian_dim = gaussian_dim;
         a.force_sh_3d = force_sh_3d; a.tan_fovx = tan_fovx; a.tan_fovy = tan_fovy;
-        a.radii = rad_c.data_ptr<int>();
-        a.geom_buffer = reinterpret_cast<const char*>(geo_c.data_ptr());
+        a.radii = rad_c.numel() ? rad_c.data_ptr<int>() : nullptr;
+        a.geom_buffer = geo_c.numel() ? reinterpret_cast<const char*>(geo_c.data_ptr()) : nullptr;
         a.binning_buffer = bin_c.numel() ? reinterpret_cast<const char*>(bin_c.data_ptr()) : nullptr;
         a.image_buffer = reinterpret_cast<const char*>(img_c.data_ptr());
         a.dL_dpix = fptr(gc_c); a.dL_depths = fptr(gd_c); a.dL_masks = fptr(gm_c); a.dL_dpix_flow = fptr(gf_c);
@@ -245,10 +271,11 @@ backward_impl(const bool sh_factor_mode, const torch::Tensor& sh_rest, const boo
         a.dL_dts = dL_dts.data_ptr<float>(); a.dL_dscale = dL_dscales.data_ptr<float>();
         a.dL_dscale_t = dL_dscales_t.data_ptr<float>(); a.dL_drot = dL_drotations.data_ptr<float>();
         a.dL_drot_r = dL_drotations_r.data_ptr<float>();
-        check(fdgs_backward(&a, (void*)stream), "backward");
+        check(fdgs_backward_bg(&a, fptr(bgi_c), want_dbg ? dL_dbg_image.data_ptr<float>() : nullptr, (void*)stream),
+              "backward");
     }
     return BackwardOut{dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dflows, dL_dts,
-                       dL_dscales, dL_dscales_t, dL_drotations, dL_drotations_r, sh_factors, dL_dsh_rest};
+                       dL_dscales, dL_dscales_t, dL_drotations, dL_drotations_r, sh_factors, dL_dsh_rest, dL_dbg_image};
 }
 
 #define FDGS_BWD_PARAMS                                                                                                \
@@ -273,16 +300,26 @@ backward_impl(const bool sh_factor_mode, const torch::Tensor& sh_rest, const boo
 std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor,
            torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
 RasterizeGaussiansBackwardCUDA(FDGS_BWD_PARAMS) {
-    BackwardOut o = backward_impl(false, torch::Tensor(), false, FDGS_BWD_ARGS);
+    BackwardOut o = backward_impl(torch::Tensor(), false, false, torch::Tensor(), false, FDGS_BWD_ARGS);
     return std::make_tuple(o.dL_dmeans2D, o.dL_dcolors, o.dL_dopacity, o.dL_dmeans3D, o.dL_dcov3D, o.dL_dsh, o.dL_dflows,
                            o.dL_dts, o.dL_dscales, o.dL_dscales_t, o.dL_drotations, o.dL_drotations_r);
 }
 
 // view-parallel variant: same arguments; dL_dsh comes back EMPTY and a 13th tensor holds the [P,3] colour factors
 std::vector<torch::Tensor> RasterizeGaussiansBackwardFactors(FDGS_BWD_PARAMS) {
-    BackwardOut o = backward_impl(true, torch::Tensor(), false, FDGS_BWD_ARGS);
+    BackwardOut o = backward_impl(torch::Tensor(), false, true, torch::Tensor(), false, FDGS_BWD_ARGS);
     return {o.dL_dmeans2D, o.dL_dcolors, o.dL_dopacity, o.dL_dmeans3D, o.dL_dcov3D, o.dL_dsh, o.dL_dflows,
             o.dL_dts, o.dL_dscales, o.dL_dscales_t, o.dL_drotations, o.dL_drotations_r, o.sh_factors};
+}
+
+// per-pixel background image (include/fdgs.h: fdgs_backward_bg): the 37 arguments + the forward's bg_image (empty =
+// none), the view-parallel switch of rasterize_gaussians_backward_factors and whether dL/dbg_image is wanted.  Returns
+// the 12 gradients, the [P,3] colour factors (sh_factor_mode, else empty) and dL_dbg_image [3,H,W] (else empty).
+std::vector<torch::Tensor> RasterizeGaussiansBackwardBg(FDGS_BWD_PARAMS, const torch::Tensor& bg_image, const bool sh_factor_mode,
+                                                        const bool want_dbg) {
+    BackwardOut o = backward_impl(bg_image, want_dbg, sh_factor_mode, torch::Tensor(), false, FDGS_BWD_ARGS);
+    return {o.dL_dmeans2D, o.dL_dcolors, o.dL_dopacity, o.dL_dmeans3D, o.dL_dcov3D, o.dL_dsh, o.dL_dflows, o.dL_dts,
+            o.dL_dscales, o.dL_dscales_t, o.dL_drotations, o.dL_drotations_r, o.sh_factors, o.dL_dbg_image};
 }
 
 // raw-parameter entry (see RasterizeGaussiansRaw): 14 tensors -- the 12 gradients (w.r.t. the RAW parameters when
@@ -290,9 +327,65 @@ std::vector<torch::Tensor> RasterizeGaussiansBackwardFactors(FDGS_BWD_PARAMS) {
 // dL_dsh_rest [P,M-1,3] (split rows, else empty)
 std::vector<torch::Tensor> RasterizeGaussiansBackwardRaw(FDGS_BWD_PARAMS, const torch::Tensor& sh_rest, const bool raw_params,
                                                          const bool sh_factor_mode) {
-    BackwardOut o = backward_impl(sh_factor_mode, sh_rest, raw_params, FDGS_BWD_ARGS);
+    BackwardOut o = backward_impl(torch::Tensor(), false, sh_factor_mode, sh_rest, raw_params, FDGS_BWD_ARGS);
     return {o.dL_dmeans2D, o.dL_dcolors, o.dL_dopacity, o.dL_dmeans3D, o.dL_dcov3D, o.dL_dsh, o.dL_dflows,
             o.dL_dts, o.dL_dscales, o.dL_dscales_t, o.dL_drotations, o.dL_drotations_r, o.sh_factors, o.dL_dsh_rest};
+}
+
+// the raw entry's 40 arguments + bg_image and want_dbg: its 14 tensors, then dL_dbg_image [3,H,W] (else empty)
+std::vector<torch::Tensor> RasterizeGaussiansBackwardRawBg(FDGS_BWD_PARAMS, const torch::Tensor& sh_rest, const bool raw_params,
+                                                           const bool sh_factor_mode, const torch::Tensor& bg_image,
+                                                           const bool want_dbg) {
+    BackwardOut o = backward_impl(bg_image, want_dbg, sh_factor_mode, sh_rest, raw_params, FDGS_BWD_ARGS);
+    return {o.dL_dmeans2D, o.dL_dcolors, o.dL_dopacity, o.dL_dmeans3D, o.dL_dcov3D, o.dL_dsh, o.dL_dflows, o.dL_dts,
+            o.dL_dscales, o.dL_dscales_t, o.dL_drotations, o.dL_drotations_r, o.sh_factors, o.dL_dsh_rest, o.dL_dbg_image};
+}
+
+// ---- environment-map sky (include/fdgs.h: fdgs_sky_forward / fdgs_sky_backward) -----------------------------------
+static fdgs_sky_args sky_args(const torch::Tensor& env_map, const torch::Tensor& c2w, const torch::Tensor& campos,
+                              const double fl_x, const double fl_y, const double cx, const double cy, const double radius,
+                              const int64_t H, const int64_t W) {
+    TORCH_CHECK(env_map.is_cuda() && env_map.scalar_type() == torch::kFloat32 && env_map.is_contiguous() && env_map.dim() == 3 &&
+                env_map.size(0) == 3, "fdgs: env_map must be a contiguous float32 CUDA tensor [3,Hm,Wm]");
+    TORCH_CHECK(c2w.is_cuda() && c2w.scalar_type() == torch::kFloat32 && c2w.is_contiguous() && c2w.numel() == 16 &&
+                campos.is_cuda() && campos.scalar_type() == torch::kFloat32 && campos.is_contiguous() && campos.numel() == 3,
+                "fdgs: c2w [4,4] / campos [3] must be contiguous float32 CUDA tensors");
+    TORCH_CHECK(c2w.device() == env_map.device() && campos.device() == env_map.device(), "fdgs: sky inputs on different devices");
+    fdgs_sky_args a;
+    memset(&a, 0, sizeof(a));
+    a.env_map = env_map.data_ptr<float>(); a.env_height = (int)env_map.size(1); a.env_width = (int)env_map.size(2);
+    a.c2w = c2w.data_ptr<float>(); a.campos = campos.data_ptr<float>();
+    a.fl_x = (float)fl_x; a.fl_y = (float)fl_y; a.cx = (float)cx; a.cy = (float)cy; a.radius = (float)radius;
+    a.width = (int)W; a.height = (int)H;
+    return a;
+}
+
+// (sky [3,H,W], miss flag int32 [1]: 1 if a ray missed the sphere)
+std::tuple<torch::Tensor, torch::Tensor> SkyForward(const torch::Tensor& env_map, const torch::Tensor& c2w, const torch::Tensor& campos,
+                                                    const double fl_x, const double fl_y, const double cx, const double cy,
+                                                    const double radius, const int64_t H, const int64_t W) {
+    const fdgs_sky_args a = sky_args(env_map, c2w, campos, fl_x, fl_y, cx, cy, radius, H, W);
+    const c10::cuda::CUDAGuard guard(env_map.device());
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    torch::Tensor sky = torch::empty({3, H, W}, env_map.options());
+    torch::Tensor miss = torch::zeros({1}, env_map.options().dtype(torch::kInt32));
+    check(fdgs_sky_forward(&a, sky.data_ptr<float>(), miss.data_ptr<int>(), (void*)stream), "sky_forward");
+    return std::make_tuple(sky, miss);
+}
+
+// dL/d env_map [3,Hm,Wm] of dL_dsky [3,H,W]
+torch::Tensor SkyBackward(const torch::Tensor& env_map, const torch::Tensor& c2w, const torch::Tensor& campos, const double fl_x,
+                          const double fl_y, const double cx, const double cy, const double radius,
+                          const torch::Tensor& dL_dsky) {
+    TORCH_CHECK(dL_dsky.is_cuda() && dL_dsky.scalar_type() == torch::kFloat32 && dL_dsky.dim() == 3 && dL_dsky.size(0) == 3,
+                "fdgs: dL_dsky must be a float32 CUDA tensor [3,H,W]");
+    const fdgs_sky_args a = sky_args(env_map, c2w, campos, fl_x, fl_y, cx, cy, radius, dL_dsky.size(1), dL_dsky.size(2));
+    const c10::cuda::CUDAGuard guard(env_map.device());
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    const auto g = dL_dsky.contiguous();
+    torch::Tensor denv = torch::zeros_like(env_map);
+    check(fdgs_sky_backward(&a, g.data_ptr<float>(), denv.data_ptr<float>(), (void*)stream), "sky_backward");
+    return denv;
 }
 
 // rebuild + sum the dL_dsh rows of all views from the gathered colour factors (include/fdgs.h: fdgs_sh_outer_sum)
@@ -603,6 +696,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("rasterize_gaussians_backward_factors", &RasterizeGaussiansBackwardFactors);
     m.def("rasterize_gaussians_raw", &RasterizeGaussiansRaw);
     m.def("rasterize_gaussians_backward_raw", &RasterizeGaussiansBackwardRaw);
+    m.def("rasterize_gaussians_bg", &RasterizeGaussiansBg);
+    m.def("rasterize_gaussians_backward_bg", &RasterizeGaussiansBackwardBg);
+    m.def("rasterize_gaussians_raw_bg", &RasterizeGaussiansRawBg);
+    m.def("rasterize_gaussians_backward_raw_bg", &RasterizeGaussiansBackwardRawBg);
+    m.def("sky_forward", &SkyForward);
+    m.def("sky_backward", &SkyBackward);
     m.def("sh_outer_sum", &ShOuterSum);
     m.def("check_rows_zero", &CheckRowsZero);
     m.def("union_maps", &UnionMaps);

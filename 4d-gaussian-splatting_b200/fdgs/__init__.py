@@ -25,6 +25,7 @@ ABI_SYMBOLS = (
     "fdgs_profile_enable", "fdgs_profile_read", "fdgs_launch_count", "fdgs_pack_rows", "fdgs_unpack_rows",
     "fdgs_sh_outer_sum", "fdgs_check_rows_zero", "fdgs_l1_ssim_forward", "fdgs_l1_ssim_backward", "fdgs_adam_step",
     "fdgs_knn_scratch_bytes", "fdgs_knn", "fdgs_debug_activate", "fdgs_union_maps", "fdgs_set_tile_cull", "fdgs_view_stats",
+    "fdgs_forward_bg", "fdgs_backward_bg", "fdgs_sky_forward", "fdgs_sky_backward",
 )
 
 STAGE_NAMES = ("preprocess_fwd", "bin_count_scan", "bin_scatter", "tile_sort_pack", "reserved", "blend_fwd", "blend_bwd",

@@ -23,6 +23,8 @@ every rank renders its own views, then `ViewParallelStep.finish()` leaves in eve
                    explicit round-to-nearest multiply-then-add -- bit-identical to accumulating the views'
                    dL_dsh tensors one after the other, and identical on every rank.  The dense 1.15 GB dL_dsh
                    tensor of a view is never materialised.
+  dense params     parameters that are not per-Gaussian rows (an environment map): their .grad are concatenated into
+                   one flat buffer and summed with ONE SUM all-reduce, launched beside the geometry all-reduce.
 
 A single-view render never communicates.  `.grad` of the parameters must be None or zero when a step starts
 (the sparse exchange and the reference's semantics both assume it); gradients that are NOT produced by the
@@ -284,7 +286,9 @@ class ViewParallelStep:
 
     # ---- the exchange -----------------------------------------------------------------------------
     def finish(self, geometry_params: Sequence[torch.Tensor], sh_params: Sequence[torch.Tensor] = (),
-               views_per_rank: Optional[int] = None) -> ViewBatchStats:
+               views_per_rank: Optional[int] = None, dense_params: Sequence[torch.Tensor] = ()) -> ViewBatchStats:
+        """`dense_params`: parameters with no per-Gaussian rows (e.g. the environment map); their gradients are summed
+        over the ranks whole, outside the union / row-guard logic of the geometry bucket."""
         group, world, P = self.group, _world(self.group), self.P
         st = self.stats
         self._marks = []
@@ -395,6 +399,13 @@ class ViewParallelStep:
                 gather_work = None
         elif want_sh:
             table = local
+        dense_flat = dense_work = None
+        if world > 1 and len(dense_params) > 0:
+            for p in dense_params:
+                if p.grad is None:
+                    p.grad = torch.zeros_like(p)
+            dense_flat = torch.cat([p.grad.reshape(-1) for p in dense_params])
+            dense_work = dist.all_reduce(dense_flat, op=dist.ReduceOp.SUM, group=group, async_op=True)
         if world > 1:
             if flat is not None:
                 geo_works = [dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=group, async_op=True)]
@@ -424,6 +435,14 @@ class ViewParallelStep:
         if flat is not None:
             _unpack(flat, bucket, idx)
             self._mark("geometry_unpack")
+        if dense_work is not None:
+            dense_work.wait()
+            off = 0
+            for p in dense_params:
+                n = p.grad.numel()
+                p.grad.copy_(dense_flat[off:off + n].view_as(p.grad))
+                off += n
+            self._mark("dense_allreduce")
         self.views = []
         self._early, self._fwd_radii, self._fwd_count = None, None, 0
         if world > 1:
@@ -472,7 +491,7 @@ class ViewParallelStep:
 
 
 def render_view_batch(render_fn, views: Iterable, params: Dict[str, torch.Tensor], loss_fn, global_batch: int,
-                      group=None, sh_keys: Sequence[str] = ()) -> Dict[str, object]:
+                      group=None, sh_keys: Sequence[str] = (), dense_keys: Sequence[str] = ()) -> Dict[str, object]:
     """One optimisation step's worth of rendering, data-parallel over views.
 
     render_fn(view) -> the dict render() returns; loss_fn(pkg, view) -> scalar loss of that view.
@@ -480,8 +499,9 @@ def render_view_batch(render_fn, views: Iterable, params: Dict[str, torch.Tensor
     holds, in .grad, the batch gradient (sum over all ranks' views of d(loss/global_batch)), exactly
     what the reference's sequential loop leaves there, and the returned stats are the merged
     densification statistics.  `sh_keys` names the entries of `params` that form the rasterizer's SH input
-    (exchanged as colour factors, see ViewParallelStep); everything else goes through the geometry bucket."""
-    first = next(iter(params.values()))
+    (exchanged as colour factors, see ViewParallelStep); `dense_keys` the entries that are not per-Gaussian (e.g.
+    "env_map"), summed whole; everything else goes through the geometry bucket."""
+    first = next(p for k, p in params.items() if k not in dense_keys)
     step = ViewParallelStep(first.shape[0], first.device, group=group, sh_factors=len(sh_keys) > 0)
     total = torch.zeros((), device=first.device)
     with step:
@@ -491,8 +511,8 @@ def render_view_batch(render_fn, views: Iterable, params: Dict[str, torch.Tensor
             loss.backward()
             total += loss.detach()
             step.add_view_stats(pkg["viewspace_points"].grad, pkg["radii"])
-    geometry = [p for k, p in params.items() if k not in sh_keys]
-    stats = step.finish(geometry, [params[k] for k in sh_keys])
+    geometry = [p for k, p in params.items() if k not in sh_keys and k not in dense_keys]
+    stats = step.finish(geometry, [params[k] for k in sh_keys], dense_params=[params[k] for k in dense_keys])
     if _world(group) > 1:
         dist.all_reduce(total, op=dist.ReduceOp.SUM, group=group)
     return {"loss": total, "stats": stats, "exchange": step.info}

@@ -17,6 +17,7 @@ from torch.nn import functional as F
 
 from .diff_gaussian_rasterization import GaussianRasterizationSettings, GaussianRasterizer
 from . import pyprep
+from fdgs.sky import sample_sky
 
 __all__ = ["render", "GaussianRasterizationSettings", "GaussianRasterizer"]
 
@@ -45,24 +46,6 @@ def _fused_prologue_ok(pc, pipe, override_color):
     return (getattr(pc, "scaling_activation", None) is torch.exp and getattr(pc, "opacity_activation", None) is torch.sigmoid
             and getattr(pc, "rotation_activation", None) is F.normalize
             and pc._features_dc.dim() == 3 and pc._features_dc.shape[1] == 1)
-
-
-def _add_sky(rendered_image, alpha, viewpoint_camera, pc):
-    """sky sphere of radius 60 sampled from the model's environment map (reference: :165-178)"""
-    assert pc.env_map is not None
-    R = 60
-    rays_o, rays_d = viewpoint_camera.get_rays()
-    od = (rays_o * rays_d).sum(-1)
-    dd = (rays_d ** 2).sum(-1)
-    delta = od ** 2 - dd * ((rays_o ** 2).sum(-1) - R ** 2)
-    assert (delta > 0).all()
-    t_inter = -od + torch.sqrt(delta) / dd
-    hit = rays_o + rays_d * t_inter.unsqueeze(-1)
-    tu = torch.atan2(hit[..., 1:2], hit[..., 0:1]) / (2 * torch.pi) + 0.5
-    tv = torch.acos(hit[..., 2:3] / R) / torch.pi
-    texcoord = torch.cat([tu, tv], dim=-1) * 2 - 1
-    sky = F.grid_sample(pc.env_map[None], texcoord[None])[0]
-    return rendered_image + (1 - alpha) * sky
 
 
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None):
@@ -104,6 +87,13 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
     )
     rasterizer = GaussianRasterizer(raster_settings=settings)
 
+    # environment-map sky (reference: :165-178): sampled by its own kernel, composed as `rendered + (1 - alpha) * sky`
+    # inside the rasterizer; a ray that misses the sphere is reported once the rasterizer's forward has synchronised
+    sky = sky_miss = None
+    if env_map_res:
+        assert pc.env_map is not None
+        sky, sky_miss = sample_sky(pc.env_map, viewpoint_camera)
+
     if _fused_prologue_ok(pc, pipe, override_color):
         # raw-parameter entry: no activation kernels, no SH concatenation (reference: :83-91,113-119 and the getters of
         # scene/gaussian_model.py:179-219)
@@ -113,10 +103,9 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
             features_rest=pc._features_rest if pc._features_rest.numel() else None, log_scales=pc._scaling,
             rotations_raw=pc._rotation, flow_2d=torch.zeros_like(xyz[:, :2]), ts=pc._t if four_d else None,
             log_scales_t=pc._scaling_t if four_d else None, rotations_r_raw=pc._rotation_r if pc.rot_4d else None,
-            prefilter_var=pc.prefilter_var if (four_d and pc.prefilter_var > 0.0) else -1.0)
-        assert not env_map_res or pc.env_map is not None
-        if env_map_res:
-            rendered_image = _add_sky(rendered_image, alpha, viewpoint_camera, pc)
+            prefilter_var=pc.prefilter_var if (four_d and pc.prefilter_var > 0.0) else -1.0, bg_image=sky)
+        if sky_miss is not None:
+            sky_miss.check()
         return {"render": rendered_image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0,
                 "radii": radii, "depth": depth, "alpha": alpha, "flow": flow}
 
@@ -186,10 +175,9 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
     rendered_image, radii, depth, alpha, flow, _covs = rasterizer(
         means3D=means3D, means2D=means2D, shs=shs, colors_precomp=colors_precomp, flow_2d=flow_2d,
         opacities=opacity, ts=ts, scales=scales, scales_t=scales_t, rotations=rotations,
-        rotations_r=rotations_r, cov3D_precomp=cov3D_precomp, prefilter_var=prefilter_var)
-
-    if env_map_res:
-        rendered_image = _add_sky(rendered_image, alpha, viewpoint_camera, pc)
+        rotations_r=rotations_r, cov3D_precomp=cov3D_precomp, prefilter_var=prefilter_var, bg_image=sky)
+    if sky_miss is not None:
+        sky_miss.check()
 
     if mask is not None:
         radii_all = radii.new_zeros(mask.shape)

@@ -45,6 +45,22 @@ def _invoke(fn, args, debug, dump_name):
         raise
 
 
+def _check_bg_image(bg_image, settings, means3D):
+    """A per-pixel background image must be a float32 [3, image_height, image_width] tensor on the device of the
+    Gaussians; None means the constant background `settings.bg` alone."""
+    if bg_image is None:
+        return
+    if not isinstance(bg_image, torch.Tensor):
+        raise TypeError("bg_image must be a torch.Tensor, got %s" % type(bg_image).__name__)
+    shape = (3, int(settings.image_height), int(settings.image_width))
+    if tuple(bg_image.shape) != shape:
+        raise ValueError("bg_image must have shape %s (3, image_height, image_width), got %s" % (shape, tuple(bg_image.shape)))
+    if bg_image.dtype != torch.float32:
+        raise ValueError("bg_image must be float32, got %s" % bg_image.dtype)
+    if bg_image.device != means3D.device:
+        raise ValueError("bg_image is on %s but the Gaussians are on %s" % (bg_image.device, means3D.device))
+
+
 def _notify_forward(radii):
     """View-parallel step (fdgs/dist.py): the radii of a view are known after its forward -- lets the step build the
     union of rendered Gaussians behind the backward pass."""
@@ -78,21 +94,26 @@ class GaussianRasterizationSettings(NamedTuple):
 
 class _RasterizeGaussians(torch.autograd.Function):
     """reference: :67-225.  Inputs, in order: means3D, means2D, sh, colors_precomp, flow_2d, opacities,
-    ts, scales, scales_t, rotations, rotations_r, cov3Ds_precomp, prefilter_var, raster_settings."""
+    ts, scales, scales_t, rotations, rotations_r, cov3Ds_precomp, prefilter_var, raster_settings, bg_image (a per-pixel
+    background [3,H,W] behind the Gaussians, or None)."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, flow_2d, opacities, ts, scales, scales_t,
-                rotations, rotations_r, cov3Ds_precomp, prefilter_var, raster_settings):
+                rotations, rotations_r, cov3Ds_precomp, prefilter_var, raster_settings, bg_image=None):
         s = raster_settings
         # positional layout of _C.rasterize_gaussians (reference: :88-119, rasterize_points.h:18-49)
         args = (s.bg, means3D, colors_precomp, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
                 s.scale_modifier, cov3Ds_precomp, prefilter_var, s.viewmatrix, s.projmatrix, s.tanfovx, s.tanfovy,
                 s.image_height, s.image_width, sh, s.sh_degree, s.sh_degree_t, s.campos, s.timestamp,
                 s.time_duration, s.rot_4d, s.gaussian_dim, s.force_sh_3d, s.prefiltered, s.debug)
-        (num_rendered, color, flow, depth, T, radii, geom_buf, binning_buf, img_buf, covs_com,
-         out_means3D) = _invoke(_C.rasterize_gaussians, args, s.debug, "snapshot_fw.dump")
+        if bg_image is None:
+            fw = _invoke(_C.rasterize_gaussians, args, s.debug, "snapshot_fw.dump")
+        else:
+            fw = _invoke(_C.rasterize_gaussians_bg, args + (bg_image,), s.debug, "snapshot_fw.dump")
+        (num_rendered, color, flow, depth, T, radii, geom_buf, binning_buf, img_buf, covs_com, out_means3D) = fw
 
         _notify_forward(radii)
+        ctx.bg_image = bg_image
         ctx.raster_settings = s
         ctx.num_rendered = num_rendered
         ctx.prefilter_var = prefilter_var
@@ -128,7 +149,20 @@ class _RasterizeGaussians(torch.autograd.Function):
         # the exchange.  No reference counterpart (its views are sequential on one GPU, train.py:104-166).
         from fdgs.dist import ViewParallelStep
         step = ViewParallelStep.current()
-        if step is not None and step.wants_factors(sh, cov3Ds_precomp) and ctx.needs_input_grad[2]:
+        factors = step is not None and step.wants_factors(sh, cov3Ds_precomp) and ctx.needs_input_grad[2]
+        g_bg = None
+        if ctx.bg_image is not None:
+            want_bg = ctx.needs_input_grad[14]
+            out = _invoke(_C.rasterize_gaussians_backward_bg, args + (ctx.bg_image, bool(factors), bool(want_bg)), s.debug,
+                          "snapshot_bw.dump")
+            (g_means2D, g_colors, g_opacities, g_means3D, g_cov3D, g_sh, g_flows, g_ts, g_scales, g_scales_t,
+             g_rot, g_rot_r, sh_factors, g_bg) = out
+            g_bg = g_bg if want_bg else None
+            if factors:
+                step.record_view(sh_factors, s, dict(means3D=means3D, ts=ts, scales=scales, scales_t=scales_t,
+                                                     rotations=rotations, rotations_r=rotations_r))
+                g_sh = None
+        elif factors:
             out = _invoke(_C.rasterize_gaussians_backward_factors, args, s.debug, "snapshot_bw.dump")
             (g_means2D, g_colors, g_opacities, g_means3D, g_cov3D, _no_sh, g_flows, g_ts, g_scales, g_scales_t,
              g_rot, g_rot_r, factors) = out
@@ -147,7 +181,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         return (g_means3D, g_means2D, for_input(g_sh, sh), for_input(g_colors, colors_precomp),
                 for_input(g_flows, flow_2d), g_opacities, for_input(g_ts, ts), for_input(g_scales, scales),
                 for_input(g_scales_t, scales_t), for_input(g_rot, rotations), for_input(g_rot_r, rotations_r),
-                for_input(g_cov3D, cov3Ds_precomp), None, None)
+                for_input(g_cov3D, cov3Ds_precomp), None, None, g_bg)
 
 
 class _RasterizeGaussiansRaw(torch.autograd.Function):
@@ -157,20 +191,24 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
     exp / F.normalize x2 / sigmoid kernels and the 1.15 GB torch.cat of the reference's getters
     (scene/gaussian_model.py:179-219), with their autograd mirror images, disappear from the frame.
     Inputs, in order: means3D, means2D, features_dc, features_rest, flow_2d, opacity_logits, ts, log_scales,
-    log_scales_t, rotations_raw, rotations_r_raw, prefilter_var, raster_settings."""
+    log_scales_t, rotations_raw, rotations_r_raw, prefilter_var, raster_settings, bg_image (or None)."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh_dc, sh_rest, flow_2d, opacities, ts, scales, scales_t, rotations,
-                rotations_r, prefilter_var, raster_settings):
+                rotations_r, prefilter_var, raster_settings, bg_image=None):
         s = raster_settings
         none = torch.Tensor([])
         args = (s.bg, means3D, none, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
                 s.scale_modifier, none, prefilter_var, s.viewmatrix, s.projmatrix, s.tanfovx, s.tanfovy,
                 s.image_height, s.image_width, sh_dc, s.sh_degree, s.sh_degree_t, s.campos, s.timestamp,
                 s.time_duration, s.rot_4d, s.gaussian_dim, s.force_sh_3d, s.prefiltered, s.debug, sh_rest, True)
-        (num_rendered, color, flow, depth, T, radii, geom_buf, binning_buf, img_buf, covs_com,
-         out_means3D) = _invoke(_C.rasterize_gaussians_raw, args, s.debug, "snapshot_fw.dump")
+        if bg_image is None:
+            fw = _invoke(_C.rasterize_gaussians_raw, args, s.debug, "snapshot_fw.dump")
+        else:
+            fw = _invoke(_C.rasterize_gaussians_raw_bg, args + (bg_image,), s.debug, "snapshot_fw.dump")
+        (num_rendered, color, flow, depth, T, radii, geom_buf, binning_buf, img_buf, covs_com, out_means3D) = fw
         _notify_forward(radii)
+        ctx.bg_image = bg_image
         ctx.raster_settings = s
         ctx.num_rendered = num_rendered
         ctx.prefilter_var = prefilter_var
@@ -201,8 +239,16 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
                 grad_depth, grad_alpha, grad_flow, sh_dc, s.sh_degree, s.sh_degree_t, s.campos, s.timestamp,
                 s.time_duration, s.rot_4d, s.gaussian_dim, s.force_sh_3d, geom_buf, ctx.num_rendered, binning_buf,
                 img_buf, s.debug, sh_rest, True, bool(factors))
+        g_bg = None
+        if ctx.bg_image is None:
+            out = _invoke(_C.rasterize_gaussians_backward_raw, args, s.debug, "snapshot_bw.dump")
+        else:
+            want_bg = ctx.needs_input_grad[13]
+            out = _invoke(_C.rasterize_gaussians_backward_raw_bg, args + (ctx.bg_image, bool(want_bg)), s.debug,
+                          "snapshot_bw.dump")
+            g_bg = out[14] if want_bg else None
         (g_means2D, g_colors, g_opacities, g_means3D, g_cov3D, g_sh, g_flows, g_ts, g_scales, g_scales_t, g_rot, g_rot_r,
-         sh_factors, g_sh_rest) = _invoke(_C.rasterize_gaussians_backward_raw, args, s.debug, "snapshot_bw.dump")
+         sh_factors, g_sh_rest) = out[:14]
         if factors:
             step.record_view(sh_factors, s, dict(means3D=means3D, ts=ts, scales=scales, scales_t=scales_t,
                                                  rotations=rotations, rotations_r=rotations_r, raw=True))
@@ -213,15 +259,18 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
 
         return (g_means3D, g_means2D, for_input(g_sh, sh_dc), for_input(g_sh_rest, sh_rest), for_input(g_flows, flow_2d),
                 g_opacities, for_input(g_ts, ts), for_input(g_scales, scales), for_input(g_scales_t, scales_t),
-                for_input(g_rot, rotations), for_input(g_rot_r, rotations_r), None, None)
+                for_input(g_rot, rotations), for_input(g_rot_r, rotations_r), None, None, g_bg)
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, flow_2d, opacities, ts, scales, scales_t,
-                        rotations, rotations_r, cov3Ds_precomp, prefilter_var, raster_settings):
-    """Functional entry point (reference: :34-65)."""
+                        rotations, rotations_r, cov3Ds_precomp, prefilter_var, raster_settings, bg_image=None):
+    """Functional entry point (reference: :34-65).  bg_image: optional per-pixel background [3,H,W] (float32, on the
+    Gaussians' device) behind the Gaussians; the image is then `rendered + (1 - alpha) * bg_image`, bit for bit, and
+    bg_image receives a gradient when it requires one."""
+    _check_bg_image(bg_image, raster_settings, means3D)
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, flow_2d, opacities, ts, scales,
                                      scales_t, rotations, rotations_r, cov3Ds_precomp, prefilter_var,
-                                     raster_settings)
+                                     raster_settings, bg_image)
 
 
 class GaussianRasterizer(nn.Module):
@@ -237,9 +286,10 @@ class GaussianRasterizer(nn.Module):
             return _C.mark_visible(positions, self.raster_settings.viewmatrix, self.raster_settings.projmatrix)
 
     def forward_raw(self, means3D, means2D, opacity_logits, features_dc, features_rest, log_scales, rotations_raw,
-                    flow_2d=None, ts=None, log_scales_t=None, rotations_r_raw=None, prefilter_var=-1.0):
+                    flow_2d=None, ts=None, log_scales_t=None, rotations_r_raw=None, prefilter_var=-1.0, bg_image=None):
         """Same 6-tuple as forward(), from the optimiser's RAW parameters (see _RasterizeGaussiansRaw): activations and
-        the SH concatenation happen inside the kernels, gradients arrive at the raw leaves directly."""
+        the SH concatenation happen inside the kernels, gradients arrive at the raw leaves directly.  bg_image: as in
+        rasterize_gaussians."""
         if self.raster_settings.rot_4d and (rotations_r_raw is None or log_scales_t is None or ts is None):
             raise Exception(
                 'Please provide exactly rotations_r and scales_t and ts if rot_4d and cov3D_precomp is None!')
@@ -247,13 +297,16 @@ class GaussianRasterizer(nn.Module):
         def opt(t):
             return torch.Tensor([]) if t is None else t
 
+        _check_bg_image(bg_image, self.raster_settings, means3D)
         return _RasterizeGaussiansRaw.apply(means3D, means2D, features_dc, opt(features_rest), opt(flow_2d), opacity_logits,
                                             opt(ts), log_scales, opt(log_scales_t), rotations_raw, opt(rotations_r_raw),
-                                            prefilter_var, self.raster_settings)
+                                            prefilter_var, self.raster_settings, bg_image)
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, flow_2d=None, ts=None,
                 scales=None, scales_t=None, rotations=None, rotations_r=None, cov3D_precomp=None,
-                prefilter_var=-1.0):
+                prefilter_var=-1.0, bg_image=None):
+        """The reference's 6-tuple (color, radii, depth, alpha, flow, covs_com).  bg_image: optional per-pixel
+        background behind the Gaussians (see rasterize_gaussians)."""
         # the three argument checks of the reference (:271-280), same messages
         if (shs is None) == (colors_precomp is None):
             raise Exception('Please provide excatly one of either SHs or precomputed colors!')
@@ -272,4 +325,4 @@ class GaussianRasterizer(nn.Module):
 
         return rasterize_gaussians(means3D, means2D, opt(shs), opt(colors_precomp), opt(flow_2d), opacities,
                                    opt(ts), opt(scales), opt(scales_t), opt(rotations), opt(rotations_r),
-                                   opt(cov3D_precomp), prefilter_var, self.raster_settings)
+                                   opt(cov3D_precomp), prefilter_var, self.raster_settings, bg_image)

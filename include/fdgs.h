@@ -210,6 +210,42 @@ int fdgs_forward(const fdgs_forward_args* args,
 /* Backward.  Fully asynchronous on `stream`. */
 int fdgs_backward(const fdgs_backward_args* args, void* stream);
 
+/* Per-pixel background image [3,H,W] (device, fp32) behind the Gaussians, e.g. an environment-map sky
+ * (fdgs_sky_forward).  The colour image becomes
+ *     out_color = (C + T * background) + (1 - (1 - T)) * bg_image
+ * rounded step by step, i.e. bit-identical to `rendered + (1 - alpha) * bg_image` evaluated in fp32 on the images
+ * fdgs_forward returns (alpha = 1 - T).  Every other output is unchanged.  bg_image == NULL: identical to
+ * fdgs_forward / fdgs_backward.  The backward takes the SAME bg_image as the forward; dL_dbg_image [3,H,W] (or
+ * NULL) is overwritten for every pixel with (1 - (1 - T)) * dL_dpix. */
+int fdgs_forward_bg(const fdgs_forward_args* args, const float* bg_image,
+                    fdgs_alloc_fn geom_alloc, void* geom_ctx,
+                    fdgs_alloc_fn binning_alloc, void* binning_ctx,
+                    fdgs_alloc_fn image_alloc, void* image_ctx,
+                    void* stream,
+                    fdgs_forward_result* result);
+int fdgs_backward_bg(const fdgs_backward_args* args, const float* bg_image, float* dL_dbg_image, void* stream);
+
+/* Environment-map sky sphere (the reference's sky for scenes with an environment map: gaussian_renderer/__init__.py
+ * and Camera.get_rays).  Each pixel's ray -- the pixel centre ((x + 0.5 - cx) / fl_x, (y + 0.5 - cy) / fl_y, 1, 1)
+ * through c2w, minus campos, normalised -- is intersected with the sphere |X| = radius; the hit point gives
+ * u = atan2(y, x) / 2pi + 0.5, v = acos(z / radius) / pi, and env_map is sampled bilinearly at (2u - 1, 2v - 1) like
+ * F.grid_sample with its defaults (align_corners = False, zero padding, u along the width). */
+typedef struct fdgs_sky_args {
+    const float* env_map;         /* [3,Hm,Wm]                                 */
+    int env_height, env_width;    /* Hm, Wm                                    */
+    const float* c2w;             /* [16] row-major camera-to-world, torch.linalg.inv(world_view_transform.T) */
+    const float* campos;          /* [3]  ray origin (camera centre)           */
+    float fl_x, fl_y, cx, cy;     /* pinhole intrinsics in pixels              */
+    float radius;                 /* sky sphere radius (60 in the reference)   */
+    int width, height;            /* image size W, H                           */
+} fdgs_sky_args;
+/* (The colatitude is evaluated as atan2(sqrt(x^2 + y^2), z), equal to acos(z / radius) on the sphere and accurate at
+ * the poles.)  out_sky [3,H,W] overwritten.  miss_flag (device int, or NULL) is set to 1 if any ray does not cross the sphere (the
+ * reference asserts on this); it is never cleared, so zero it before the call. */
+int fdgs_sky_forward(const fdgs_sky_args* args, float* out_sky, int* miss_flag, void* stream);
+/* dL_denv [3,Hm,Wm] += the share of dL_dsky [3,H,W] of every texel (accumulated: zero it for a fresh gradient). */
+int fdgs_sky_backward(const fdgs_sky_args* args, const float* dL_dsky, float* dL_denv, void* stream);
+
 /* present[i] = (view-space z of means3D[i] > 0.2)
  * (reference: rasterizer_impl.cu:54-67, auxiliary.h:140-163). */
 int fdgs_mark_visible(int P, const float* means3D, const float* viewmatrix,
