@@ -562,6 +562,95 @@ int fdgs_view_stats(long long P, const float* viewspace_grad, int grad_stride, c
     return FDGS_OK;
 }
 
+// ---- densification (densify.cu) -----------------------------------------------------------------------------------
+static int check_densify_args(const fdgs_densify_args* a) {
+    if (!a) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    if (a->P < 0 || a->P > 0x7fffffffLL || a->N < 1) return fail(FDGS_ERR_INVALID_ARG, "bad P / N");
+    if ((a->gaussian_dim != 3 && a->gaussian_dim != 4) || (a->rot_4d && a->gaussian_dim != 4))
+        return fail(FDGS_ERR_INVALID_ARG, "gaussian_dim must be 3 or 4 (4 with rot_4d)");
+    if (a->num_tensors < 0 || a->num_tensors > FDGS_DENSIFY_MAX_TENSORS) return fail(FDGS_ERR_INVALID_ARG, "bad tensor count");
+    if (a->P == 0) return FDGS_OK;
+    if (!a->scaling || !a->opacity) return fail(FDGS_ERR_INVALID_ARG, "null argument: scaling / opacity required");
+    if (!a->prune_only) {
+        if (!a->xyz_gradient_accum || !a->denom || !a->xyz || !a->rotation)
+            return fail(FDGS_ERR_INVALID_ARG, "null argument: densifying needs xyz_gradient_accum / denom / xyz / rotation");
+        if (a->gaussian_dim == 4 && (!a->t || !a->scaling_t))
+            return fail(FDGS_ERR_INVALID_ARG, "null argument: gaussian_dim 4 needs t / scaling_t");
+        if (a->rot_4d && !a->rotation_r) return fail(FDGS_ERR_INVALID_ARG, "null argument: rot_4d needs rotation_r");
+    } else if (a->use_max_screen_size && !a->max_radii2D) {
+        return fail(FDGS_ERR_INVALID_ARG, "null argument: max_screen_size needs max_radii2D");
+    }
+    for (int i = 0; i < a->num_tensors; ++i) {
+        const int k = a->kind[i], w = a->width[i];
+        if (!a->src[i] || !a->dst[i]) return fail(FDGS_ERR_INVALID_ARG, "null argument: tensor table entry");
+        if (k < FDGS_DENSIFY_COPY || k > FDGS_DENSIFY_SCALING_T) return fail(FDGS_ERR_INVALID_ARG, "bad tensor kind");
+        const int need = (k == FDGS_DENSIFY_XYZ || k == FDGS_DENSIFY_SCALING) ? 3 : (k == FDGS_DENSIFY_T || k == FDGS_DENSIFY_SCALING_T) ? 1 : 0;
+        if (w <= 0 || (need && w != need)) return fail(FDGS_ERR_INVALID_ARG, "tensor width does not match its kind");
+        if ((k == FDGS_DENSIFY_T || k == FDGS_DENSIFY_SCALING_T) && a->gaussian_dim != 4)
+            return fail(FDGS_ERR_INVALID_ARG, "t / scaling_t rows need gaussian_dim 4");
+    }
+    return FDGS_OK;
+}
+
+size_t fdgs_densify_scratch_bytes(long long P) { return fdgs::densify_scratch_bytes(P > 0 ? P : 0); }
+
+int fdgs_densify_plan(const fdgs_densify_args* a, char* scratch, int* totals, void* stream_v) {
+    g_last_error.clear();
+    const int rc = check_densify_args(a);
+    if (rc != FDGS_OK) return rc;
+    if (!totals || (a->P > 0 && !scratch)) return fail(FDGS_ERR_INVALID_ARG, "null argument: scratch / totals");
+    FDGS_CUDA(fdgs::launch_densify_plan(*a, scratch, totals, reinterpret_cast<cudaStream_t>(stream_v)), "densify_plan");
+    g_kernel_launches += a->P > 0 ? 4 : 0;
+    return FDGS_OK;
+}
+
+int fdgs_densify_apply(const fdgs_densify_args* a, const char* scratch, const int* totals, void* stream_v) {
+    g_last_error.clear();
+    const int rc = check_densify_args(a);
+    if (rc != FDGS_OK) return rc;
+    if (!totals || (a->P > 0 && !scratch)) return fail(FDGS_ERR_INVALID_ARG, "null argument: scratch / totals");
+    for (int i = 0; i < 4; ++i)
+        if (totals[i] < 0 || totals[i] > a->P) return fail(FDGS_ERR_INVALID_ARG, "totals inconsistent with P");
+    const long long S = totals[2], kept = totals[3];
+    if (kept > S || (a->prune_only && (totals[1] || S))) return fail(FDGS_ERR_INVALID_ARG, "totals inconsistent with the call");
+    if (S > 0 && (!a->samples || (a->gaussian_dim == 4 && !a->rot_4d && !a->samples_t)))
+        return fail(FDGS_ERR_INVALID_ARG, "null argument: split rows need samples (and samples_t)");
+    FDGS_CUDA(fdgs::launch_densify_apply(*a, scratch, S, kept, reinterpret_cast<cudaStream_t>(stream_v)), "densify_apply");
+    // the compaction, and the split-position kernel when children survive and xyz / t rows are in the table
+    bool positions = false;
+    for (int i = 0; i < a->num_tensors; ++i)
+        positions |= a->kind[i] == FDGS_DENSIFY_XYZ || a->kind[i] == FDGS_DENSIFY_T;
+    g_kernel_launches += (a->P > 0 && a->num_tensors > 0) ? 1 + (positions && kept > 0) : 0;
+    return FDGS_OK;
+}
+
+int fdgs_reset_opacity(long long P, float* opacity, float* exp_avg, float* exp_avg_sq, void* stream_v) {
+    g_last_error.clear();
+    if (P < 0) return fail(FDGS_ERR_INVALID_ARG, "bad P");
+    if (P == 0) return FDGS_OK;
+    if (!opacity) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    FDGS_CUDA(fdgs::launch_reset_opacity(P, opacity, exp_avg, exp_avg_sq, reinterpret_cast<cudaStream_t>(stream_v)), "reset_opacity");
+    g_kernel_launches += 1;
+    return FDGS_OK;
+}
+
+int fdgs_densify_stats(long long P, int batch_size, const float* point_grad, int point_grad_stride, const float* visibility_count,
+                       const int* radii, const float* t_grad, float* xyz_gradient_accum, float* denom, float* t_gradient_accum,
+                       float* max_radii2D, void* stream_v) {
+    g_last_error.clear();
+    if (P < 0 || batch_size < 1) return fail(FDGS_ERR_INVALID_ARG, "bad P / batch size");
+    if (batch_size == 1 ? point_grad_stride < 2 : point_grad_stride != 1) return fail(FDGS_ERR_INVALID_ARG, "bad gradient row stride");
+    if (P == 0) return FDGS_OK;
+    if (!point_grad || !radii || !xyz_gradient_accum || !denom || !max_radii2D || (batch_size > 1 && !visibility_count))
+        return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    if (!t_grad != !t_gradient_accum) return fail(FDGS_ERR_INVALID_ARG, "t_grad and t_gradient_accum go together");
+    FDGS_CUDA(fdgs::launch_densify_stats(P, batch_size, point_grad, point_grad_stride, visibility_count, radii, t_grad,
+                                         xyz_gradient_accum, denom, t_gradient_accum, max_radii2D,
+                                         reinterpret_cast<cudaStream_t>(stream_v)), "densify_stats");
+    g_kernel_launches += 1;
+    return FDGS_OK;
+}
+
 int fdgs_check_rows_zero(int n, const float* const* tensors, const int* widths, long long P, const int* radii, int* flag,
                          void* stream_v) {
     g_last_error.clear();

@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <atomic>
+#include "../../include/fdgs.h"
 #include "fdgs_common.cuh"
 
 namespace fdgs {
@@ -231,6 +232,17 @@ cudaError_t launch_knn_bruteforce(int n, int k, const float* xyz, int* idx, floa
 
 cudaError_t launch_mark_visible(int P, const float* means3D, const float* viewmatrix, unsigned char* present,
                                 cudaStream_t stream);
+
+// ---- densification surgery and statistics (densify.cu; the arguments are validated by fdgs_api.cu) ---------------
+size_t densify_scratch_bytes(long long P);
+cudaError_t launch_densify_plan(const fdgs_densify_args& a, char* scratch, int* totals, cudaStream_t stream);
+// S = rows selected for splitting, child_kept = children kept per copy (the host copy of the plan's totals)
+cudaError_t launch_densify_apply(const fdgs_densify_args& a, const char* scratch, long long S, long long child_kept,
+                                 cudaStream_t stream);
+cudaError_t launch_reset_opacity(long long P, float* opacity, float* m, float* v, cudaStream_t stream);
+cudaError_t launch_densify_stats(long long P, int B, const float* pgrad, int stride, const float* vis, const int* radii,
+                                 const float* tgrad, float* accum, float* denom, float* taccum, float* max_radii2D,
+                                 cudaStream_t stream);
 
 // ---- environment-map sky (sky.cu) ------------------------------------------------------------------
 struct SkyParams {

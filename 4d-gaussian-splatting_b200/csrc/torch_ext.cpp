@@ -652,6 +652,141 @@ void AdamStep(std::vector<torch::Tensor> params, std::vector<torch::Tensor> grad
           "adam_step");
 }
 
+// ---- densification (include/fdgs.h: fdgs_densify_*, fdgs_reset_opacity) --------------------------------------------
+// An undefined or empty tensor is "not provided" (NULL; the C-ABI rejects a NULL it needs).  dtype, layout and shape are checked before the device, so a
+// malformed argument is rejected before any GPU work.
+static float* rows_ptr(const torch::Tensor& t, long long P, long long width, const char* name) {
+    if (!t.defined() || t.numel() == 0) return nullptr;
+    TORCH_CHECK(t.scalar_type() == torch::kFloat32, "fdgs: ", name, " must be float32");
+    TORCH_CHECK(t.is_contiguous(), "fdgs: ", name, " must be contiguous");
+    TORCH_CHECK(t.dim() >= 1 && t.size(0) == P && (width < 0 || t.numel() == P * width), "fdgs: ", name, " has the wrong shape");
+    return t.data_ptr<float>();
+}
+
+// after every tensor of a call passed rows_ptr: all of them on the CUDA device of the first
+static void same_cuda_device(std::initializer_list<const torch::Tensor*> ts) {
+    const torch::Tensor* first = nullptr;
+    for (const torch::Tensor* t : ts) {
+        if (!t->defined() || t->numel() == 0) continue;
+        TORCH_CHECK(t->is_cuda(), "fdgs: densification tensors must be CUDA tensors");
+        if (!first) first = t;
+        TORCH_CHECK(t->device() == first->device(), "fdgs: densification tensors on different devices");
+    }
+}
+
+// geo = [xyz, t, scaling, scaling_t, rotation, rotation_r, opacity]; stats = [xyz_gradient_accum, denom, max_radii2D];
+// thresholds = [max_grad, min_opacity, percent_dense * extent, 0.1 * extent, max_screen_size] (rounded to fp32 here,
+// as ATen rounds a Python scalar it compares an fp32 tensor with); flags = [N, gaussian_dim, rot_4d, prune_only,
+// use_max_screen_size]
+static fdgs_densify_args densify_args(const std::vector<torch::Tensor>& geo, const std::vector<torch::Tensor>& stats,
+                                      const std::vector<double>& thr, const std::vector<int64_t>& flags) {
+    TORCH_CHECK(geo.size() == 7 && stats.size() == 3 && thr.size() == 5 && flags.size() == 5, "fdgs: densify argument lists");
+    fdgs_densify_args a;
+    memset(&a, 0, sizeof(a));
+    const long long P = geo[2].defined() ? geo[2].size(0) : 0;
+    a.P = P;
+    a.N = (int)flags[0]; a.gaussian_dim = (int)flags[1]; a.rot_4d = (int)flags[2]; a.prune_only = (int)flags[3];
+    a.use_max_screen_size = (int)flags[4];
+    a.max_grad = (float)thr[0]; a.min_opacity = (float)thr[1]; a.dense_extent = (float)thr[2]; a.big_extent = (float)thr[3];
+    a.max_screen_size = (float)thr[4];
+    a.xyz = rows_ptr(geo[0], P, 3, "xyz");
+    a.t = rows_ptr(geo[1], P, 1, "t");
+    a.scaling = rows_ptr(geo[2], P, 3, "scaling");
+    a.scaling_t = rows_ptr(geo[3], P, 1, "scaling_t");
+    a.rotation = rows_ptr(geo[4], P, 4, "rotation");
+    a.rotation_r = rows_ptr(geo[5], P, 4, "rotation_r");
+    a.opacity = rows_ptr(geo[6], P, 1, "opacity");
+    a.xyz_gradient_accum = rows_ptr(stats[0], P, 1, "xyz_gradient_accum");
+    a.denom = rows_ptr(stats[1], P, 1, "denom");
+    a.max_radii2D = rows_ptr(stats[2], P, 1, "max_radii2D");
+    same_cuda_device({&geo[0], &geo[1], &geo[2], &geo[3], &geo[4], &geo[5], &geo[6], &stats[0], &stats[1], &stats[2]});
+    return a;
+}
+
+std::tuple<torch::Tensor, torch::Tensor> DensifyPlan(const std::vector<torch::Tensor>& geo, const std::vector<torch::Tensor>& stats,
+                                                     const std::vector<double>& thr, const std::vector<int64_t>& flags) {
+    fdgs_densify_args a = densify_args(geo, stats, thr, flags);
+    TORCH_CHECK(geo[2].defined() && geo[2].is_cuda(), "fdgs: scaling must be a CUDA tensor");
+    const c10::cuda::CUDAGuard guard(geo[2].device());
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    auto opts = geo[2].options();
+    torch::Tensor scratch = torch::empty({(int64_t)fdgs_densify_scratch_bytes(a.P) + 16}, opts.dtype(torch::kByte));
+    torch::Tensor totals = torch::empty({4}, opts.dtype(torch::kInt32));
+    check(fdgs_densify_plan(&a, reinterpret_cast<char*>(scratch.data_ptr()), totals.data_ptr<int>(), (void*)stream), "densify_plan");
+    return std::make_tuple(scratch, totals);
+}
+
+// srcs / dsts / kinds: the compaction table (include/fdgs.h FDGS_DENSIFY_*); totals: the plan's totals on the host
+void DensifyApply(const std::vector<torch::Tensor>& geo, const std::vector<torch::Tensor>& stats, const std::vector<double>& thr,
+                  const std::vector<int64_t>& flags, const std::vector<torch::Tensor>& srcs, const std::vector<torch::Tensor>& dsts,
+                  const std::vector<int64_t>& kinds, const torch::Tensor& scratch, const std::vector<int64_t>& totals,
+                  const torch::Tensor& samples, const torch::Tensor& samples_t) {
+    fdgs_densify_args a = densify_args(geo, stats, thr, flags);
+    const size_t n = srcs.size();
+    TORCH_CHECK(n <= FDGS_DENSIFY_MAX_TENSORS && dsts.size() == n && kinds.size() == n && totals.size() == 4,
+                "fdgs: densify tensor table mismatch");
+    const long long P_new = totals[0] + totals[1] + (long long)a.N * totals[3];
+    a.num_tensors = (int)n;
+    for (size_t i = 0; i < n; ++i) {
+        const long long w = a.P > 0 ? srcs[i].numel() / a.P : 1;
+        a.src[i] = rows_ptr(srcs[i], a.P, w, "source row tensor");
+        a.dst[i] = rows_ptr(dsts[i], P_new, w, "destination row tensor");
+        if (a.P == 0 || P_new == 0) { a.num_tensors = 0; break; }     // nothing to copy from or to
+        TORCH_CHECK(a.src[i] && a.dst[i], "fdgs: densify tensor table entry missing");
+        a.kind[i] = (int)kinds[i];
+        a.width[i] = (int)w;
+    }
+    const long long SN = totals[2] * (long long)a.N;
+    a.samples = rows_ptr(samples, SN, a.rot_4d ? 4 : 3, "samples");
+    a.samples_t = rows_ptr(samples_t, SN, 1, "samples_t");
+    for (size_t i = 0; i < n; ++i) same_cuda_device({&geo[2], &srcs[i], &dsts[i]});
+    same_cuda_device({&geo[2], &samples, &samples_t});
+    TORCH_CHECK(scratch.is_cuda() && scratch.scalar_type() == torch::kByte &&
+                scratch.numel() >= (int64_t)fdgs_densify_scratch_bytes(a.P), "fdgs: densify scratch of the plan required");
+    int tot[4];
+    for (int i = 0; i < 4; ++i) tot[i] = (int)totals[i];
+    const c10::cuda::CUDAGuard guard(scratch.device());
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check(fdgs_densify_apply(&a, reinterpret_cast<const char*>(scratch.data_ptr()), tot, (void*)stream), "densify_apply");
+}
+
+void ResetOpacity(torch::Tensor& opacity, torch::Tensor& exp_avg, torch::Tensor& exp_avg_sq) {
+    const long long P = opacity.size(0);
+    float* o = rows_ptr(opacity, P, 1, "opacity");
+    float* m = rows_ptr(exp_avg, P, 1, "exp_avg");
+    float* v = rows_ptr(exp_avg_sq, P, 1, "exp_avg_sq");
+    same_cuda_device({&opacity, &exp_avg, &exp_avg_sq});
+    if (P == 0) return;
+    const c10::cuda::CUDAGuard guard(opacity.device());
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check(fdgs_reset_opacity(P, o, m, v, (void*)stream), "reset_opacity");
+}
+
+// batch_size 1: point_grad = viewspace_points.grad [P, >= 2], visibility_count empty; batch_size > 1: point_grad =
+// the summed norms [P] and visibility_count [P] (fdgs.dist.ViewBatchStats).  t_grad / t_gradient_accum empty for 3D.
+void DensifyStats(int64_t batch_size, const torch::Tensor& point_grad, const torch::Tensor& visibility_count,
+                  const torch::Tensor& radii, const torch::Tensor& t_grad, torch::Tensor& xyz_gradient_accum, torch::Tensor& denom,
+                  torch::Tensor& t_gradient_accum, torch::Tensor& max_radii2D) {
+    const long long P = xyz_gradient_accum.size(0);
+    float* acc = rows_ptr(xyz_gradient_accum, P, 1, "xyz_gradient_accum");
+    float* den = rows_ptr(denom, P, 1, "denom");
+    float* tacc = rows_ptr(t_gradient_accum, P, 1, "t_gradient_accum");
+    float* mr = rows_ptr(max_radii2D, P, 1, "max_radii2D");
+    const float* tg = rows_ptr(t_grad, P, 1, "t_grad");
+    const float* vis = rows_ptr(visibility_count, P, 1, "visibility_count");
+    const float* pg = rows_ptr(point_grad, P, batch_size == 1 ? -1 : 1, "point_grad");
+    TORCH_CHECK(point_grad.defined() && (batch_size > 1 || point_grad.dim() == 2), "fdgs: point_grad must be [P, >= 2] for one view");
+    TORCH_CHECK(radii.defined() && radii.scalar_type() == torch::kInt32 && radii.is_contiguous() && radii.numel() == P,
+                "fdgs: radii must be contiguous int32 [P]");
+    same_cuda_device({&xyz_gradient_accum, &denom, &t_gradient_accum, &max_radii2D, &t_grad, &visibility_count, &point_grad, &radii});
+    const int stride = batch_size == 1 ? (int)(point_grad.dim() == 2 ? point_grad.size(1) : 0) : 1;
+    if (P == 0) return;
+    const c10::cuda::CUDAGuard guard(xyz_gradient_accum.device());
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    check(fdgs_densify_stats(P, (int)batch_size, pg, stride, vis, radii.data_ptr<int>(), tg, acc, den, tacc, mr, (void*)stream),
+          "densify_stats");
+}
+
 // ---- k nearest neighbours (include/fdgs.h: fdgs_knn) ---------------------------------------------------------------
 std::tuple<torch::Tensor, torch::Tensor> Knn(const torch::Tensor& xyz, const int64_t k, const bool brute_force) {
     TORCH_CHECK(xyz.is_cuda() && xyz.scalar_type() == torch::kFloat32 && xyz.dim() == 2 && xyz.size(1) == 3,
@@ -689,6 +824,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("l1_ssim_backward", &L1SsimBackward);
     m.def("adam_step", &AdamStep);
     m.def("knn", &Knn);
+    m.def("densify_plan", &DensifyPlan);
+    m.def("densify_apply", &DensifyApply);
+    m.def("reset_opacity", &ResetOpacity);
+    m.def("densify_stats", &DensifyStats);
     m.def("pack_rows", &PackRows);
     m.def("unpack_rows", &UnpackRows);
     m.def("rasterize_gaussians", &RasterizeGaussiansCUDA);

@@ -26,6 +26,7 @@ ABI_SYMBOLS = (
     "fdgs_sh_outer_sum", "fdgs_check_rows_zero", "fdgs_l1_ssim_forward", "fdgs_l1_ssim_backward", "fdgs_adam_step",
     "fdgs_knn_scratch_bytes", "fdgs_knn", "fdgs_debug_activate", "fdgs_union_maps", "fdgs_set_tile_cull", "fdgs_view_stats",
     "fdgs_forward_bg", "fdgs_backward_bg", "fdgs_sky_forward", "fdgs_sky_backward",
+    "fdgs_densify_scratch_bytes", "fdgs_densify_plan", "fdgs_densify_apply", "fdgs_reset_opacity", "fdgs_densify_stats",
 )
 
 STAGE_NAMES = ("preprocess_fwd", "bin_count_scan", "bin_scatter", "tile_sort_pack", "reserved", "blend_fwd", "blend_bwd",
@@ -51,6 +52,7 @@ def lib():
         for n in ("fdgs_geom_bytes", "fdgs_image_bytes", "fdgs_binning_bytes"):
             getattr(_lib, n).restype = ctypes.c_size_t
         _lib.fdgs_launch_count.restype = ctypes.c_longlong
+        _lib.fdgs_densify_scratch_bytes.restype = ctypes.c_size_t
     return _lib
 
 

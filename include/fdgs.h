@@ -304,6 +304,88 @@ int fdgs_check_rows_zero(int n, const float* const* tensors, const int* widths, 
 int fdgs_view_stats(long long P, const float* viewspace_grad, int grad_stride, const int* radii, float* grad_norm_sum,
                     float* visibility_count, int* max_radii, void* stream);
 
+/* Densification statistics of one optimisation step (reference: train.py:168-183 and :233-237,
+ * scene/gaussian_model.py:579-589 add_densification_stats / _grad), one pass over the P Gaussians.
+ *   batch_size == 1: point_grad = the view's viewspace_points.grad [P, point_grad_stride >= 2], visibility_count NULL,
+ *                    radii = the view's radii; visible = radii > 0, g = ||point_grad[i, 0:2]||, tg = t_grad[i].
+ *   batch_size  > 1: point_grad = the views' summed gradient norms [P] (stride 1), visibility_count [P] and radii (the
+ *                    MAX over the views) as ViewBatchStats holds them; visible = visibility_count > 0,
+ *                    g = point_grad[i] * batch_size / visibility_count[i], tg = t_grad[i] * batch_size / visibility_count[i].
+ * For visible rows: xyz_gradient_accum += g, denom += 1, t_gradient_accum += tg, max_radii2D = max(max_radii2D, radii).
+ * t_grad / t_gradient_accum: [P] (the _t.grad column), both NULL for 3D Gaussians. */
+int fdgs_densify_stats(long long P, int batch_size, const float* point_grad, int point_grad_stride,
+                       const float* visibility_count, const int* radii, const float* t_grad, float* xyz_gradient_accum,
+                       float* denom, float* t_gradient_accum, float* max_radii2D, void* stream);
+
+/* Densify and prune (reference: scene/gaussian_model.py:486-577 densify_and_prune with densify_and_clone,
+ * densify_and_split and prune_points) as one compaction of every parameter row and Adam-moment row into new tensors.
+ * The result rows are, in this order and each part in source order without its pruned rows: the original rows that
+ * were neither split nor pruned; the clones; copy 1 of every split row; copy 2; ... copy N.
+ *   grads = xyz_gradient_accum / denom (NaN -> 0); smax = max(exp(scaling[i, :]))
+ *   clone : |grads| >= max_grad and smax <= dense_extent            (dense_extent = fp32(percent_dense * extent))
+ *   split : grads >= max_grad and smax > dense_extent
+ *   prune : sigmoid(opacity) < min_opacity, or with use_max_screen_size
+ *           max_radii2D > max_screen_size or smax > big_extent   (big_extent = fp32(0.1 * extent)), tested on every
+ *           output row with its own values; a densifying call has already zeroed max_radii2D, so only prune_only
+ *           calls read it.
+ * Split children: scaling(_t) = log(exp(scaling(_t)) * fp32(1 / fp32(0.8 N))), position = R sample + mean where
+ * sample = samples row * exp(scaling) (rot_4d: 4-vector over [scaling, scaling_t] rotated by the 4D rotation of
+ * (rotation, rotation_r), giving xyz and t; otherwise R = rotation matrix of `rotation` and t = t + samples_t row *
+ * exp(scaling_t)).  Sample rows are [k * S + j] for copy k of the j-th selected row (S = split rows selected), as
+ * torch.normal over the reference's repeat(N, 1) tiles draws them; positions are evaluated in double and rounded once.
+ * The tensor table lists every row tensor to compact: src [P, width], dst [P_new, width] (caller-allocated):
+ *   COPY       every output row copies its source row (features, opacity, rotations)
+ *   MOMENT     original rows copy, clones and split children are zero (Adam moments; statistics of prune_only)
+ *   XYZ/T/SCALING/SCALING_T  the parameters split children compute (widths 3 / 1 / 3 / 1). */
+#define FDGS_DENSIFY_MAX_TENSORS 32
+#define FDGS_DENSIFY_COPY 0
+#define FDGS_DENSIFY_MOMENT 1
+#define FDGS_DENSIFY_XYZ 2
+#define FDGS_DENSIFY_T 3
+#define FDGS_DENSIFY_SCALING 4
+#define FDGS_DENSIFY_SCALING_T 5
+typedef struct fdgs_densify_args {
+    long long P;                  /* rows before the call                      */
+    int N;                        /* children per split row (reference: 2)     */
+    int gaussian_dim;             /* 3 or 4                                    */
+    int rot_4d;
+    int prune_only;
+    int use_max_screen_size;      /* max_screen_size given (truthy)            */
+    float max_grad;
+    float min_opacity;
+    float dense_extent;
+    float big_extent;
+    float max_screen_size;
+    const float* xyz_gradient_accum;  /* [P]  (densifying calls)               */
+    const float* denom;               /* [P]  (densifying calls)               */
+    const float* max_radii2D;         /* [P]  (prune_only with use_max_screen_size) */
+    const float* xyz;                 /* [P,3]                                 */
+    const float* t;                   /* [P]   gaussian_dim 4                  */
+    const float* scaling;             /* [P,3] log-scales                      */
+    const float* scaling_t;           /* [P]   gaussian_dim 4                  */
+    const float* rotation;            /* [P,4]                                 */
+    const float* rotation_r;          /* [P,4] rot_4d                          */
+    const float* opacity;             /* [P]   logits                          */
+    const float* samples;             /* [S*N, 3] (rot_4d: [S*N, 4]) standard normal draws */
+    const float* samples_t;           /* [S*N]  gaussian_dim 4 without rot_4d  */
+    int num_tensors;
+    int kind[FDGS_DENSIFY_MAX_TENSORS];
+    int width[FDGS_DENSIFY_MAX_TENSORS];
+    const float* src[FDGS_DENSIFY_MAX_TENSORS];
+    float* dst[FDGS_DENSIFY_MAX_TENSORS];
+} fdgs_densify_args;
+/* Bytes of device scratch fdgs_densify_plan needs for P rows; hand the same buffer to fdgs_densify_apply. */
+size_t fdgs_densify_scratch_bytes(long long P);
+/* Decides every row's fate and each output row's index.  totals (device int[4]) receives: original rows kept, clones
+ * kept, rows selected for splitting (S), children kept per copy; P_new = totals[0] + totals[1] + N * totals[3].
+ * Asynchronous: the caller copies totals to the host once to size the outputs and the samples. */
+int fdgs_densify_plan(const fdgs_densify_args* args, char* scratch, int* totals, void* stream);
+/* Writes every dst tensor; totals = the HOST copy of fdgs_densify_plan's totals.  Fully asynchronous. */
+int fdgs_densify_apply(const fdgs_densify_args* args, const char* scratch, const int* totals, void* stream);
+/* Reset opacity in place (reference: scene/gaussian_model.py:371-374): opacity = log(x / (1 - x)) with
+ * x = min(sigmoid(opacity), 0.01); exp_avg and exp_avg_sq (or NULL) of those rows are zeroed. */
+int fdgs_reset_opacity(long long P, float* opacity, float* exp_avg, float* exp_avg_sq, void* stream);
+
 /* ---- the callers either side of the rasterizer in a training step (SURVEY.md section 8(f)) ---------------------- */
 
 /* Fused photometric loss (reference: utils/loss_utils.py:18-64 l1_loss + ssim, combined as train.py:115-117):
