@@ -722,6 +722,71 @@ int fdgs_knn(int n, int k, const float* xyz, char* scratch, int* idx, float* dis
     return FDGS_OK;
 }
 
+// ---- rigidity and motion regularisers (regularize.cu) ----------------------------------------------------------------
+static int check_rigid_size(int n, int k) {
+    if (n <= 0 || k < 1 || k > 32) return fail(FDGS_ERR_INVALID_ARG, "bad n / k (n > 0, 1 <= k <= 32)");
+    if ((long long)n * k > 0x7fffffffLL) return fail(FDGS_ERR_INVALID_ARG, "n * k exceeds 2^31 - 1 edges");
+    return FDGS_OK;
+}
+
+static int check_rigid_args(const fdgs_rigid_args* a, bool rigid, bool transpose) {
+    if (!a) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    if (int rc = check_rigid_size(a->n, a->k)) return rc;
+    if (!a->t || !a->scaling || !a->scaling_t || !a->rotation || !a->rotation_r)
+        return fail(FDGS_ERR_INVALID_ARG, "null argument: t / scaling / scaling_t / rotation / rotation_r required");
+    if (rigid && (!a->idx || !a->weight)) return fail(FDGS_ERR_INVALID_ARG, "null argument: the rigidity loss needs idx / weight");
+    if (transpose && (!a->in_offsets || !a->in_edges))
+        return fail(FDGS_ERR_INVALID_ARG, "null argument: the rigidity backward needs in_offsets / in_edges");
+    return FDGS_OK;
+}
+
+static fdgs::RigidParams rigid_params(const fdgs_rigid_args* a) {
+    fdgs::RigidParams p;
+    p.n = a->n; p.k = a->k; p.t = a->t; p.scaling = a->scaling; p.scaling_t = a->scaling_t;
+    p.rotation = a->rotation; p.rotation_r = a->rotation_r; p.idx = a->idx; p.weight = a->weight;
+    p.in_offsets = a->in_offsets; p.in_edges = a->in_edges; p.velocity = a->velocity;
+    return p;
+}
+
+size_t fdgs_rigid_scratch_bytes(int n, int k) {
+    return (n > 0 && k >= 1 && k <= 32 && (long long)n * k <= 0x7fffffffLL) ? fdgs::rigid_scratch_bytes(n, k) : 0;
+}
+
+int fdgs_rigid_neighbours(int n, int k, const int* idx, const float* dist2, char* scratch, float* weight, int* in_offsets,
+                          int* in_edges, void* stream_v) {
+    g_last_error.clear();
+    if (int rc = check_rigid_size(n, k)) return rc;
+    if (!idx || !dist2 || !scratch || !weight || !in_offsets || !in_edges) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    FDGS_CUDA(fdgs::launch_rigid_neighbours(n, k, idx, dist2, scratch, weight, in_offsets, in_edges,
+                                            reinterpret_cast<cudaStream_t>(stream_v)), "rigid_neighbours");
+    g_kernel_launches += 2;     // + the radix sort's own kernels
+    return FDGS_OK;
+}
+
+int fdgs_rigid_forward(const fdgs_rigid_args* a, char* scratch, float* loss_rigid, float* loss_motion, void* stream_v) {
+    g_last_error.clear();
+    if (int rc = check_rigid_args(a, loss_rigid != nullptr, false)) return rc;
+    if (!a->velocity) return fail(FDGS_ERR_INVALID_ARG, "null argument: velocity");
+    if ((loss_rigid || loss_motion) && !scratch) return fail(FDGS_ERR_INVALID_ARG, "null argument: scratch");
+    FDGS_CUDA(fdgs::launch_rigid_forward(rigid_params(a), scratch, loss_rigid, loss_motion, reinterpret_cast<cudaStream_t>(stream_v)),
+              "rigid_forward");
+    g_kernel_launches += (loss_rigid || loss_motion) ? 3 : 1;
+    return FDGS_OK;
+}
+
+int fdgs_rigid_backward(const fdgs_rigid_args* a, const float* grad_rigid, const float* grad_motion, float* dL_dscaling,
+                        float* dL_dscaling_t, float* dL_drotation, float* dL_drotation_r, void* stream_v) {
+    g_last_error.clear();
+    if (int rc = check_rigid_args(a, grad_rigid != nullptr, grad_rigid != nullptr)) return rc;
+    if (!a->velocity) return fail(FDGS_ERR_INVALID_ARG, "null argument: the forward's velocity is required");
+    if (!dL_dscaling || !dL_dscaling_t || !dL_drotation || !dL_drotation_r) return fail(FDGS_ERR_INVALID_ARG, "null argument: gradient outputs");
+    FDGS_CUDA(fdgs::launch_rigid_backward(rigid_params(a), grad_rigid, grad_motion, dL_dscaling, dL_dscaling_t, dL_drotation,
+                                          dL_drotation_r, reinterpret_cast<cudaStream_t>(stream_v)),
+              "rigid_backward");
+    g_kernel_launches += 1;
+    return FDGS_OK;
+}
+
 int fdgs_debug_activate(int n, const float* log_s, const float* logit, const float* quat, int mode, float* s_out, float* o_out,
                         float* q_out, void* stream_v) {
     g_last_error.clear();

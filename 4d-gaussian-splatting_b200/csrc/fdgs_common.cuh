@@ -151,6 +151,68 @@ __device__ __forceinline__ void sigma_from_M(Sigma4& S) {
     S.s33 = col_dot4(S.M[3], S.M[3]);
 }
 
+// 4x4 helper, glm convention: A[c][r], (A*B)[c][r] = sum_k A[k][r] * B[c][k]
+template <typename T>
+__device__ __forceinline__ void mat4_mul(const T A[4][4], const T B[4][4], T C[4][4]) {
+#pragma unroll
+    for (int c = 0; c < 4; ++c)
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+            C[c][r] = A[0][r] * B[c][0] + A[1][r] * B[c][1] + A[2][r] * B[c][2] + A[3][r] * B[c][3];
+}
+
+// Backward of the 4D covariance Sigma = M^T M (build_M4 + sigma_from_M), reference: backward.cu:784-834.  Gradient in
+// the rasterizer's convention -- every symmetric pair is one variable: d[6] = dL/d(Sigma_xyz upper triangle, as
+// dL_dcov3D), dc12[3] = dL/d(Sigma[0..2][3]), dcovt = dL/d(Sigma[3][3]).  M, R = build_M4's matrices, sc = the scales
+// it was given, rot / rot_r = the normalised quaternions.  Out: gs = dL/d(sc), g_rot / g_rotr = dL/d(rot / rot_r).
+// Shared by geom_bwd_kernel (preprocess_bwd.cu, T = float, Q = float4) and the rigidity backward (regularize.cu, in
+// double: T = double, Q = double4).
+template <typename T, typename Q>
+__device__ __forceinline__ void cov4_bwd(const T d[6], const T dc12[3], T dcovt, const T M[4][4], const T R4[4][4],
+                                         const T sc[4], const Q rot, const Q rotr, T gs[4], T g_rot[4], T g_rotr[4]) {
+    T dS[4][4];
+    dS[0][0] = d[0]; dS[1][1] = d[3]; dS[2][2] = d[5]; dS[3][3] = dcovt;
+    dS[0][1] = dS[1][0] = 0.5f * d[1];
+    dS[0][2] = dS[2][0] = 0.5f * d[2];
+    dS[1][2] = dS[2][1] = 0.5f * d[4];
+    dS[0][3] = dS[3][0] = 0.5f * dc12[0];
+    dS[1][3] = dS[3][1] = 0.5f * dc12[1];
+    dS[2][3] = dS[3][2] = 0.5f * dc12[2];
+    T M2[4][4], dM[4][4];
+#pragma unroll
+    for (int c = 0; c < 4; ++c)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) M2[c][r] = 2.0f * M[c][r];
+    mat4_mul(M2, dS, dM);   // dL_dM = 2 * M * dL_dSigma
+    // dL_dscale_i = sum_c R[c][i] * dL_dM[c][i]
+    T N[4][4];   // N[i][j] = s_i * dL_dM[j][i]   (= scaled dL_dMt)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        T acc = 0.f;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            acc += R4[c][i] * dM[c][i];
+            N[i][c] = sc[i] * dM[c][i];
+        }
+        gs[i] = acc;
+    }
+    const T qa = rot.x, qb = rot.y, qc = rot.z, qd = rot.w;
+    const T qp = rotr.x, qq = rotr.y, qr = rotr.z, qs = rotr.w;
+    const T Ml[4][4] = {{qa, qb, -qc, qd}, {-qb, qa, qd, qc}, {qc, -qd, qa, qb}, {-qd, -qc, -qb, qa}};
+    const T Mr[4][4] = {{qp, qq, -qr, -qs}, {-qq, qp, qs, -qr}, {qr, -qs, qp, -qq}, {qs, qr, qq, qp}};
+    T X[4][4], Y[4][4];
+    mat4_mul(N, Mr, X);    // dL_dml_t = dL_dMt * M_r
+    mat4_mul(Ml, N, Y);    // dL_dmr_t = M_l * dL_dMt
+    g_rot[0] = X[0][0] + X[1][1] + X[2][2] + X[3][3];
+    g_rot[1] = -X[0][1] + X[1][0] - X[2][3] + X[3][2];
+    g_rot[2] = X[0][2] - X[1][3] - X[2][0] + X[3][1];
+    g_rot[3] = -X[0][3] - X[1][2] + X[2][1] + X[3][0];
+    g_rotr[0] = Y[0][0] + Y[1][1] + Y[2][2] + Y[3][3];
+    g_rotr[1] = -Y[0][1] + Y[1][0] + Y[2][3] - Y[3][2];
+    g_rotr[2] = Y[0][2] + Y[1][3] - Y[2][0] - Y[3][1];
+    g_rotr[3] = Y[0][3] - Y[1][2] + Y[2][1] - Y[3][0];
+}
+
 // marginal_t = __expf(-0.5*dt*dt / cov_t')   reference: forward.cu:333 (double-promoted argument)
 __device__ __forceinline__ float marginal_from(float dt, float cov_t, float prefilter_var) {
     const float den = (prefilter_var > 0.0f) ? fadd(prefilter_var, cov_t) : cov_t;

@@ -230,6 +230,27 @@ size_t knn_scratch_bytes(int n);
 cudaError_t launch_knn(int n, int k, const float* xyz, char* scratch, int* idx, float* dist2, cudaStream_t stream);
 cudaError_t launch_knn_bruteforce(int n, int k, const float* xyz, int* idx, float* dist2, cudaStream_t stream);
 
+// rigidity and motion regularisers (regularize.cu; the arguments are validated by fdgs_api.cu)
+struct RigidParams {
+    int n, k;
+    const float* t;           // [n]
+    const float* scaling;     // [n,3] log-scales
+    const float* scaling_t;   // [n]   log-scale
+    const float* rotation;    // [n,4] raw quaternions
+    const float* rotation_r;  // [n,4]
+    const int* idx;           // [n,k] neighbour list (fdgs_rigid_neighbours)
+    const float* weight;      // [n,k]
+    const int* in_offsets;    // [n+1]
+    const int* in_edges;      // [n*k]
+    float* velocity;          // [n,3] written by the forward, read by the backward
+};
+size_t rigid_scratch_bytes(int n, int k);
+cudaError_t launch_rigid_neighbours(int n, int k, const int* idx, const float* dist2, char* scratch, float* weight,
+                                    int* in_offsets, int* in_edges, cudaStream_t stream);
+cudaError_t launch_rigid_forward(const RigidParams& p, char* scratch, float* loss_rigid, float* loss_motion, cudaStream_t stream);
+cudaError_t launch_rigid_backward(const RigidParams& p, const float* grad_rigid, const float* grad_motion, float* dL_dscaling,
+                                  float* dL_dscaling_t, float* dL_drotation, float* dL_drotation_r, cudaStream_t stream);
+
 cudaError_t launch_mark_visible(int P, const float* means3D, const float* viewmatrix, unsigned char* present,
                                 cudaStream_t stream);
 

@@ -557,14 +557,7 @@ __global__ void __launch_bounds__(128) sh_outer_sum_kernel(const ShSumParams a, 
     }
 }
 
-// 4x4 / 3x3 helpers, glm convention: A[c][r], (A*B)[c][r] = sum_k A[k][r] * B[c][k]
-__device__ __forceinline__ void mat4_mul(const float A[4][4], const float B[4][4], float C[4][4]) {
-#pragma unroll
-    for (int c = 0; c < 4; ++c)
-#pragma unroll
-        for (int r = 0; r < 4; ++r)
-            C[c][r] = A[0][r] * B[c][0] + A[1][r] * B[c][1] + A[2][r] * B[c][2] + A[3][r] * B[c][3];
-}
+// 3x3 helper, glm convention as mat4_mul (fdgs_common.cuh): A[c][r], (A*B)[c][r] = sum_k A[k][r] * B[c][k]
 __device__ __forceinline__ void mat3_mul(const float A[3][3], const float B[3][3], float C[3][3]) {
 #pragma unroll
     for (int c = 0; c < 3; ++c)
@@ -737,49 +730,9 @@ __global__ void __launch_bounds__(GB_THREADS, 8) geom_bwd_kernel(const Preproces
                     dL_dt += -ddot / cov_t;
                     g_ts += dL_dt;
 
-                    float dS[4][4];
-                    dS[0][0] = d[0]; dS[1][1] = d[3]; dS[2][2] = d[5]; dS[3][3] = dcovt;
-                    dS[0][1] = dS[1][0] = 0.5f * d[1];
-                    dS[0][2] = dS[2][0] = 0.5f * d[2];
-                    dS[1][2] = dS[2][1] = 0.5f * d[4];
-                    dS[0][3] = dS[3][0] = 0.5f * dc12[0];
-                    dS[1][3] = dS[3][1] = 0.5f * dc12[1];
-                    dS[2][3] = dS[3][2] = 0.5f * dc12[2];
-                    float M2[4][4], dM[4][4];
-#pragma unroll
-                    for (int c = 0; c < 4; ++c)
-#pragma unroll
-                        for (int r = 0; r < 4; ++r) M2[c][r] = 2.0f * S.M[c][r];
-                    mat4_mul(M2, dS, dM);   // dL_dM = 2 * M * dL_dSigma
-                    // dL_dscale_i = sum_c R[c][i] * dL_dM[c][i]
-                    float N[4][4];   // N[i][j] = s_i * dL_dM[j][i]   (= scaled dL_dMt)
                     float gs[4];
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        float acc = 0.f;
-#pragma unroll
-                        for (int c = 0; c < 4; ++c) {
-                            acc += R4[c][i] * dM[c][i];
-                            N[i][c] = sc[i] * dM[c][i];
-                        }
-                        gs[i] = acc;
-                    }
+                    cov4_bwd(d, dc12, dcovt, S.M, R4, sc, rot, rotr, gs, g_rot, g_rotr);
                     g_scale[0] = gs[0]; g_scale[1] = gs[1]; g_scale[2] = gs[2]; g_scale_t = gs[3];
-                    const float qa = rot.x, qb = rot.y, qc = rot.z, qd = rot.w;
-                    const float qp = rotr.x, qq = rotr.y, qr = rotr.z, qs = rotr.w;
-                    const float Ml[4][4] = {{qa, qb, -qc, qd}, {-qb, qa, qd, qc}, {qc, -qd, qa, qb}, {-qd, -qc, -qb, qa}};
-                    const float Mr[4][4] = {{qp, qq, -qr, -qs}, {-qq, qp, qs, -qr}, {qr, -qs, qp, -qq}, {qs, qr, qq, qp}};
-                    float X[4][4], Y[4][4];
-                    mat4_mul(N, Mr, X);    // dL_dml_t = dL_dMt * M_r
-                    mat4_mul(Ml, N, Y);    // dL_dmr_t = M_l * dL_dMt
-                    g_rot[0] = X[0][0] + X[1][1] + X[2][2] + X[3][3];
-                    g_rot[1] = -X[0][1] + X[1][0] - X[2][3] + X[3][2];
-                    g_rot[2] = X[0][2] - X[1][3] - X[2][0] + X[3][1];
-                    g_rot[3] = -X[0][3] - X[1][2] + X[2][1] + X[3][0];
-                    g_rotr[0] = Y[0][0] + Y[1][1] + Y[2][2] + Y[3][3];
-                    g_rotr[1] = -Y[0][1] + Y[1][0] + Y[2][3] - Y[3][2];
-                    g_rotr[2] = Y[0][2] + Y[1][3] - Y[2][0] - Y[3][1];
-                    g_rotr[3] = Y[0][3] - Y[1][2] + Y[2][1] - Y[3][0];
                 }
             } else {
                 // backward.cu:621-684 (and no marginal-opacity gradient for non-rot 4D, :917-919)

@@ -804,6 +804,129 @@ std::tuple<torch::Tensor, torch::Tensor> Knn(const torch::Tensor& xyz, const int
     return std::make_tuple(idx, d2);
 }
 
+// ---- rigidity and motion regularisers (include/fdgs.h: fdgs_rigid_*) -----------------------------------------------
+// Every tensor is checked for dtype, layout, shape and device before the device is touched.  An undefined or empty
+// optional tensor is "not provided".
+static const void* rigid_ptr(const torch::Tensor& t, torch::ScalarType dtype, int64_t rows, int64_t numel, const char* name) {
+    TORCH_CHECK(t.defined(), "fdgs: ", name, " is required");
+    TORCH_CHECK(t.scalar_type() == dtype, "fdgs: ", name, " must be ", c10::toString(dtype));
+    TORCH_CHECK(t.is_contiguous(), "fdgs: ", name, " must be contiguous");
+    TORCH_CHECK(t.dim() >= 1 && t.size(0) == rows && t.numel() == numel, "fdgs: ", name, " has the wrong shape");
+    return t.data_ptr();
+}
+
+static void rigid_same_device(std::initializer_list<const torch::Tensor*> ts) {
+    const torch::Tensor* first = nullptr;
+    for (const torch::Tensor* t : ts) {
+        if (!t->defined() || t->numel() == 0) continue;
+        TORCH_CHECK(t->is_cuda(), "fdgs: regulariser tensors must be CUDA tensors");
+        if (!first) first = t;
+        TORCH_CHECK(t->device() == first->device(), "fdgs: regulariser tensors on different devices");
+    }
+}
+
+// params = [t [n,1], scaling [n,3], scaling_t [n,1], rotation [n,4], rotation_r [n,4]] (the raw parameters)
+static fdgs_rigid_args rigid_args(const std::vector<torch::Tensor>& params, int64_t k) {
+    TORCH_CHECK(params.size() == 5, "fdgs: five parameter tensors (t, scaling, scaling_t, rotation, rotation_r)");
+    TORCH_CHECK(params[1].defined() && params[1].dim() == 2, "fdgs: scaling must be [n,3]");
+    const int64_t n = params[1].size(0);
+    fdgs_rigid_args a;
+    memset(&a, 0, sizeof(a));
+    a.n = (int)n;
+    a.k = (int)k;
+    a.t = static_cast<const float*>(rigid_ptr(params[0], torch::kFloat32, n, n, "t"));
+    a.scaling = static_cast<const float*>(rigid_ptr(params[1], torch::kFloat32, n, 3 * n, "scaling"));
+    a.scaling_t = static_cast<const float*>(rigid_ptr(params[2], torch::kFloat32, n, n, "scaling_t"));
+    a.rotation = static_cast<const float*>(rigid_ptr(params[3], torch::kFloat32, n, 4 * n, "rotation"));
+    a.rotation_r = static_cast<const float*>(rigid_ptr(params[4], torch::kFloat32, n, 4 * n, "rotation_r"));
+    return a;
+}
+
+static void rigid_list(fdgs_rigid_args& a, const torch::Tensor& idx, const torch::Tensor& weight) {
+    const int64_t n = a.n, k = a.k;
+    a.idx = static_cast<const int*>(rigid_ptr(idx, torch::kInt32, n, n * k, "idx"));
+    a.weight = static_cast<const float*>(rigid_ptr(weight, torch::kFloat32, n, n * k, "weight"));
+}
+
+static const float* rigid_scalar(const torch::Tensor& g, const char* name) {
+    if (!g.defined() || g.numel() == 0) return nullptr;
+    TORCH_CHECK(g.scalar_type() == torch::kFloat32 && g.numel() == 1, "fdgs: ", name, " must be one float32 element");
+    return g.data_ptr<float>();
+}
+
+// (weight, in_offsets, in_edges) of fdgs_knn's (idx, dist2)
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> RigidNeighbours(const torch::Tensor& idx, const torch::Tensor& dist2) {
+    TORCH_CHECK(idx.defined() && idx.dim() == 2, "fdgs: idx must be [n,k]");
+    const int64_t n = idx.size(0), k = idx.size(1);
+    TORCH_CHECK(n > 0 && k >= 1 && k <= 32, "fdgs: bad n / k (n > 0, 1 <= k <= 32)");
+    const int* ip = static_cast<const int*>(rigid_ptr(idx, torch::kInt32, n, n * k, "idx"));
+    const float* dp = static_cast<const float*>(rigid_ptr(dist2, torch::kFloat32, n, n * k, "dist2"));
+    rigid_same_device({&idx, &dist2});
+    const c10::cuda::CUDAGuard guard(idx.device());
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    auto opts = dist2.options();
+    torch::Tensor weight = torch::empty({n, k}, opts);
+    torch::Tensor in_offsets = torch::empty({n + 1}, opts.dtype(torch::kInt32));
+    torch::Tensor in_edges = torch::empty({n * k}, opts.dtype(torch::kInt32));
+    torch::Tensor scratch = torch::empty({(int64_t)fdgs_rigid_scratch_bytes((int)n, (int)k) + 256}, opts.dtype(torch::kByte));
+    check(fdgs_rigid_neighbours((int)n, (int)k, ip, dp, reinterpret_cast<char*>(scratch.data_ptr()), weight.data_ptr<float>(),
+                                in_offsets.data_ptr<int>(), in_edges.data_ptr<int>(), (void*)stream),
+          "rigid_neighbours");
+    return std::make_tuple(weight, in_offsets, in_edges);
+}
+
+// (velocity [n,3], loss_rigid, loss_motion); an unwanted loss comes back as 0
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> RigidForward(const std::vector<torch::Tensor>& params, const int64_t k,
+                                                                     const torch::Tensor& idx, const torch::Tensor& weight,
+                                                                     const bool want_rigid, const bool want_motion) {
+    fdgs_rigid_args a = rigid_args(params, k);
+    if (want_rigid) rigid_list(a, idx, weight);
+    rigid_same_device({&params[0], &params[1], &params[2], &params[3], &params[4], &idx, &weight});
+    TORCH_CHECK(params[1].is_cuda(), "fdgs: regulariser tensors must be CUDA tensors");
+    const c10::cuda::CUDAGuard guard(params[1].device());
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    auto opts = params[1].options();
+    torch::Tensor velocity = torch::empty({params[1].size(0), 3}, opts);
+    torch::Tensor lr = want_rigid ? torch::empty({}, opts) : torch::zeros({}, opts);
+    torch::Tensor lm = want_motion ? torch::empty({}, opts) : torch::zeros({}, opts);
+    const size_t sb = fdgs_rigid_scratch_bytes(a.n, a.k);
+    torch::Tensor scratch = torch::empty({(int64_t)sb + 256}, opts.dtype(torch::kByte));
+    a.velocity = velocity.data_ptr<float>();
+    check(fdgs_rigid_forward(&a, reinterpret_cast<char*>(scratch.data_ptr()), want_rigid ? lr.data_ptr<float>() : nullptr,
+                             want_motion ? lm.data_ptr<float>() : nullptr, (void*)stream),
+          "rigid_forward");
+    return std::make_tuple(velocity, lr, lm);
+}
+
+// gradients (scaling, scaling_t, rotation, rotation_r) shaped like the parameters; grad_rigid / grad_motion: the upstream
+// gradients (0-dim device tensors, empty = no such term)
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor> RigidBackward(
+    const std::vector<torch::Tensor>& params, const int64_t k, const torch::Tensor& velocity, const torch::Tensor& idx,
+    const torch::Tensor& weight, const torch::Tensor& in_offsets, const torch::Tensor& in_edges, const torch::Tensor& grad_rigid,
+    const torch::Tensor& grad_motion) {
+    fdgs_rigid_args a = rigid_args(params, k);
+    const int64_t n = a.n;
+    a.velocity = static_cast<float*>(const_cast<void*>(rigid_ptr(velocity, torch::kFloat32, n, 3 * n, "velocity")));
+    const float* gr = rigid_scalar(grad_rigid, "grad_rigid");
+    const float* gm = rigid_scalar(grad_motion, "grad_motion");
+    if (gr) {
+        rigid_list(a, idx, weight);
+        a.in_offsets = static_cast<const int*>(rigid_ptr(in_offsets, torch::kInt32, n + 1, n + 1, "in_offsets"));
+        a.in_edges = static_cast<const int*>(rigid_ptr(in_edges, torch::kInt32, n * k, n * k, "in_edges"));
+    }
+    rigid_same_device({&params[0], &params[1], &params[2], &params[3], &params[4], &velocity, &idx, &weight, &in_offsets, &in_edges,
+                       &grad_rigid, &grad_motion});
+    TORCH_CHECK(params[1].is_cuda(), "fdgs: regulariser tensors must be CUDA tensors");
+    const c10::cuda::CUDAGuard guard(params[1].device());
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    torch::Tensor ds = torch::empty_like(params[1]), dst = torch::empty_like(params[2]);
+    torch::Tensor dr = torch::empty_like(params[3]), drr = torch::empty_like(params[4]);
+    check(fdgs_rigid_backward(&a, gr, gm, ds.data_ptr<float>(), dst.data_ptr<float>(), dr.data_ptr<float>(), drr.data_ptr<float>(),
+                              (void*)stream),
+          "rigid_backward");
+    return std::make_tuple(ds, dst, dr, drr);
+}
+
 std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> DebugActivate(const torch::Tensor& log_s, const torch::Tensor& logit,
                                                                       const torch::Tensor& quat, const int64_t mode) {
     const c10::cuda::CUDAGuard guard(log_s.device());
@@ -824,6 +947,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("l1_ssim_backward", &L1SsimBackward);
     m.def("adam_step", &AdamStep);
     m.def("knn", &Knn);
+    m.def("rigid_neighbours", &RigidNeighbours);
+    m.def("rigid_forward", &RigidForward);
+    m.def("rigid_backward", &RigidBackward);
     m.def("densify_plan", &DensifyPlan);
     m.def("densify_apply", &DensifyApply);
     m.def("reset_opacity", &ResetOpacity);

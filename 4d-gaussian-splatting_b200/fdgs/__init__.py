@@ -27,6 +27,7 @@ ABI_SYMBOLS = (
     "fdgs_knn_scratch_bytes", "fdgs_knn", "fdgs_debug_activate", "fdgs_union_maps", "fdgs_set_tile_cull", "fdgs_view_stats",
     "fdgs_forward_bg", "fdgs_backward_bg", "fdgs_sky_forward", "fdgs_sky_backward",
     "fdgs_densify_scratch_bytes", "fdgs_densify_plan", "fdgs_densify_apply", "fdgs_reset_opacity", "fdgs_densify_stats",
+    "fdgs_rigid_scratch_bytes", "fdgs_rigid_neighbours", "fdgs_rigid_forward", "fdgs_rigid_backward",
 )
 
 STAGE_NAMES = ("preprocess_fwd", "bin_count_scan", "bin_scatter", "tile_sort_pack", "reserved", "blend_fwd", "blend_bwd",
@@ -53,6 +54,7 @@ def lib():
             getattr(_lib, n).restype = ctypes.c_size_t
         _lib.fdgs_launch_count.restype = ctypes.c_longlong
         _lib.fdgs_densify_scratch_bytes.restype = ctypes.c_size_t
+        _lib.fdgs_rigid_scratch_bytes.restype = ctypes.c_size_t
     return _lib
 
 

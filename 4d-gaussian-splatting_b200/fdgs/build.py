@@ -20,7 +20,7 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_DIR = os.path.join(PKG_DIR, "fdgs", "lib")
 OBJ_DIR = os.path.join(LIB_DIR, "obj")
 
-CU_SOURCES = ["preprocess_fwd.cu", "binning.cu", "blend_fwd.cu", "blend_bwd.cu", "preprocess_bwd.cu", "exchange.cu", "loss.cu", "optim.cu", "knn.cu", "sky.cu", "densify.cu", "fdgs_api.cu"]
+CU_SOURCES = ["preprocess_fwd.cu", "binning.cu", "blend_fwd.cu", "blend_bwd.cu", "preprocess_bwd.cu", "exchange.cu", "loss.cu", "optim.cu", "knn.cu", "sky.cu", "densify.cu", "regularize.cu", "fdgs_api.cu"]
 HEADERS = ["fdgs_common.cuh", "fdgs_internal.h", os.path.join(REPO_DIR, "include", "fdgs.h")]
 
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",

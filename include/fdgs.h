@@ -415,6 +415,46 @@ int fdgs_adam_step(int n, float* const* params, float* const* grads, float* cons
 size_t fdgs_knn_scratch_bytes(int n);
 int fdgs_knn(int n, int k, const float* xyz, char* scratch, int* idx, float* dist2, int brute_force, void* stream);
 
+/* Rigidity and motion regularisers (reference: train.py:132-159, with the velocity of scene/gaussian_model.py:34-47,
+ * 247-251 get_current_covariance_and_mean_offset(1.0, t + 0.1) for rot_4d models):
+ *   dt = (t + 0.1f) - t;  v_i = Sigma[0:3,3] / Sigma[3,3] * dt   (Sigma = the 4D covariance of the raw parameters:
+ *        scales exp(scaling), exp(scaling_t); quaternions q / ||q||; scaling modifier 1)
+ *   w_ij = exp(-100 * dist2_ij)  over the k neighbours of fdgs_knn (the point itself first)
+ *   loss_rigid  = (sum_i sum_j w_ij ||v_j - v_i||) / k / n        loss_motion = mean_i ||v_i||
+ * v is evaluated in double from the fp32 parameters and rounded once; the sums are accumulated in double in a fixed
+ * order and rounded once: results are bit-identical run to run.
+ * Gradients go to scaling, scaling_t, rotation and rotation_r only (the reference's t gradient is exactly 0 and its
+ * kNN input is detached); an edge with ||v_j - v_i|| = 0 contributes no gradient, like torch's norm backward.
+ * Nothing synchronises the host. */
+typedef struct fdgs_rigid_args {
+    int n;                        /* Gaussians                                 */
+    int k;                        /* neighbours per row, 1..32                 */
+    const float* t;               /* [n]                                       */
+    const float* scaling;         /* [n,3] log-scales                          */
+    const float* scaling_t;       /* [n]   log-scale                           */
+    const float* rotation;        /* [n,4] un-normalised                       */
+    const float* rotation_r;      /* [n,4] un-normalised                       */
+    const int* idx;               /* [n,k] neighbour list (rigidity only)      */
+    const float* weight;          /* [n,k]                                     */
+    const int* in_offsets;        /* [n+1] incoming edges (rigidity backward)  */
+    const int* in_edges;          /* [n*k]                                     */
+    float* velocity;              /* [n,3] written by the forward, read by the backward */
+} fdgs_rigid_args;
+/* Bytes of device scratch fdgs_rigid_neighbours and fdgs_rigid_forward need. */
+size_t fdgs_rigid_scratch_bytes(int n, int k);
+/* The neighbour list of one set of positions, reusable by every call until the positions change: weight [n,k] =
+ * exp(-100 * dist2) (bit-identical to torch.exp(-100 * dist)) and the transpose -- the incoming edges of row j are
+ * in_edges[in_offsets[j] .. in_offsets[j+1]), edge id = i * k + slot, ascending.  idx / dist2 = fdgs_knn's output. */
+int fdgs_rigid_neighbours(int n, int k, const int* idx, const float* dist2, char* scratch, float* weight, int* in_offsets,
+                          int* in_edges, void* stream);
+/* Writes velocity and the requested losses (device floats; NULL = not wanted; the rigidity loss needs idx / weight). */
+int fdgs_rigid_forward(const fdgs_rigid_args* args, char* scratch, float* loss_rigid, float* loss_motion, void* stream);
+/* Gradients w.r.t. the raw parameters, overwritten for every row, given the upstream gradients of the two losses
+ * (device scalars; NULL = no such term; the rigidity term needs the whole neighbour list).  args->velocity must hold
+ * the forward's velocity. */
+int fdgs_rigid_backward(const fdgs_rigid_args* args, const float* grad_rigid, const float* grad_motion, float* dL_dscaling,
+                        float* dL_dscaling_t, float* dL_drotation, float* dL_drotation_r, void* stream);
+
 /* Union bookkeeping of the exchange: cs = inclusive prefix sum of (radii > 0) over the P Gaussians (device, int32).
  * Writes slot_of[i] = cs[i] - 1 for union Gaussians, -1 otherwise, and the inverse map idx[slot] = i (idx: K =
  * cs[P-1] entries, int64). */
