@@ -787,6 +787,35 @@ int fdgs_rigid_backward(const fdgs_rigid_args* a, const float* grad_rigid, const
     return FDGS_OK;
 }
 
+// ---- evaluation metrics (metrics.cu) --------------------------------------------------------------------------------
+static int check_metrics_size(int B, int C, int H, int W) {
+    if (B <= 0 || C <= 0 || H <= 0 || W <= 0) return fail(FDGS_ERR_INVALID_ARG, "bad B / C / H / W");
+    if (H < 176 || W < 176) return fail(FDGS_ERR_INVALID_ARG, "H and W must be at least 176 (MS-SSIM's five scales)");
+    if ((long long)B * C > 65535) return fail(FDGS_ERR_INVALID_ARG, "B * C exceeds 65535 image planes");
+    // the float64 pyramid is about 2/3 of 16 bytes per input pixel; tile rows must fit the grid's y extent
+    if ((double)B * C * H * W * 16.0 > 9.0e18 || (H + 31) / 32 > 65535)
+        return fail(FDGS_ERR_INVALID_ARG, "image size overflow");
+    return FDGS_OK;
+}
+
+size_t fdgs_metrics_scratch_bytes(int B, int C, int H, int W) {
+    if (check_metrics_size(B, C, H, W) != FDGS_OK) {
+        g_last_error.clear();
+        return 0;
+    }
+    return fdgs::metrics_scratch_bytes(B, C, H, W);
+}
+
+int fdgs_image_metrics(const fdgs_metrics_args* a, char* scratch, void* stream_v) {
+    g_last_error.clear();
+    if (!a) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    if (int rc = check_metrics_size(a->B, a->C, a->H, a->W)) return rc;
+    if (!a->x || !a->y || !a->out || !scratch) return fail(FDGS_ERR_INVALID_ARG, "null argument: x / y / out / scratch");
+    FDGS_CUDA(fdgs::launch_image_metrics(*a, scratch, reinterpret_cast<cudaStream_t>(stream_v)), "image_metrics");
+    g_kernel_launches += a->accum ? 7 : 6;
+    return FDGS_OK;
+}
+
 int fdgs_debug_activate(int n, const float* log_s, const float* logit, const float* quat, int mode, float* s_out, float* o_out,
                         float* q_out, void* stream_v) {
     g_last_error.clear();

@@ -251,6 +251,10 @@ cudaError_t launch_rigid_forward(const RigidParams& p, char* scratch, float* los
 cudaError_t launch_rigid_backward(const RigidParams& p, const float* grad_rigid, const float* grad_motion, float* dL_dscaling,
                                   float* dL_dscaling_t, float* dL_drotation, float* dL_drotation_r, cudaStream_t stream);
 
+// evaluation metrics: L1, PSNR, SSIM, MS-SSIM (metrics.cu; the arguments are validated by fdgs_api.cu)
+size_t metrics_scratch_bytes(int B, int C, int H, int W);
+cudaError_t launch_image_metrics(const fdgs_metrics_args& a, char* scratch, cudaStream_t stream);
+
 cudaError_t launch_mark_visible(int P, const float* means3D, const float* viewmatrix, unsigned char* present,
                                 cudaStream_t stream);
 

@@ -16,18 +16,15 @@
 // (181 MB at 3 x 1352 x 1014) against ~60 for the reference's op-by-op path; the kernels are bound by the shared-memory
 // filter passes, not by HBM.  dL/dx is the dL_dpix the blend backward consumes (fdgs_backward_args.dL_dpix).
 #include "fdgs_internal.h"
+#include "ssim_common.cuh"
 
 namespace fdgs {
 namespace {
 
 constexpr int LT = 32;            // tile edge (pixels)
-constexpr int LR = 5;             // filter radius: window_size 11 (reference: utils/loss_utils.py:39)
+constexpr int LR = SSIM_R;        // filter radius (ssim_common.cuh)
 constexpr int LW = LT + 2 * LR;   // staged edge
 constexpr int LTHREADS = 256;
-
-struct GaussWin {
-    float g[2 * LR + 1];
-};
 
 // x, y: [C,H,W]; maps: [3,C,H,W] (a = dS/dmu_x, b = dS/dE[xx], c = dS/dE[xy]); sums[0] += sum|x-y|, sums[1] += sum SSIM
 __global__ void __launch_bounds__(LTHREADS) ssim_fwd_kernel(const float* __restrict__ x, const float* __restrict__ y, int H, int W,
@@ -79,13 +76,8 @@ __global__ void __launch_bounds__(LTHREADS) ssim_fwd_kernel(const float* __restr
             e22 = fmaf(w, hz[3][r + k][c], e22);
             e12 = fmaf(w, hz[4][r + k][c], e12);
         }
-        // reference: utils/loss_utils.py:50-60
-        const float C1 = 0.01f * 0.01f, C2 = 0.03f * 0.03f;
-        const float m11 = m1 * m1, m22 = m2 * m2, m12 = m1 * m2;
-        const float s11 = e11 - m11, s22 = e22 - m22, s12 = e12 - m12;
-        const float A1 = 2.f * m12 + C1, A2 = 2.f * s12 + C2, B1 = m11 + m22 + C1, B2 = s11 + s22 + C2;
-        const float inv = 1.f / (B1 * B2);
-        const float S = A1 * A2 * inv;
+        const SsimTerms<float> t = ssim_terms(m1, m2, e11, e22, e12);
+        const float A1 = t.A1, A2 = t.A2, B1 = t.B1, B2 = t.B2, inv = t.inv, S = t.S;
         // S as a function of (mu_x, E[xx], E[xy]) with the ground-truth moments fixed
         const float da = 2.f * m2 * (A2 - A1) * inv + 2.f * m1 * S * (1.f / B2 - 1.f / B1);
         const float db = -S / B2;
@@ -163,19 +155,6 @@ __global__ void __launch_bounds__(LTHREADS) ssim_bwd_kernel(const float* __restr
         const float sgn = (d > 0.f) ? 1.f : ((d < 0.f) ? -1.f : 0.f);   // torch.abs backward: sign, 0 at 0
         dL_dx[o] = gs * (k_ssim * (ca + 2.f * xv * cb + yv * cc) + k_l1 * sgn);
     }
-}
-
-GaussWin make_window() {
-    // reference: utils/loss_utils.py:24-26 gaussian(11, 1.5): float32 exp values normalised by their float32 sum
-    GaussWin w;
-    float v[2 * LR + 1];
-    float s = 0.f;
-    for (int i = 0; i <= 2 * LR; ++i) {
-        v[i] = (float)exp(-(double)((i - LR) * (i - LR)) / (2.0 * 1.5 * 1.5));
-        s += v[i];
-    }
-    for (int i = 0; i <= 2 * LR; ++i) w.g[i] = v[i] / s;
-    return w;
 }
 
 }  // namespace

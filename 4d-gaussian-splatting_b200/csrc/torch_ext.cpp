@@ -927,6 +927,39 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor> RigidBack
     return std::make_tuple(ds, dst, dr, drr);
 }
 
+// ---- evaluation metrics (include/fdgs.h: fdgs_image_metrics) ---------------------------------------------------------
+// x, y: [B,C,H,W] float32 contiguous CUDA tensors; accum: float64 [5] on the same device, or empty = none.
+// Returns out [B,4] float64 (l1, psnr, ssim, msssim per view).  Checks dtype, layout and shape before the device.
+torch::Tensor ImageMetrics(const torch::Tensor& x, const torch::Tensor& y, const bool clamp, const torch::Tensor& accum) {
+    TORCH_CHECK(x.defined() && y.defined(), "fdgs: image_metrics needs two images");
+    TORCH_CHECK(x.scalar_type() == torch::kFloat32 && y.scalar_type() == torch::kFloat32, "fdgs: images must be Float (float32)");
+    TORCH_CHECK(x.is_contiguous() && y.is_contiguous(), "fdgs: images must be contiguous");
+    TORCH_CHECK(x.dim() == 4 && x.sizes() == y.sizes(), "fdgs: images must be [B,C,H,W] of equal shape");
+    const bool has_accum = accum.defined() && accum.numel() > 0;
+    if (has_accum) {
+        TORCH_CHECK(accum.scalar_type() == torch::kFloat64 && accum.is_contiguous() && accum.numel() == 5,
+                    "fdgs: accum must be a contiguous Double (float64) tensor of 5 elements");
+    }
+    TORCH_CHECK(x.is_cuda() && y.is_cuda() && x.device() == y.device() && (!has_accum || accum.device() == x.device()),
+                "fdgs: image_metrics tensors must be CUDA tensors on one device");
+    fdgs_metrics_args a;
+    memset(&a, 0, sizeof(a));
+    a.B = (int)x.size(0); a.C = (int)x.size(1); a.H = (int)x.size(2); a.W = (int)x.size(3);
+    TORCH_CHECK(x.size(0) == a.B && x.size(1) == a.C && x.size(2) == a.H && x.size(3) == a.W, "fdgs: image size overflow");
+    const size_t sb = fdgs_metrics_scratch_bytes(a.B, a.C, a.H, a.W);
+    const c10::cuda::CUDAGuard guard(x.device());
+    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    torch::Tensor out = torch::empty({x.size(0), 4}, x.options().dtype(torch::kFloat64));
+    torch::Tensor scratch = torch::empty({(int64_t)sb}, x.options().dtype(torch::kByte));
+    a.x = x.data_ptr<float>();
+    a.y = y.data_ptr<float>();
+    a.clamp = clamp ? 1 : 0;
+    a.out = out.data_ptr<double>();
+    a.accum = has_accum ? accum.data_ptr<double>() : nullptr;
+    check(fdgs_image_metrics(&a, reinterpret_cast<char*>(scratch.data_ptr()), (void*)stream), "image_metrics");
+    return out;
+}
+
 std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> DebugActivate(const torch::Tensor& log_s, const torch::Tensor& logit,
                                                                       const torch::Tensor& quat, const int64_t mode) {
     const c10::cuda::CUDAGuard guard(log_s.device());
@@ -950,6 +983,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("rigid_neighbours", &RigidNeighbours);
     m.def("rigid_forward", &RigidForward);
     m.def("rigid_backward", &RigidBackward);
+    m.def("image_metrics", &ImageMetrics);
     m.def("densify_plan", &DensifyPlan);
     m.def("densify_apply", &DensifyApply);
     m.def("reset_opacity", &ResetOpacity);

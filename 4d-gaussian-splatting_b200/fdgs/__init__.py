@@ -28,6 +28,7 @@ ABI_SYMBOLS = (
     "fdgs_forward_bg", "fdgs_backward_bg", "fdgs_sky_forward", "fdgs_sky_backward",
     "fdgs_densify_scratch_bytes", "fdgs_densify_plan", "fdgs_densify_apply", "fdgs_reset_opacity", "fdgs_densify_stats",
     "fdgs_rigid_scratch_bytes", "fdgs_rigid_neighbours", "fdgs_rigid_forward", "fdgs_rigid_backward",
+    "fdgs_metrics_scratch_bytes", "fdgs_image_metrics",
 )
 
 STAGE_NAMES = ("preprocess_fwd", "bin_count_scan", "bin_scatter", "tile_sort_pack", "reserved", "blend_fwd", "blend_bwd",
@@ -55,6 +56,7 @@ def lib():
         _lib.fdgs_launch_count.restype = ctypes.c_longlong
         _lib.fdgs_densify_scratch_bytes.restype = ctypes.c_size_t
         _lib.fdgs_rigid_scratch_bytes.restype = ctypes.c_size_t
+        _lib.fdgs_metrics_scratch_bytes.restype = ctypes.c_size_t
     return _lib
 
 

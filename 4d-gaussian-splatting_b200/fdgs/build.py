@@ -20,8 +20,8 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_DIR = os.path.join(PKG_DIR, "fdgs", "lib")
 OBJ_DIR = os.path.join(LIB_DIR, "obj")
 
-CU_SOURCES = ["preprocess_fwd.cu", "binning.cu", "blend_fwd.cu", "blend_bwd.cu", "preprocess_bwd.cu", "exchange.cu", "loss.cu", "optim.cu", "knn.cu", "sky.cu", "densify.cu", "regularize.cu", "fdgs_api.cu"]
-HEADERS = ["fdgs_common.cuh", "fdgs_internal.h", os.path.join(REPO_DIR, "include", "fdgs.h")]
+CU_SOURCES = ["preprocess_fwd.cu", "binning.cu", "blend_fwd.cu", "blend_bwd.cu", "preprocess_bwd.cu", "exchange.cu", "loss.cu", "optim.cu", "knn.cu", "sky.cu", "densify.cu", "regularize.cu", "metrics.cu", "fdgs_api.cu"]
+HEADERS = ["fdgs_common.cuh", "fdgs_internal.h", "ssim_common.cuh", os.path.join(REPO_DIR, "include", "fdgs.h")]
 
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]

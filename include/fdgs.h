@@ -455,6 +455,29 @@ int fdgs_rigid_forward(const fdgs_rigid_args* args, char* scratch, float* loss_r
 int fdgs_rigid_backward(const fdgs_rigid_args* args, const float* grad_rigid, const float* grad_motion, float* dL_dscaling,
                         float* dL_dscaling_t, float* dL_drotation, float* dL_drotation_r, void* stream);
 
+/* Evaluation metrics of B image pairs (reference: train.py:312-334 training_report), per view b, in float64:
+ *   out[4b + 0] = mean |x - y|                                            (utils/loss_utils.py:18-19)
+ *   out[4b + 1] = mean over channels of 20 log10(1 / sqrt(mse_c))         (utils/image_utils.py:17-19; mse_c = 0: +inf)
+ *   out[4b + 2] = mean of the SSIM map: 11x11 Gaussian, sigma 1.5, zero padding (utils/loss_utils.py:34-64)
+ *   out[4b + 3] = MS-SSIM of torchmetrics 0.11.4 MultiScaleStructuralSimilarityIndexMeasure(data_range=1.0):
+ *                 five scales, 2x2 average pooling between them, valid windows, betas (0.0448, 0.2856, 0.3001,
+ *                 0.2363, 0.1333), relu of the per-scale means.
+ * clamp != 0 clamps x (never y) to [0, 1] first.  accum (NULL = none): accum[0..3] += the four numbers and
+ * accum[4] += 1 per view, in view order.  Per-tile partials are reduced in a fixed order, so results are bit-identical
+ * run to run and a batch gives what B single-view calls give.  H and W must be at least 176 (MS-SSIM's five scales),
+ * B * C at most 65535.  `scratch` holds fdgs_metrics_scratch_bytes bytes.  Nothing synchronises the host. */
+typedef struct fdgs_metrics_args {
+    int B, C, H, W;
+    const float* x;               /* [B,C,H,W] render                          */
+    const float* y;               /* [B,C,H,W] ground truth                    */
+    int clamp;                    /* != 0: x is clamped to [0, 1]              */
+    double* out;                  /* [B,4] l1, psnr, ssim, msssim              */
+    double* accum;                /* [5] four sums and a view count, or NULL   */
+} fdgs_metrics_args;
+/* Bytes of device scratch fdgs_image_metrics needs (0 for sizes it rejects). */
+size_t fdgs_metrics_scratch_bytes(int B, int C, int H, int W);
+int fdgs_image_metrics(const fdgs_metrics_args* args, char* scratch, void* stream);
+
 /* Union bookkeeping of the exchange: cs = inclusive prefix sum of (radii > 0) over the P Gaussians (device, int32).
  * Writes slot_of[i] = cs[i] - 1 for union Gaussians, -1 otherwise, and the inverse map idx[slot] = i (idx: K =
  * cs[P-1] entries, int64). */
