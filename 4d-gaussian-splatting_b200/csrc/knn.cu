@@ -167,12 +167,16 @@ __global__ void __launch_bounds__(128) knn_search_kernel(int n, int k, const flo
     float bd[KNN_MAX_K];
     int bi[KNN_MAX_K];
     int cnt = 0;
-    // distance from the query to the nearest face of its own cell: everything beyond shell r is at least r*h + margin away
+    // distance from the query to the nearest face of its own cell: everything beyond shell r is at least r*h + margin away.
+    // The faces the binning uses are where fl(fl(x - lo) * inv_h) crosses an integer, not the c*h measured here: the two
+    // differ by the rounding of x - lo, of the product and of inv_h = fl(1/h), up to ~3 * 2^-24 * (c + 1) * h.  A query
+    // within that of a face could otherwise stop at shell 0 before a closer point the rounding put in the next cell, so
+    // the margin gives up 1e-6 * (res + 1) * h (>= 16x the bound; at most 1.6e-4 h at 160 cells per axis).
     float margin = g.h;
     {
         const float fx = (qx - g.lo[0]) - cx * g.h, fy = (qy - g.lo[1]) - cy * g.h, fz = (qz - g.lo[2]) - cz * g.h;
         margin = fminf(margin, fminf(fminf(fx, g.h - fx), fminf(fminf(fy, g.h - fy), fminf(fz, g.h - fz))));
-        margin = fmaxf(margin, 0.f);
+        margin = fmaxf(margin - 1e-6f * (float)(res + 1) * g.h, 0.f);
     }
     for (int r = 0; r < res; ++r) {
         const int z0 = cz - r, z1 = cz + r, y0 = cy - r, y1 = cy + r, x0 = cx - r, x1 = cx + r;

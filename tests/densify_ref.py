@@ -144,8 +144,7 @@ def clone_model(m, optim=None):
         c.optimizer = torch.optim.Adam(groups, lr=0.0, eps=1e-15)
     else:
         from fdgs.optim import FusedAdam
-        c.optimizer = FusedAdam(groups, lr=0.0, eps=1e-15)
-        c.optimizer.step_count = getattr(m.optimizer, "step_count", 1)
+        c.optimizer = FusedAdam(groups, lr=0.0, eps=1e-15)     # the copied state carries each tensor's "step"
     for g_old, g_new in zip(m.optimizer.param_groups, c.optimizer.param_groups):
         st = m.optimizer.state.get(g_old["params"][0])
         if st is not None:

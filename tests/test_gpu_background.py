@@ -14,6 +14,7 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 CASES = ["small", "flowbg", "ragged", "rotcam", "n3v", "mid", "cfg5"]
 CHAIN = {"scales", "scales_t", "rotations", "rotations_r", "ts"}
+RAW_CHAIN = {"scaling", "scaling_t", "rotation", "rotation_r", "t"}     # the same leaves under RawModel's names
 
 
 def _bg_image(cfg):
@@ -136,7 +137,10 @@ def test_raw_entry_with_background_image(name):
     assert torch.equal(out["native"][2], out["torch"][2])
     for k, a in out["native"][1].items():
         b = out["torch"][1][k]
-        assert helpers.l2_rel(helpers.to_np(a.grad), helpers.to_np(b.grad)) <= 1e-4, k
+        # the chain leaves at P >= 50000: the bar of test_gradients_match_autograd_through_the_composition (the same
+        # native path run twice differs there by up to 1.2e-4 rel-L2: the blend backward's atomics, amplified)
+        bar = 2e-3 if (k in RAW_CHAIN and cfg["P"] >= 50000) else 1e-4
+        assert helpers.l2_rel(helpers.to_np(a.grad), helpers.to_np(b.grad)) <= bar, k
     assert helpers.l2_rel(helpers.to_np(out["native"][3]), helpers.to_np(out["torch"][3])) <= 1e-4
 
 

@@ -182,7 +182,11 @@ def test_render_with_environment_map(name, pipe):
     for k in list(A.leaves()) + ["viewspace_points"]:
         a, b = (pa[k].grad, pb[k].grad) if k == "viewspace_points" else (A.leaves()[k].grad, B.leaves()[k].grad)
         e = helpers.l2_rel(helpers.to_np(a), helpers.to_np(b))
-        bar = max(2e-3 if (k in chain and cfg["P"] >= 50000) else 1e-4, 4 * floor[k])
+        # the chain leaves' bar at every size: the blend backward accumulates per Gaussian with atomics, and the chain
+        # to scales and rotations amplifies that order's rounding -- the same native render run twice differs there by
+        # up to 7e-5 (n3v, 3000 Gaussians) and 1.2e-4 (mid) rel-L2 on an H100, so a 1e-4 bar on the distance of two
+        # such runs fails about half the time
+        bar = max(2e-3 if k in chain else 1e-4, 4 * floor[k])
         print("%s %-17s rel-L2 %.2e (constant-background formulations %.2e, bar %.2e)" % (name, k, e, floor[k], bar))
         assert e <= bar, (k, e, floor[k])
 
