@@ -10,6 +10,12 @@
 //   rasterize_gaussians_backward(37 args) -> 12 gradient tensors
 //   mark_visible(means3D, viewmatrix, projmatrix) -> bool[P]
 //
+// and one extended entry per direction, which the autograd Function of this package calls:
+//
+//   rasterize_gaussians_ext(30 args, sh_rest, raw_params, bg_image)  -> the same 11-tuple
+//   rasterize_gaussians_backward_ext(37 args, sh_rest, raw_params, bg_image, sh_factor_mode, want_dbg)
+//                                         -> [12 gradients, sh_factors, dL_dsh_rest, dL_dbg_image]
+//
 // PyTorch is plumbing only: it owns the memory (tensors, the three growable byte buffers handed
 // to the library through the allocation callback) and supplies the current CUDA stream.  No
 // arithmetic happens here.  Differences from the reference shim, all performance-motivated and
@@ -21,6 +27,7 @@
 #include <torch/extension.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <c10/cuda/CUDAStream.h>
+#include <string>
 #include <tuple>
 #include <vector>
 #include "../../include/fdgs.h"
@@ -33,8 +40,20 @@ char* resize_cb(void* ctx, size_t bytes) {
     return reinterpret_cast<char*>(t->data_ptr());
 }
 
+void check(int rc, const char* where) {
+    if (rc != FDGS_OK) throw std::runtime_error(std::string("fdgs ") + where + " failed: " + fdgs_last_error());
+}
+
+// The device guard and current stream every launch of a binding runs under.
+struct DeviceStream {
+    c10::cuda::CUDAGuard guard;
+    cudaStream_t stream;
+    explicit DeviceStream(const torch::Tensor& t) : guard(t.device()), stream(c10::cuda::getCurrentCUDAStream().stream()) {}
+};
+
+// ---- the rasterizer's contract (the reference's): any layout is accepted and copied contiguous; an empty tensor is
+// "not provided", a null pointer in C (reference: diff_gaussian_rasterization.py:282-300) ----------------------------
 const float* fptr(const torch::Tensor& t) {
-    // empty tensor == "not provided" (reference: diff_gaussian_rasterization.py:282-300)
     if (!t.defined() || t.numel() == 0) return nullptr;
     TORCH_CHECK(t.is_cuda(), "fdgs: expected a CUDA tensor");
     TORCH_CHECK(t.scalar_type() == torch::kFloat32, "fdgs: expected a float32 tensor");
@@ -53,47 +72,68 @@ torch::Tensor background_image(const torch::Tensor& bg_image, const torch::Tenso
     return bg_image.contiguous();
 }
 
-void check(int rc, const char* where) {
-    if (rc != FDGS_OK) throw std::runtime_error(std::string("fdgs ") + where + " failed: " + fdgs_last_error());
+// ---- the training-step bindings' strict contract: no copies, so a tensor of the wrong dtype, layout or shape is an
+// error.  dtype, layout and shape of every argument are checked first (arg), then the device (same_cuda_device), and
+// only then is anything allocated or launched: a malformed call fails before any GPU work. ---------------------------
+
+// "Float (float32)": ATen's name of a dtype and torch's
+std::string dtype_name(torch::ScalarType t) {
+    return std::string(c10::toString(t)) + " (" + c10::getDtypeNames(t).first + ")";
+}
+
+constexpr bool REQUIRED = true;
+
+// The data pointer of tensor argument `name`: dtype T, contiguous, `rows` rows (size(0); < 0: any) and `numel`
+// elements (< 0: any).  An undefined or empty optional tensor is "not provided" (nullptr; the C-ABI rejects a null it
+// needs); a required one is checked like any other.
+template <typename T>
+T* arg(const torch::Tensor& t, const char* name, int64_t rows = -1, int64_t numel = -1, bool required = false) {
+    TORCH_CHECK(!required || t.defined(), "fdgs: ", name, " is required");
+    if (!t.defined() || (!required && t.numel() == 0)) return nullptr;
+    const torch::ScalarType dtype = c10::CppTypeToScalarType<T>::value;
+    TORCH_CHECK(t.scalar_type() == dtype, "fdgs: ", name, " must be ", dtype_name(dtype));
+    TORCH_CHECK(t.is_contiguous(), "fdgs: ", name, " must be contiguous");
+    TORCH_CHECK((rows < 0 || (t.dim() >= 1 && t.size(0) == rows)) && (numel < 0 || t.numel() == numel), "fdgs: ", name,
+                " has the wrong shape");
+    return t.data_ptr<T>();
+}
+
+// every provided (defined, non-empty) tensor of a call on one CUDA device, that of the first
+void same_cuda_device(const char* what, const std::vector<torch::Tensor>& ts) {
+    const torch::Tensor* first = nullptr;
+    for (const torch::Tensor& t : ts) {
+        if (!t.defined() || t.numel() == 0) continue;
+        TORCH_CHECK(t.is_cuda(), "fdgs: ", what, " tensors must be CUDA tensors");
+        if (!first) first = &t;
+        TORCH_CHECK(t.device() == first->device(), "fdgs: ", what, " tensors on different devices");
+    }
 }
 
 }  // namespace
 
-#define FDGS_FWD_PARAMS                                                                                                \
-    const torch::Tensor &background, const torch::Tensor &means3D, const torch::Tensor &colors,                        \
-        const torch::Tensor &flows, const torch::Tensor &opacity, const torch::Tensor &ts, const torch::Tensor &scales, \
-        const torch::Tensor &scales_t, const torch::Tensor &rotations, const torch::Tensor &rotations_r,               \
-        const float scale_modifier, const torch::Tensor &cov3D_precomp, const float prefilter_var,                     \
-        const torch::Tensor &viewmatrix, const torch::Tensor &projmatrix, const float tan_fovx, const float tan_fovy,  \
-        const int image_height, const int image_width, const torch::Tensor &sh, const int degree, const int degree_t,  \
-        const torch::Tensor &campos, const float timestamp, const float time_duration, const bool rot_4d,              \
-        const int gaussian_dim, const bool force_sh_3d, const bool prefiltered, const bool debug
-#define FDGS_FWD_ARGS                                                                                                  \
-    background, means3D, colors, flows, opacity, ts, scales, scales_t, rotations, rotations_r, scale_modifier,         \
-        cov3D_precomp, prefilter_var, viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh,       \
-        degree, degree_t, campos, timestamp, time_duration, rot_4d, gaussian_dim, force_sh_3d, prefiltered, debug
-
 using ForwardOut = std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor,
                               torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>;
 
-// sh_rest (possibly empty) / raw_params: the raw-parameter entry of include/fdgs.h (fdgs_forward_args.raw_params)
-static ForwardOut
-forward_impl(const torch::Tensor& bg_image, const torch::Tensor& sh_rest, const bool raw_params,
-                       const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors,
-                       const torch::Tensor& flows, const torch::Tensor& opacity, const torch::Tensor& ts,
-                       const torch::Tensor& scales, const torch::Tensor& scales_t, const torch::Tensor& rotations,
-                       const torch::Tensor& rotations_r, const float scale_modifier, const torch::Tensor& cov3D_precomp,
-                       const float prefilter_var, const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix,
-                       const float tan_fovx, const float tan_fovy, const int image_height, const int image_width,
-                       const torch::Tensor& sh, const int degree, const int degree_t, const torch::Tensor& campos,
-                       const float timestamp, const float time_duration, const bool rot_4d, const int gaussian_dim,
-                       const bool force_sh_3d, const bool prefiltered, const bool debug) {
+// The reference's 30 arguments (rasterize_points.h:18-49) + the extensions of include/fdgs.h, each empty / false when
+// unused: sh_rest and raw_params, the raw-parameter entry (fdgs_forward_args.raw_params: scales = log-scales, rotations
+// un-normalised, opacity = logits; sh = features_dc [P,1,3], sh_rest = features_rest [P,M-1,3]), and bg_image, a
+// per-pixel background [3,H,W] (fdgs_forward_bg).  Returns the reference's 11-tuple.
+ForwardOut RasterizeGaussiansExt(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors,
+                                 const torch::Tensor& flows, const torch::Tensor& opacity, const torch::Tensor& ts,
+                                 const torch::Tensor& scales, const torch::Tensor& scales_t, const torch::Tensor& rotations,
+                                 const torch::Tensor& rotations_r, const float scale_modifier,
+                                 const torch::Tensor& cov3D_precomp, const float prefilter_var,
+                                 const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx,
+                                 const float tan_fovy, const int image_height, const int image_width,
+                                 const torch::Tensor& sh, const int degree, const int degree_t, const torch::Tensor& campos,
+                                 const float timestamp, const float time_duration, const bool rot_4d,
+                                 const int gaussian_dim, const bool force_sh_3d, const bool prefiltered, const bool debug,
+                                 const torch::Tensor& sh_rest, const bool raw_params, const torch::Tensor& bg_image) {
     if (means3D.ndimension() != 2 || means3D.size(1) != 3) {
         AT_ERROR("means3D must have dimensions (num_points, 3)");   // reference: rasterize_points.cu:69-71
     }
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor");
-    const c10::cuda::CUDAGuard guard(means3D.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    const DeviceStream on(means3D);
 
     const int P = means3D.size(0);
     const int H = image_height, W = image_width;
@@ -144,7 +184,7 @@ forward_impl(const torch::Tensor& bg_image, const torch::Tensor& sh_rest, const 
     const auto bgi_c = background_image(bg_image, means3D, H, W);
     fdgs_forward_result r;
     check(fdgs_forward_bg(&a, fptr(bgi_c), resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer,
-                          (void*)stream, &r),
+                          (void*)on.stream, &r),
           "forward");
 
     torch::Tensor covs3D_com;
@@ -159,52 +199,45 @@ forward_impl(const torch::Tensor& bg_image, const torch::Tensor& sh_rest, const 
 }
 
 // the reference's entry point: 30 positional arguments, 11-tuple (rasterize_points.h:18-49)
-ForwardOut RasterizeGaussiansCUDA(FDGS_FWD_PARAMS) { return forward_impl(torch::Tensor(), torch::Tensor(), false, FDGS_FWD_ARGS); }
-
-// the same + a per-pixel background image bg_image [3,H,W] (include/fdgs.h: fdgs_forward_bg; empty = none)
-ForwardOut RasterizeGaussiansBg(FDGS_FWD_PARAMS, const torch::Tensor& bg_image) {
-    return forward_impl(bg_image, torch::Tensor(), false, FDGS_FWD_ARGS);
+ForwardOut RasterizeGaussiansCUDA(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors,
+                                  const torch::Tensor& flows, const torch::Tensor& opacity, const torch::Tensor& ts,
+                                  const torch::Tensor& scales, const torch::Tensor& scales_t, const torch::Tensor& rotations,
+                                  const torch::Tensor& rotations_r, const float scale_modifier,
+                                  const torch::Tensor& cov3D_precomp, const float prefilter_var,
+                                  const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx,
+                                  const float tan_fovy, const int image_height, const int image_width,
+                                  const torch::Tensor& sh, const int degree, const int degree_t, const torch::Tensor& campos,
+                                  const float timestamp, const float time_duration, const bool rot_4d,
+                                  const int gaussian_dim, const bool force_sh_3d, const bool prefiltered, const bool debug) {
+    return RasterizeGaussiansExt(background, means3D, colors, flows, opacity, ts, scales, scales_t, rotations, rotations_r,
+                                 scale_modifier, cov3D_precomp, prefilter_var, viewmatrix, projmatrix, tan_fovx, tan_fovy,
+                                 image_height, image_width, sh, degree, degree_t, campos, timestamp, time_duration, rot_4d,
+                                 gaussian_dim, force_sh_3d, prefiltered, debug, torch::Tensor(), false, torch::Tensor());
 }
 
-// raw-parameter entry: the same 30 arguments (scales = log-scales, rotations un-normalised, opacity = logits when
-// raw_params) + the second SH tensor (sh = features_dc [P,1,3], sh_rest = features_rest [P,M-1,3]; may be empty)
-ForwardOut RasterizeGaussiansRaw(FDGS_FWD_PARAMS, const torch::Tensor& sh_rest, const bool raw_params) {
-    return forward_impl(torch::Tensor(), sh_rest, raw_params, FDGS_FWD_ARGS);
-}
-
-ForwardOut RasterizeGaussiansRawBg(FDGS_FWD_PARAMS, const torch::Tensor& sh_rest, const bool raw_params,
-                                   const torch::Tensor& bg_image) {
-    return forward_impl(bg_image, sh_rest, raw_params, FDGS_FWD_ARGS);
-}
-
-namespace {
-struct BackwardOut {
-    torch::Tensor dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dflows, dL_dts, dL_dscales,
-        dL_dscales_t, dL_drotations, dL_drotations_r, sh_factors, dL_dsh_rest, dL_dbg_image;
-};
-}  // namespace
-
-// sh_factor_mode: view-parallel mode -- no dL_dsh rows, the [P,3] colour factors instead (include/fdgs.h: sh_factors)
-static BackwardOut
-backward_impl(const torch::Tensor& bg_image, const bool want_dbg, const bool sh_factor_mode, const torch::Tensor& sh_rest,
-                               const bool raw_params,
-                               const torch::Tensor& background, const torch::Tensor& means3D,
-                               const torch::Tensor& out_means3D, const torch::Tensor& radii, const torch::Tensor& colors,
-                               const torch::Tensor& flows_2d, const torch::Tensor& opacities, const torch::Tensor& ts,
-                               const torch::Tensor& scales, const torch::Tensor& scales_t, const torch::Tensor& rotations,
-                               const torch::Tensor& rotations_r, const float scale_modifier,
-                               const torch::Tensor& cov3D_precomp, const float prefilter_var,
-                               const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx,
-                               const float tan_fovy, const torch::Tensor& dL_dout_color,
-                               const torch::Tensor& dL_dout_depth, const torch::Tensor& dL_dout_mask,
-                               const torch::Tensor& dL_dout_flow, const torch::Tensor& sh, const int degree,
-                               const int degree_t, const torch::Tensor& campos, const float timestamp,
-                               const float time_duration, const bool rot_4d, const int gaussian_dim,
-                               const bool force_sh_3d, const torch::Tensor& geomBuffer, const int R,
-                               const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer, const bool debug) {
+// The reference's 37 arguments (rasterize_points.h:51-89) + the forward's sh_rest, raw_params and bg_image, and:
+//   sh_factor_mode: the view-parallel mode -- no dL_dsh rows, the [P,3] colour factors instead (include/fdgs.h: sh_factors)
+//   want_dbg:       whether dL/dbg_image is wanted (fdgs_backward_bg)
+// Returns 15 tensors: the 12 gradients (w.r.t. the raw parameters under raw_params; dL_dsh is [P,1,3] when sh_rest is
+// given), sh_factors [P,3], dL_dsh_rest [P,M-1,3] and dL_dbg_image [3,H,W]; a tensor not asked for comes back empty.
+std::vector<torch::Tensor>
+RasterizeGaussiansBackwardExt(const torch::Tensor& background, const torch::Tensor& means3D,
+                              const torch::Tensor& out_means3D, const torch::Tensor& radii, const torch::Tensor& colors,
+                              const torch::Tensor& flows_2d, const torch::Tensor& opacities, const torch::Tensor& ts,
+                              const torch::Tensor& scales, const torch::Tensor& scales_t, const torch::Tensor& rotations,
+                              const torch::Tensor& rotations_r, const float scale_modifier,
+                              const torch::Tensor& cov3D_precomp, const float prefilter_var,
+                              const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx,
+                              const float tan_fovy, const torch::Tensor& dL_dout_color, const torch::Tensor& dL_dout_depth,
+                              const torch::Tensor& dL_dout_mask, const torch::Tensor& dL_dout_flow, const torch::Tensor& sh,
+                              const int degree, const int degree_t, const torch::Tensor& campos, const float timestamp,
+                              const float time_duration, const bool rot_4d, const int gaussian_dim,
+                              const bool force_sh_3d, const torch::Tensor& geomBuffer, const int R,
+                              const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer, const bool debug,
+                              const torch::Tensor& sh_rest, const bool raw_params, const torch::Tensor& bg_image,
+                              const bool sh_factor_mode, const bool want_dbg) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor");
-    const c10::cuda::CUDAGuard guard(means3D.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    const DeviceStream on(means3D);
     const int P = means3D.size(0);
     const int H = dL_dout_color.size(1), W = dL_dout_color.size(2);
     const bool split = sh_rest.defined() && sh_rest.numel() != 0;
@@ -271,90 +304,50 @@ backward_impl(const torch::Tensor& bg_image, const bool want_dbg, const bool sh_
         a.dL_dts = dL_dts.data_ptr<float>(); a.dL_dscale = dL_dscales.data_ptr<float>();
         a.dL_dscale_t = dL_dscales_t.data_ptr<float>(); a.dL_drot = dL_drotations.data_ptr<float>();
         a.dL_drot_r = dL_drotations_r.data_ptr<float>();
-        check(fdgs_backward_bg(&a, fptr(bgi_c), want_dbg ? dL_dbg_image.data_ptr<float>() : nullptr, (void*)stream),
+        check(fdgs_backward_bg(&a, fptr(bgi_c), want_dbg ? dL_dbg_image.data_ptr<float>() : nullptr, (void*)on.stream),
               "backward");
     }
-    return BackwardOut{dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dflows, dL_dts,
-                       dL_dscales, dL_dscales_t, dL_drotations, dL_drotations_r, sh_factors, dL_dsh_rest, dL_dbg_image};
+    return {dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dflows, dL_dts, dL_dscales,
+            dL_dscales_t, dL_drotations, dL_drotations_r, sh_factors, dL_dsh_rest, dL_dbg_image};
 }
-
-#define FDGS_BWD_PARAMS                                                                                                \
-    const torch::Tensor &background, const torch::Tensor &means3D, const torch::Tensor &out_means3D,                  \
-        const torch::Tensor &radii, const torch::Tensor &colors, const torch::Tensor &flows_2d,                        \
-        const torch::Tensor &opacities, const torch::Tensor &ts, const torch::Tensor &scales,                          \
-        const torch::Tensor &scales_t, const torch::Tensor &rotations, const torch::Tensor &rotations_r,               \
-        const float scale_modifier, const torch::Tensor &cov3D_precomp, const float prefilter_var,                     \
-        const torch::Tensor &viewmatrix, const torch::Tensor &projmatrix, const float tan_fovx, const float tan_fovy,  \
-        const torch::Tensor &dL_dout_color, const torch::Tensor &dL_dout_depth, const torch::Tensor &dL_dout_mask,     \
-        const torch::Tensor &dL_dout_flow, const torch::Tensor &sh, const int degree, const int degree_t,              \
-        const torch::Tensor &campos, const float timestamp, const float time_duration, const bool rot_4d,              \
-        const int gaussian_dim, const bool force_sh_3d, const torch::Tensor &geomBuffer, const int R,                  \
-        const torch::Tensor &binningBuffer, const torch::Tensor &imageBuffer, const bool debug
-#define FDGS_BWD_ARGS                                                                                                  \
-    background, means3D, out_means3D, radii, colors, flows_2d, opacities, ts, scales, scales_t, rotations, rotations_r, \
-        scale_modifier, cov3D_precomp, prefilter_var, viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color,       \
-        dL_dout_depth, dL_dout_mask, dL_dout_flow, sh, degree, degree_t, campos, timestamp, time_duration, rot_4d,     \
-        gaussian_dim, force_sh_3d, geomBuffer, R, binningBuffer, imageBuffer, debug
 
 // the reference's entry point: 37 positional arguments, 12 gradients (rasterize_points.h:51-89)
 std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor,
            torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
-RasterizeGaussiansBackwardCUDA(FDGS_BWD_PARAMS) {
-    BackwardOut o = backward_impl(torch::Tensor(), false, false, torch::Tensor(), false, FDGS_BWD_ARGS);
-    return std::make_tuple(o.dL_dmeans2D, o.dL_dcolors, o.dL_dopacity, o.dL_dmeans3D, o.dL_dcov3D, o.dL_dsh, o.dL_dflows,
-                           o.dL_dts, o.dL_dscales, o.dL_dscales_t, o.dL_drotations, o.dL_drotations_r);
-}
-
-// view-parallel variant: same arguments; dL_dsh comes back EMPTY and a 13th tensor holds the [P,3] colour factors
-std::vector<torch::Tensor> RasterizeGaussiansBackwardFactors(FDGS_BWD_PARAMS) {
-    BackwardOut o = backward_impl(torch::Tensor(), false, true, torch::Tensor(), false, FDGS_BWD_ARGS);
-    return {o.dL_dmeans2D, o.dL_dcolors, o.dL_dopacity, o.dL_dmeans3D, o.dL_dcov3D, o.dL_dsh, o.dL_dflows,
-            o.dL_dts, o.dL_dscales, o.dL_dscales_t, o.dL_drotations, o.dL_drotations_r, o.sh_factors};
-}
-
-// per-pixel background image (include/fdgs.h: fdgs_backward_bg): the 37 arguments + the forward's bg_image (empty =
-// none), the view-parallel switch of rasterize_gaussians_backward_factors and whether dL/dbg_image is wanted.  Returns
-// the 12 gradients, the [P,3] colour factors (sh_factor_mode, else empty) and dL_dbg_image [3,H,W] (else empty).
-std::vector<torch::Tensor> RasterizeGaussiansBackwardBg(FDGS_BWD_PARAMS, const torch::Tensor& bg_image, const bool sh_factor_mode,
-                                                        const bool want_dbg) {
-    BackwardOut o = backward_impl(bg_image, want_dbg, sh_factor_mode, torch::Tensor(), false, FDGS_BWD_ARGS);
-    return {o.dL_dmeans2D, o.dL_dcolors, o.dL_dopacity, o.dL_dmeans3D, o.dL_dcov3D, o.dL_dsh, o.dL_dflows, o.dL_dts,
-            o.dL_dscales, o.dL_dscales_t, o.dL_drotations, o.dL_drotations_r, o.sh_factors, o.dL_dbg_image};
-}
-
-// raw-parameter entry (see RasterizeGaussiansRaw): 14 tensors -- the 12 gradients (w.r.t. the RAW parameters when
-// raw_params; dL_dsh is [P,1,3] when sh_rest is given), the [P,3] colour factors (sh_factor_mode, else empty) and
-// dL_dsh_rest [P,M-1,3] (split rows, else empty)
-std::vector<torch::Tensor> RasterizeGaussiansBackwardRaw(FDGS_BWD_PARAMS, const torch::Tensor& sh_rest, const bool raw_params,
-                                                         const bool sh_factor_mode) {
-    BackwardOut o = backward_impl(torch::Tensor(), false, sh_factor_mode, sh_rest, raw_params, FDGS_BWD_ARGS);
-    return {o.dL_dmeans2D, o.dL_dcolors, o.dL_dopacity, o.dL_dmeans3D, o.dL_dcov3D, o.dL_dsh, o.dL_dflows,
-            o.dL_dts, o.dL_dscales, o.dL_dscales_t, o.dL_drotations, o.dL_drotations_r, o.sh_factors, o.dL_dsh_rest};
-}
-
-// the raw entry's 40 arguments + bg_image and want_dbg: its 14 tensors, then dL_dbg_image [3,H,W] (else empty)
-std::vector<torch::Tensor> RasterizeGaussiansBackwardRawBg(FDGS_BWD_PARAMS, const torch::Tensor& sh_rest, const bool raw_params,
-                                                           const bool sh_factor_mode, const torch::Tensor& bg_image,
-                                                           const bool want_dbg) {
-    BackwardOut o = backward_impl(bg_image, want_dbg, sh_factor_mode, sh_rest, raw_params, FDGS_BWD_ARGS);
-    return {o.dL_dmeans2D, o.dL_dcolors, o.dL_dopacity, o.dL_dmeans3D, o.dL_dcov3D, o.dL_dsh, o.dL_dflows, o.dL_dts,
-            o.dL_dscales, o.dL_dscales_t, o.dL_drotations, o.dL_drotations_r, o.sh_factors, o.dL_dsh_rest, o.dL_dbg_image};
+RasterizeGaussiansBackwardCUDA(const torch::Tensor& background, const torch::Tensor& means3D,
+                               const torch::Tensor& out_means3D, const torch::Tensor& radii, const torch::Tensor& colors,
+                               const torch::Tensor& flows_2d, const torch::Tensor& opacities, const torch::Tensor& ts,
+                               const torch::Tensor& scales, const torch::Tensor& scales_t, const torch::Tensor& rotations,
+                               const torch::Tensor& rotations_r, const float scale_modifier,
+                               const torch::Tensor& cov3D_precomp, const float prefilter_var,
+                               const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx,
+                               const float tan_fovy, const torch::Tensor& dL_dout_color, const torch::Tensor& dL_dout_depth,
+                               const torch::Tensor& dL_dout_mask, const torch::Tensor& dL_dout_flow, const torch::Tensor& sh,
+                               const int degree, const int degree_t, const torch::Tensor& campos, const float timestamp,
+                               const float time_duration, const bool rot_4d, const int gaussian_dim,
+                               const bool force_sh_3d, const torch::Tensor& geomBuffer, const int R,
+                               const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer, const bool debug) {
+    const std::vector<torch::Tensor> o = RasterizeGaussiansBackwardExt(
+        background, means3D, out_means3D, radii, colors, flows_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
+        scale_modifier, cov3D_precomp, prefilter_var, viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color,
+        dL_dout_depth, dL_dout_mask, dL_dout_flow, sh, degree, degree_t, campos, timestamp, time_duration, rot_4d,
+        gaussian_dim, force_sh_3d, geomBuffer, R, binningBuffer, imageBuffer, debug, torch::Tensor(), false,
+        torch::Tensor(), false, false);
+    return std::make_tuple(o[0], o[1], o[2], o[3], o[4], o[5], o[6], o[7], o[8], o[9], o[10], o[11]);
 }
 
 // ---- environment-map sky (include/fdgs.h: fdgs_sky_forward / fdgs_sky_backward) -----------------------------------
 static fdgs_sky_args sky_args(const torch::Tensor& env_map, const torch::Tensor& c2w, const torch::Tensor& campos,
                               const double fl_x, const double fl_y, const double cx, const double cy, const double radius,
                               const int64_t H, const int64_t W) {
-    TORCH_CHECK(env_map.is_cuda() && env_map.scalar_type() == torch::kFloat32 && env_map.is_contiguous() && env_map.dim() == 3 &&
-                env_map.size(0) == 3, "fdgs: env_map must be a contiguous float32 CUDA tensor [3,Hm,Wm]");
-    TORCH_CHECK(c2w.is_cuda() && c2w.scalar_type() == torch::kFloat32 && c2w.is_contiguous() && c2w.numel() == 16 &&
-                campos.is_cuda() && campos.scalar_type() == torch::kFloat32 && campos.is_contiguous() && campos.numel() == 3,
-                "fdgs: c2w [4,4] / campos [3] must be contiguous float32 CUDA tensors");
-    TORCH_CHECK(c2w.device() == env_map.device() && campos.device() == env_map.device(), "fdgs: sky inputs on different devices");
     fdgs_sky_args a;
     memset(&a, 0, sizeof(a));
-    a.env_map = env_map.data_ptr<float>(); a.env_height = (int)env_map.size(1); a.env_width = (int)env_map.size(2);
-    a.c2w = c2w.data_ptr<float>(); a.campos = campos.data_ptr<float>();
+    a.env_map = arg<float>(env_map, "env_map", 3, -1, REQUIRED);
+    TORCH_CHECK(env_map.dim() == 3, "fdgs: env_map must be [3,Hm,Wm]");
+    a.c2w = arg<float>(c2w, "c2w", -1, 16, REQUIRED);
+    a.campos = arg<float>(campos, "campos", -1, 3, REQUIRED);
+    same_cuda_device("sky", {env_map, c2w, campos});
+    a.env_height = (int)env_map.size(1); a.env_width = (int)env_map.size(2);
     a.fl_x = (float)fl_x; a.fl_y = (float)fl_y; a.cx = (float)cx; a.cy = (float)cy; a.radius = (float)radius;
     a.width = (int)W; a.height = (int)H;
     return a;
@@ -365,11 +358,10 @@ std::tuple<torch::Tensor, torch::Tensor> SkyForward(const torch::Tensor& env_map
                                                     const double fl_x, const double fl_y, const double cx, const double cy,
                                                     const double radius, const int64_t H, const int64_t W) {
     const fdgs_sky_args a = sky_args(env_map, c2w, campos, fl_x, fl_y, cx, cy, radius, H, W);
-    const c10::cuda::CUDAGuard guard(env_map.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    const DeviceStream on(env_map);
     torch::Tensor sky = torch::empty({3, H, W}, env_map.options());
     torch::Tensor miss = torch::zeros({1}, env_map.options().dtype(torch::kInt32));
-    check(fdgs_sky_forward(&a, sky.data_ptr<float>(), miss.data_ptr<int>(), (void*)stream), "sky_forward");
+    check(fdgs_sky_forward(&a, sky.data_ptr<float>(), miss.data_ptr<int>(), (void*)on.stream), "sky_forward");
     return std::make_tuple(sky, miss);
 }
 
@@ -380,11 +372,10 @@ torch::Tensor SkyBackward(const torch::Tensor& env_map, const torch::Tensor& c2w
     TORCH_CHECK(dL_dsky.is_cuda() && dL_dsky.scalar_type() == torch::kFloat32 && dL_dsky.dim() == 3 && dL_dsky.size(0) == 3,
                 "fdgs: dL_dsky must be a float32 CUDA tensor [3,H,W]");
     const fdgs_sky_args a = sky_args(env_map, c2w, campos, fl_x, fl_y, cx, cy, radius, dL_dsky.size(1), dL_dsky.size(2));
-    const c10::cuda::CUDAGuard guard(env_map.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    const DeviceStream on(env_map);
     const auto g = dL_dsky.contiguous();
     torch::Tensor denv = torch::zeros_like(env_map);
-    check(fdgs_sky_backward(&a, g.data_ptr<float>(), denv.data_ptr<float>(), (void*)stream), "sky_backward");
+    check(fdgs_sky_backward(&a, g.data_ptr<float>(), denv.data_ptr<float>(), (void*)on.stream), "sky_backward");
     return denv;
 }
 
@@ -397,24 +388,26 @@ void ShOuterSum(const torch::Tensor& table, const int64_t view_stride, const int
                 const bool rot_4d, const int64_t gaussian_dim, const bool force_sh_3d, const int64_t D, const int64_t D_t,
                 std::vector<torch::Tensor> outs, const bool accumulate) {
     TORCH_CHECK(outs.size() == 1 || outs.size() == 2, "fdgs: one or two output tensors");
-    TORCH_CHECK(slot_of.is_cuda() && slot_of.scalar_type() == torch::kInt32 && slot_of.is_contiguous(), "fdgs: slot_of must be int32 CUDA");
     const int P = means3D.size(0);
-    for (auto& o : outs)
-        TORCH_CHECK(o.is_cuda() && o.scalar_type() == torch::kFloat32 && o.is_contiguous() && o.dim() == 3 && o.size(0) == P &&
-                    o.size(2) == 3, "fdgs: outputs must be contiguous float32 [P, m, 3] CUDA tensors");
-    const c10::cuda::CUDAGuard guard(means3D.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    const auto m_c = contig(means3D), ts_c = contig(ts), sc_c = contig(scales), sct_c = contig(scales_t),
-               rot_c = contig(rotations), rotr_c = contig(rotations_r), tb_c = contig(table);
     fdgs_sh_sum_args a;
     memset(&a, 0, sizeof(a));
+    a.slot_of = arg<int>(slot_of, "slot_of", -1, -1, REQUIRED);
+    for (auto& o : outs) {
+        arg<float>(o, "outputs", P, -1, REQUIRED);
+        TORCH_CHECK(o.dim() == 3 && o.size(2) == 3, "fdgs: outputs must be [P, m, 3]");
+    }
+    a.union_idx = reinterpret_cast<const long long*>(arg<int64_t>(union_idx, "union_idx", -1, K, REQUIRED));
+    std::vector<torch::Tensor> dev(outs);
+    dev.push_back(slot_of);
+    dev.push_back(union_idx);
+    same_cuda_device("sh_outer_sum", dev);
+    const DeviceStream on(means3D);
+    const auto m_c = contig(means3D), ts_c = contig(ts), sc_c = contig(scales), sct_c = contig(scales_t),
+               rot_c = contig(rotations), rotr_c = contig(rotations_r), tb_c = contig(table);
     a.P = P; a.V = (int)V; a.K = (int)K; a.table = fptr(tb_c); a.view_stride = view_stride; a.meta_off = meta_off;
-    TORCH_CHECK(union_idx.is_cuda() && union_idx.scalar_type() == torch::kInt64 && union_idx.is_contiguous() &&
-                union_idx.numel() == K, "fdgs: union_idx must be int64 CUDA [K]");
     torch::Tensor dirs = torch::empty({std::max<int64_t>(V * K * 8, 1)}, means3D.options().dtype(torch::kFloat32));
-    a.union_idx = reinterpret_cast<const long long*>(union_idx.data_ptr<int64_t>());
     a.dir_scratch = dirs.data_ptr<float>();
-    a.slot_of = slot_of.data_ptr<int>(); a.means3D = fptr(m_c); a.ts = fptr(ts_c); a.scales = fptr(sc_c);
+    a.means3D = fptr(m_c); a.ts = fptr(ts_c); a.scales = fptr(sc_c);
     a.scales_t = fptr(sct_c); a.rotations = fptr(rot_c); a.rotations_r = fptr(rotr_c);
     a.scale_modifier = (float)scale_modifier; a.time_duration = (float)time_duration; a.rot_4d = rot_4d;
     a.gaussian_dim = (int)gaussian_dim; a.force_sh_3d = force_sh_3d; a.D = (int)D; a.D_t = (int)D_t;
@@ -424,20 +417,19 @@ void ShOuterSum(const torch::Tensor& table, const int64_t view_stride, const int
     a.out1 = outs.size() == 2 ? outs[1].data_ptr<float>() : nullptr;
     a.accumulate = accumulate;
     if (V > 0) TORCH_CHECK(tb_c.numel() >= V * view_stride, "fdgs: factor table too small");
-    check(fdgs_sh_outer_sum(&a, (void*)stream), "sh_outer_sum");
+    check(fdgs_sh_outer_sum(&a, (void*)on.stream), "sh_outer_sum");
 }
 
 // (slot_of int32 [P], idx int64 [K]) from the radii, their inclusive prefix sum cs and K = cs[-1] (known to the host)
 std::tuple<torch::Tensor, torch::Tensor> UnionMaps(const torch::Tensor& radii, const torch::Tensor& cs, const int64_t K) {
-    TORCH_CHECK(radii.is_cuda() && radii.scalar_type() == torch::kInt32 && radii.is_contiguous() && cs.is_cuda() &&
-                cs.scalar_type() == torch::kInt32 && cs.is_contiguous() && cs.numel() == radii.numel(),
-                "fdgs: radii / cs must be contiguous int32 CUDA tensors of equal length");
-    const c10::cuda::CUDAGuard guard(radii.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    const int* r = arg<int>(radii, "radii", -1, -1, REQUIRED);
+    const int* c = arg<int>(cs, "cs", -1, radii.numel(), REQUIRED);
+    same_cuda_device("union_maps", {radii, cs});
+    const DeviceStream on(radii);
     torch::Tensor slot_of = torch::empty_like(radii);
     torch::Tensor idx = torch::empty({K}, radii.options().dtype(torch::kInt64));
-    check(fdgs_union_maps(radii.numel(), radii.data_ptr<int>(), cs.data_ptr<int>(), slot_of.data_ptr<int>(),
-                          reinterpret_cast<long long*>(idx.data_ptr<int64_t>()), (void*)stream),
+    check(fdgs_union_maps(radii.numel(), r, c, slot_of.data_ptr<int>(), reinterpret_cast<long long*>(idx.data_ptr<int64_t>()),
+                          (void*)on.stream),
           "union_maps");
     return std::make_tuple(slot_of, idx);
 }
@@ -446,38 +438,34 @@ std::tuple<torch::Tensor, torch::Tensor> UnionMaps(const torch::Tensor& radii, c
 void ViewStats(const torch::Tensor& viewspace_grad, const torch::Tensor& radii, torch::Tensor& grad_norm_sum,
                torch::Tensor& visibility_count, torch::Tensor& max_radii) {
     const long long P = radii.numel();
-    TORCH_CHECK(viewspace_grad.is_cuda() && viewspace_grad.scalar_type() == torch::kFloat32 && viewspace_grad.is_contiguous() &&
-                viewspace_grad.dim() == 2 && viewspace_grad.size(0) == P && viewspace_grad.size(1) >= 2, "fdgs: viewspace_grad must be [P,>=2] float32 CUDA");
-    TORCH_CHECK(radii.is_cuda() && radii.scalar_type() == torch::kInt32 && radii.is_contiguous(), "fdgs: radii must be int32 CUDA");
-    TORCH_CHECK(grad_norm_sum.is_contiguous() && grad_norm_sum.numel() == P && grad_norm_sum.scalar_type() == torch::kFloat32 &&
-                visibility_count.is_contiguous() && visibility_count.numel() == P && visibility_count.scalar_type() == torch::kFloat32 &&
-                max_radii.is_contiguous() && max_radii.numel() == P && max_radii.scalar_type() == torch::kInt32, "fdgs: statistics tensors");
-    const c10::cuda::CUDAGuard guard(radii.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    check(fdgs_view_stats(P, viewspace_grad.data_ptr<float>(), (int)viewspace_grad.size(1), radii.data_ptr<int>(),
-                          grad_norm_sum.data_ptr<float>(), visibility_count.data_ptr<float>(), max_radii.data_ptr<int>(), (void*)stream),
-          "view_stats");
+    const float* vg = arg<float>(viewspace_grad, "viewspace_grad", P, -1, REQUIRED);
+    TORCH_CHECK(viewspace_grad.dim() == 2 && viewspace_grad.size(1) >= 2, "fdgs: viewspace_grad must be [P, >= 2]");
+    const int* r = arg<int>(radii, "radii", -1, -1, REQUIRED);
+    float* gn = arg<float>(grad_norm_sum, "grad_norm_sum", -1, P, REQUIRED);
+    float* vc = arg<float>(visibility_count, "visibility_count", -1, P, REQUIRED);
+    int* mr = arg<int>(max_radii, "max_radii", -1, P, REQUIRED);
+    same_cuda_device("view_stats", {viewspace_grad, radii});
+    const DeviceStream on(radii);
+    check(fdgs_view_stats(P, vg, (int)viewspace_grad.size(1), r, gn, vc, mr, (void*)on.stream), "view_stats");
 }
 
 // 1-element int32 tensor, non-zero if a row of `tensors` outside radii > 0 is not all-zero (sparse-exchange guard)
 torch::Tensor CheckRowsZero(std::vector<torch::Tensor> tensors, const torch::Tensor& radii) {
     TORCH_CHECK((int)tensors.size() <= FDGS_MAX_PACK, "fdgs: too many tensors");
-    TORCH_CHECK(radii.is_cuda() && radii.scalar_type() == torch::kInt32 && radii.is_contiguous(), "fdgs: radii must be int32 CUDA");
+    const int* r = arg<int>(radii, "radii", -1, -1, REQUIRED);
+    same_cuda_device("check_rows_zero", {radii});
     torch::Tensor flag = torch::zeros({1}, radii.options());
     const long long P = radii.numel();
     if (tensors.empty() || P == 0) return flag;
     std::vector<const float*> ptr;
     std::vector<int> widths;
     for (const auto& t : tensors) {
-        TORCH_CHECK(t.is_cuda() && t.scalar_type() == torch::kFloat32 && t.is_contiguous() && t.size(0) == P,
-                    "fdgs: gradient tensors must be contiguous float32 CUDA tensors with P rows");
-        ptr.push_back(t.data_ptr<float>());
+        ptr.push_back(arg<float>(t, "gradient tensor", P, -1, REQUIRED));
         widths.push_back((int)(t.numel() / P));
     }
-    const c10::cuda::CUDAGuard guard(radii.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    check(fdgs_check_rows_zero((int)ptr.size(), ptr.data(), widths.data(), P, radii.data_ptr<int>(), flag.data_ptr<int>(),
-                               (void*)stream),
+    same_cuda_device("check_rows_zero", tensors);
+    const DeviceStream on(radii);
+    check(fdgs_check_rows_zero((int)ptr.size(), ptr.data(), widths.data(), P, r, flag.data_ptr<int>(), (void*)on.stream),
           "check_rows_zero");
     return flag;
 }
@@ -486,11 +474,10 @@ torch::Tensor markVisible(torch::Tensor& means3D, torch::Tensor& viewmatrix, tor
     const int P = means3D.size(0);
     torch::Tensor present = torch::full({P}, false, means3D.options().dtype(at::kBool));
     if (P != 0) {
-        const c10::cuda::CUDAGuard guard(means3D.device());
-        cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+        const DeviceStream on(means3D);
         const auto m = means3D.contiguous(), v = viewmatrix.contiguous(), pr = projmatrix.contiguous();
         check(fdgs_mark_visible(P, m.data_ptr<float>(), v.data_ptr<float>(), pr.data_ptr<float>(),
-                                reinterpret_cast<unsigned char*>(present.data_ptr<bool>()), (void*)stream),
+                                reinterpret_cast<unsigned char*>(present.data_ptr<bool>()), (void*)on.stream),
               "mark_visible");
     }
     return present;
@@ -499,8 +486,7 @@ torch::Tensor markVisible(torch::Tensor& means3D, torch::Tensor& viewmatrix, tor
 // Test hooks: private forward state as plain tensors (parity tests compare them with the oracle).
 std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
 DebugExportGeom(const torch::Tensor& geomBuffer, const int P) {
-    const c10::cuda::CUDAGuard guard(geomBuffer.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    const DeviceStream on(geomBuffer);
     auto f = geomBuffer.options().dtype(torch::kFloat32);
     torch::Tensor depths = torch::zeros({P}, f), means2D = torch::zeros({P, 2}, f), conic = torch::zeros({P, 4}, f),
                   rgb = torch::zeros({P, 3}, f);
@@ -510,7 +496,7 @@ DebugExportGeom(const torch::Tensor& geomBuffer, const int P) {
         check(fdgs_debug_export_geom(reinterpret_cast<const char*>(geomBuffer.data_ptr()), P, depths.data_ptr<float>(),
                                      means2D.data_ptr<float>(), conic.data_ptr<float>(), rgb.data_ptr<float>(),
                                      clamped.data_ptr<uint8_t>(), reinterpret_cast<unsigned int*>(tiles.data_ptr<int>()),
-                                     (void*)stream),
+                                     (void*)on.stream),
               "debug_export_geom");
     return std::make_tuple(depths, means2D, conic, rgb, clamped, tiles);
 }
@@ -518,8 +504,7 @@ DebugExportGeom(const torch::Tensor& geomBuffer, const int P) {
 std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> DebugExportBinning(const torch::Tensor& binningBuffer,
                                                                            const torch::Tensor& imgBuffer, const int R,
                                                                            const int W, const int H) {
-    const c10::cuda::CUDAGuard guard(imgBuffer.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    const DeviceStream on(imgBuffer);
     auto i32 = imgBuffer.options().dtype(torch::kInt32);
     const int tiles = ((W + 15) / 16) * ((H + 15) / 16);
     torch::Tensor point_list = torch::zeros({R}, i32), ranges = torch::zeros({tiles, 2}, i32),
@@ -528,7 +513,7 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> DebugExportBinning(const
                                     reinterpret_cast<const char*>(imgBuffer.data_ptr()), R, W, H,
                                     reinterpret_cast<unsigned int*>(point_list.data_ptr<int>()),
                                     reinterpret_cast<unsigned int*>(ranges.data_ptr<int>()),
-                                    reinterpret_cast<unsigned int*>(n_contrib.data_ptr<int>()), (void*)stream),
+                                    reinterpret_cast<unsigned int*>(n_contrib.data_ptr<int>()), (void*)on.stream),
           "debug_export_binning");
     return std::make_tuple(point_list, ranges, n_contrib);
 }
@@ -540,8 +525,8 @@ static std::vector<long long> block_offsets(const std::vector<torch::Tensor>& ts
     std::vector<long long> off;
     total = 0;
     for (const auto& t : ts) {
-        TORCH_CHECK(t.is_cuda() && t.scalar_type() == torch::kFloat32 && t.is_contiguous() && t.dim() >= 1,
-                    "fdgs: gradient tensors must be contiguous float32 CUDA tensors");
+        arg<float>(t, "gradient tensor", -1, -1, REQUIRED);
+        TORCH_CHECK(t.dim() >= 1, "fdgs: gradient tensor has the wrong shape");
         const long long w = t.size(0) > 0 ? t.numel() / t.size(0) : 0;
         TORCH_CHECK(w > 0, "fdgs: empty gradient tensor");
         widths.push_back((int)w);
@@ -553,19 +538,21 @@ static std::vector<long long> block_offsets(const std::vector<torch::Tensor>& ts
 
 torch::Tensor PackRows(std::vector<torch::Tensor> tensors, const torch::Tensor& idx) {
     TORCH_CHECK((int)tensors.size() <= FDGS_MAX_PACK, "fdgs: too many tensors");
-    TORCH_CHECK(idx.is_cuda() && idx.scalar_type() == torch::kInt64 && idx.is_contiguous(), "fdgs: idx must be int64 CUDA");
+    const long long* ip = reinterpret_cast<const long long*>(arg<int64_t>(idx, "idx", -1, -1, REQUIRED));
     const long long K = idx.numel();
     std::vector<int> widths;
     long long total = 0;
     std::vector<long long> off = block_offsets(tensors, K, widths, total);
+    std::vector<torch::Tensor> dev(tensors);
+    dev.push_back(idx);
+    same_cuda_device("pack_rows", dev);
     torch::Tensor flat = torch::empty({total}, idx.options().dtype(torch::kFloat32));
     if (K == 0 || tensors.empty()) return flat;
-    const c10::cuda::CUDAGuard guard(idx.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    const DeviceStream on(idx);
     std::vector<const float*> ptr;
     for (const auto& t : tensors) ptr.push_back(t.data_ptr<float>());
-    check(fdgs_pack_rows((int)tensors.size(), ptr.data(), widths.data(), off.data(), reinterpret_cast<const long long*>(idx.data_ptr<int64_t>()), K,
-                         flat.data_ptr<float>(), (void*)stream),
+    check(fdgs_pack_rows((int)tensors.size(), ptr.data(), widths.data(), off.data(), ip, K, flat.data_ptr<float>(),
+                         (void*)on.stream),
           "pack_rows");
     return flat;
 }
@@ -576,45 +563,44 @@ void UnpackRows(const torch::Tensor& flat, std::vector<torch::Tensor> tensors, c
     std::vector<int> widths;
     long long total = 0;
     std::vector<long long> off = block_offsets(tensors, K, widths, total);
-    TORCH_CHECK(flat.numel() == total && flat.is_contiguous() && flat.scalar_type() == torch::kFloat32, "fdgs: flat buffer mismatch");
+    float* fp = arg<float>(flat, "flat buffer", -1, total, REQUIRED);
+    same_cuda_device("unpack_rows", tensors);
     if (K == 0 || tensors.empty()) return;
-    const c10::cuda::CUDAGuard guard(idx.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    const DeviceStream on(idx);
     std::vector<float*> ptr;
     for (auto& t : tensors) ptr.push_back(t.data_ptr<float>());
-    check(fdgs_unpack_rows((int)tensors.size(), ptr.data(), widths.data(), off.data(), reinterpret_cast<const long long*>(idx.data_ptr<int64_t>()), K,
-                           flat.data_ptr<float>(), (void*)stream),
+    check(fdgs_unpack_rows((int)tensors.size(), ptr.data(), widths.data(), off.data(),
+                           reinterpret_cast<const long long*>(idx.data_ptr<int64_t>()), K, fp, (void*)on.stream),
           "unpack_rows");
 }
 
 // ---- fused L1 + SSIM (include/fdgs.h: fdgs_l1_ssim_forward / _backward) ------------------------------------------
 // returns (sums double[2] = {sum |x - y|, sum SSIM}, maps float[3,C,H,W])
 std::tuple<torch::Tensor, torch::Tensor> L1SsimForward(const torch::Tensor& x, const torch::Tensor& y) {
-    TORCH_CHECK(x.is_cuda() && y.is_cuda() && x.scalar_type() == torch::kFloat32 && y.scalar_type() == torch::kFloat32,
-                "fdgs: images must be float32 CUDA tensors");
+    TORCH_CHECK(x.scalar_type() == torch::kFloat32 && y.scalar_type() == torch::kFloat32,
+                "fdgs: images must be ", dtype_name(torch::kFloat32));
     TORCH_CHECK(x.dim() == 3 && x.sizes() == y.sizes(), "fdgs: images must be [C,H,W] of equal shape");
-    const c10::cuda::CUDAGuard guard(x.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    same_cuda_device("l1_ssim", {x, y});
+    const DeviceStream on(x);
     const auto xc = x.contiguous(), yc = y.contiguous();
     const int C = x.size(0), H = x.size(1), W = x.size(2);
     torch::Tensor sums = torch::empty({2}, x.options().dtype(torch::kFloat64));
     torch::Tensor maps = torch::empty({3, C, H, W}, x.options());
     check(fdgs_l1_ssim_forward(xc.data_ptr<float>(), yc.data_ptr<float>(), C, H, W, maps.data_ptr<float>(),
-                               sums.data_ptr<double>(), (void*)stream),
+                               sums.data_ptr<double>(), (void*)on.stream),
           "l1_ssim_forward");
     return std::make_tuple(sums, maps);
 }
 
 torch::Tensor L1SsimBackward(const torch::Tensor& x, const torch::Tensor& y, const torch::Tensor& maps,
                              const torch::Tensor& grad_scale, const double lambda_dssim) {
-    const c10::cuda::CUDAGuard guard(x.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    const DeviceStream on(x);
     const auto xc = x.contiguous(), yc = y.contiguous(), gs = grad_scale.to(torch::kFloat32).contiguous();
     const int C = x.size(0), H = x.size(1), W = x.size(2);
     torch::Tensor dx = torch::empty({C, H, W}, x.options());
     check(fdgs_l1_ssim_backward(xc.data_ptr<float>(), yc.data_ptr<float>(), C, H, W, maps.data_ptr<float>(),
                                 gs.numel() ? gs.data_ptr<float>() : nullptr, (float)lambda_dssim, dx.data_ptr<float>(),
-                                (void*)stream),
+                                (void*)on.stream),
           "l1_ssim_backward");
     return dx;
 }
@@ -632,48 +618,27 @@ void AdamStep(std::vector<torch::Tensor> params, std::vector<torch::Tensor> grad
     std::vector<int> widths;
     std::vector<float> lr;
     for (size_t i = 0; i < n; ++i) {
-        for (const torch::Tensor* t : {&params[i], &grads[i], &exp_avg[i], &exp_avg_sq[i]})
-            TORCH_CHECK(t->is_cuda() && t->scalar_type() == torch::kFloat32 && t->is_contiguous() && t->size(0) == P &&
-                        t->numel() == params[i].numel(), "fdgs: adam tensors must be contiguous float32 CUDA [P, ...]");
-        p.push_back(params[i].data_ptr<float>()); g.push_back(grads[i].data_ptr<float>());
-        m.push_back(exp_avg[i].data_ptr<float>()); v.push_back(exp_avg_sq[i].data_ptr<float>());
-        widths.push_back(P > 0 ? (int)(params[i].numel() / P) : 1);
+        const int64_t numel = params[i].numel();
+        p.push_back(arg<float>(params[i], "adam tensor", P, numel, REQUIRED));
+        g.push_back(arg<float>(grads[i], "adam tensor", P, numel, REQUIRED));
+        m.push_back(arg<float>(exp_avg[i], "adam tensor", P, numel, REQUIRED));
+        v.push_back(arg<float>(exp_avg_sq[i], "adam tensor", P, numel, REQUIRED));
+        widths.push_back(P > 0 ? (int)(numel / P) : 1);
         lr.push_back((float)lrs[i]);
     }
-    if (sparse) {
-        TORCH_CHECK(rows.is_cuda() && rows.scalar_type() == torch::kInt64 && rows.is_contiguous(), "fdgs: rows must be int64 CUDA");
-        if (rows.numel() == 0) return;
-    }
-    const c10::cuda::CUDAGuard guard(params[0].device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    check(fdgs_adam_step((int)n, p.data(), g.data(), m.data(), v.data(), widths.data(), lr.data(), P,
-                         sparse ? reinterpret_cast<const long long*>(rows.data_ptr<int64_t>()) : nullptr, sparse ? rows.numel() : 0,
-                         step, beta1, beta2, eps, zero_grad, (void*)stream),
+    const long long* rp = sparse ? reinterpret_cast<const long long*>(arg<int64_t>(rows, "rows", -1, -1, REQUIRED)) : nullptr;
+    std::vector<torch::Tensor> dev;
+    for (size_t i = 0; i < n; ++i) dev.insert(dev.end(), {params[i], grads[i], exp_avg[i], exp_avg_sq[i]});
+    if (sparse) dev.push_back(rows);
+    same_cuda_device("adam", dev);
+    if (sparse && rows.numel() == 0) return;
+    const DeviceStream on(params[0]);
+    check(fdgs_adam_step((int)n, p.data(), g.data(), m.data(), v.data(), widths.data(), lr.data(), P, rp,
+                         sparse ? rows.numel() : 0, step, beta1, beta2, eps, zero_grad, (void*)on.stream),
           "adam_step");
 }
 
 // ---- densification (include/fdgs.h: fdgs_densify_*, fdgs_reset_opacity) --------------------------------------------
-// An undefined or empty tensor is "not provided" (NULL; the C-ABI rejects a NULL it needs).  dtype, layout and shape are checked before the device, so a
-// malformed argument is rejected before any GPU work.
-static float* rows_ptr(const torch::Tensor& t, long long P, long long width, const char* name) {
-    if (!t.defined() || t.numel() == 0) return nullptr;
-    TORCH_CHECK(t.scalar_type() == torch::kFloat32, "fdgs: ", name, " must be float32");
-    TORCH_CHECK(t.is_contiguous(), "fdgs: ", name, " must be contiguous");
-    TORCH_CHECK(t.dim() >= 1 && t.size(0) == P && (width < 0 || t.numel() == P * width), "fdgs: ", name, " has the wrong shape");
-    return t.data_ptr<float>();
-}
-
-// after every tensor of a call passed rows_ptr: all of them on the CUDA device of the first
-static void same_cuda_device(std::initializer_list<const torch::Tensor*> ts) {
-    const torch::Tensor* first = nullptr;
-    for (const torch::Tensor* t : ts) {
-        if (!t->defined() || t->numel() == 0) continue;
-        TORCH_CHECK(t->is_cuda(), "fdgs: densification tensors must be CUDA tensors");
-        if (!first) first = t;
-        TORCH_CHECK(t->device() == first->device(), "fdgs: densification tensors on different devices");
-    }
-}
-
 // geo = [xyz, t, scaling, scaling_t, rotation, rotation_r, opacity]; stats = [xyz_gradient_accum, denom, max_radii2D];
 // thresholds = [max_grad, min_opacity, percent_dense * extent, 0.1 * extent, max_screen_size] (rounded to fp32 here,
 // as ATen rounds a Python scalar it compares an fp32 tensor with); flags = [N, gaussian_dim, rot_4d, prune_only,
@@ -689,17 +654,17 @@ static fdgs_densify_args densify_args(const std::vector<torch::Tensor>& geo, con
     a.use_max_screen_size = (int)flags[4];
     a.max_grad = (float)thr[0]; a.min_opacity = (float)thr[1]; a.dense_extent = (float)thr[2]; a.big_extent = (float)thr[3];
     a.max_screen_size = (float)thr[4];
-    a.xyz = rows_ptr(geo[0], P, 3, "xyz");
-    a.t = rows_ptr(geo[1], P, 1, "t");
-    a.scaling = rows_ptr(geo[2], P, 3, "scaling");
-    a.scaling_t = rows_ptr(geo[3], P, 1, "scaling_t");
-    a.rotation = rows_ptr(geo[4], P, 4, "rotation");
-    a.rotation_r = rows_ptr(geo[5], P, 4, "rotation_r");
-    a.opacity = rows_ptr(geo[6], P, 1, "opacity");
-    a.xyz_gradient_accum = rows_ptr(stats[0], P, 1, "xyz_gradient_accum");
-    a.denom = rows_ptr(stats[1], P, 1, "denom");
-    a.max_radii2D = rows_ptr(stats[2], P, 1, "max_radii2D");
-    same_cuda_device({&geo[0], &geo[1], &geo[2], &geo[3], &geo[4], &geo[5], &geo[6], &stats[0], &stats[1], &stats[2]});
+    a.xyz = arg<float>(geo[0], "xyz", P, 3 * P);
+    a.t = arg<float>(geo[1], "t", P, P);
+    a.scaling = arg<float>(geo[2], "scaling", P, 3 * P);
+    a.scaling_t = arg<float>(geo[3], "scaling_t", P, P);
+    a.rotation = arg<float>(geo[4], "rotation", P, 4 * P);
+    a.rotation_r = arg<float>(geo[5], "rotation_r", P, 4 * P);
+    a.opacity = arg<float>(geo[6], "opacity", P, P);
+    a.xyz_gradient_accum = arg<float>(stats[0], "xyz_gradient_accum", P, P);
+    a.denom = arg<float>(stats[1], "denom", P, P);
+    a.max_radii2D = arg<float>(stats[2], "max_radii2D", P, P);
+    same_cuda_device("densification", {geo[0], geo[1], geo[2], geo[3], geo[4], geo[5], geo[6], stats[0], stats[1], stats[2]});
     return a;
 }
 
@@ -707,12 +672,12 @@ std::tuple<torch::Tensor, torch::Tensor> DensifyPlan(const std::vector<torch::Te
                                                      const std::vector<double>& thr, const std::vector<int64_t>& flags) {
     fdgs_densify_args a = densify_args(geo, stats, thr, flags);
     TORCH_CHECK(geo[2].defined() && geo[2].is_cuda(), "fdgs: scaling must be a CUDA tensor");
-    const c10::cuda::CUDAGuard guard(geo[2].device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    const DeviceStream on(geo[2]);
     auto opts = geo[2].options();
     torch::Tensor scratch = torch::empty({(int64_t)fdgs_densify_scratch_bytes(a.P) + 16}, opts.dtype(torch::kByte));
     torch::Tensor totals = torch::empty({4}, opts.dtype(torch::kInt32));
-    check(fdgs_densify_plan(&a, reinterpret_cast<char*>(scratch.data_ptr()), totals.data_ptr<int>(), (void*)stream), "densify_plan");
+    check(fdgs_densify_plan(&a, reinterpret_cast<char*>(scratch.data_ptr()), totals.data_ptr<int>(), (void*)on.stream),
+          "densify_plan");
     return std::make_tuple(scratch, totals);
 }
 
@@ -729,37 +694,35 @@ void DensifyApply(const std::vector<torch::Tensor>& geo, const std::vector<torch
     a.num_tensors = (int)n;
     for (size_t i = 0; i < n; ++i) {
         const long long w = a.P > 0 ? srcs[i].numel() / a.P : 1;
-        a.src[i] = rows_ptr(srcs[i], a.P, w, "source row tensor");
-        a.dst[i] = rows_ptr(dsts[i], P_new, w, "destination row tensor");
+        a.src[i] = arg<float>(srcs[i], "source row tensor", a.P, a.P * w);
+        a.dst[i] = arg<float>(dsts[i], "destination row tensor", P_new, P_new * w);
         if (a.P == 0 || P_new == 0) { a.num_tensors = 0; break; }     // nothing to copy from or to
         TORCH_CHECK(a.src[i] && a.dst[i], "fdgs: densify tensor table entry missing");
         a.kind[i] = (int)kinds[i];
         a.width[i] = (int)w;
     }
     const long long SN = totals[2] * (long long)a.N;
-    a.samples = rows_ptr(samples, SN, a.rot_4d ? 4 : 3, "samples");
-    a.samples_t = rows_ptr(samples_t, SN, 1, "samples_t");
-    for (size_t i = 0; i < n; ++i) same_cuda_device({&geo[2], &srcs[i], &dsts[i]});
-    same_cuda_device({&geo[2], &samples, &samples_t});
+    a.samples = arg<float>(samples, "samples", SN, SN * (a.rot_4d ? 4 : 3));
+    a.samples_t = arg<float>(samples_t, "samples_t", SN, SN);
+    for (size_t i = 0; i < n; ++i) same_cuda_device("densification", {geo[2], srcs[i], dsts[i]});
+    same_cuda_device("densification", {geo[2], samples, samples_t});
     TORCH_CHECK(scratch.is_cuda() && scratch.scalar_type() == torch::kByte &&
                 scratch.numel() >= (int64_t)fdgs_densify_scratch_bytes(a.P), "fdgs: densify scratch of the plan required");
     int tot[4];
     for (int i = 0; i < 4; ++i) tot[i] = (int)totals[i];
-    const c10::cuda::CUDAGuard guard(scratch.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    check(fdgs_densify_apply(&a, reinterpret_cast<const char*>(scratch.data_ptr()), tot, (void*)stream), "densify_apply");
+    const DeviceStream on(scratch);
+    check(fdgs_densify_apply(&a, reinterpret_cast<const char*>(scratch.data_ptr()), tot, (void*)on.stream), "densify_apply");
 }
 
 void ResetOpacity(torch::Tensor& opacity, torch::Tensor& exp_avg, torch::Tensor& exp_avg_sq) {
     const long long P = opacity.size(0);
-    float* o = rows_ptr(opacity, P, 1, "opacity");
-    float* m = rows_ptr(exp_avg, P, 1, "exp_avg");
-    float* v = rows_ptr(exp_avg_sq, P, 1, "exp_avg_sq");
-    same_cuda_device({&opacity, &exp_avg, &exp_avg_sq});
+    float* o = arg<float>(opacity, "opacity", P, P);
+    float* m = arg<float>(exp_avg, "exp_avg", P, P);
+    float* v = arg<float>(exp_avg_sq, "exp_avg_sq", P, P);
+    same_cuda_device("densification", {opacity, exp_avg, exp_avg_sq});
     if (P == 0) return;
-    const c10::cuda::CUDAGuard guard(opacity.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    check(fdgs_reset_opacity(P, o, m, v, (void*)stream), "reset_opacity");
+    const DeviceStream on(opacity);
+    check(fdgs_reset_opacity(P, o, m, v, (void*)on.stream), "reset_opacity");
 }
 
 // batch_size 1: point_grad = viewspace_points.grad [P, >= 2], visibility_count empty; batch_size > 1: point_grad =
@@ -768,63 +731,42 @@ void DensifyStats(int64_t batch_size, const torch::Tensor& point_grad, const tor
                   const torch::Tensor& radii, const torch::Tensor& t_grad, torch::Tensor& xyz_gradient_accum, torch::Tensor& denom,
                   torch::Tensor& t_gradient_accum, torch::Tensor& max_radii2D) {
     const long long P = xyz_gradient_accum.size(0);
-    float* acc = rows_ptr(xyz_gradient_accum, P, 1, "xyz_gradient_accum");
-    float* den = rows_ptr(denom, P, 1, "denom");
-    float* tacc = rows_ptr(t_gradient_accum, P, 1, "t_gradient_accum");
-    float* mr = rows_ptr(max_radii2D, P, 1, "max_radii2D");
-    const float* tg = rows_ptr(t_grad, P, 1, "t_grad");
-    const float* vis = rows_ptr(visibility_count, P, 1, "visibility_count");
-    const float* pg = rows_ptr(point_grad, P, batch_size == 1 ? -1 : 1, "point_grad");
+    float* acc = arg<float>(xyz_gradient_accum, "xyz_gradient_accum", P, P);
+    float* den = arg<float>(denom, "denom", P, P);
+    float* tacc = arg<float>(t_gradient_accum, "t_gradient_accum", P, P);
+    float* mr = arg<float>(max_radii2D, "max_radii2D", P, P);
+    const float* tg = arg<float>(t_grad, "t_grad", P, P);
+    const float* vis = arg<float>(visibility_count, "visibility_count", P, P);
+    const float* pg = arg<float>(point_grad, "point_grad", P, batch_size == 1 ? -1 : P);
     TORCH_CHECK(point_grad.defined() && (batch_size > 1 || point_grad.dim() == 2), "fdgs: point_grad must be [P, >= 2] for one view");
-    TORCH_CHECK(radii.defined() && radii.scalar_type() == torch::kInt32 && radii.is_contiguous() && radii.numel() == P,
-                "fdgs: radii must be contiguous int32 [P]");
-    same_cuda_device({&xyz_gradient_accum, &denom, &t_gradient_accum, &max_radii2D, &t_grad, &visibility_count, &point_grad, &radii});
+    const int* r = arg<int>(radii, "radii", -1, P, REQUIRED);
+    same_cuda_device("densification",
+                     {xyz_gradient_accum, denom, t_gradient_accum, max_radii2D, t_grad, visibility_count, point_grad, radii});
     const int stride = batch_size == 1 ? (int)(point_grad.dim() == 2 ? point_grad.size(1) : 0) : 1;
     if (P == 0) return;
-    const c10::cuda::CUDAGuard guard(xyz_gradient_accum.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
-    check(fdgs_densify_stats(P, (int)batch_size, pg, stride, vis, radii.data_ptr<int>(), tg, acc, den, tacc, mr, (void*)stream),
+    const DeviceStream on(xyz_gradient_accum);
+    check(fdgs_densify_stats(P, (int)batch_size, pg, stride, vis, r, tg, acc, den, tacc, mr, (void*)on.stream),
           "densify_stats");
 }
 
 // ---- k nearest neighbours (include/fdgs.h: fdgs_knn) ---------------------------------------------------------------
 std::tuple<torch::Tensor, torch::Tensor> Knn(const torch::Tensor& xyz, const int64_t k, const bool brute_force) {
-    TORCH_CHECK(xyz.is_cuda() && xyz.scalar_type() == torch::kFloat32 && xyz.dim() == 2 && xyz.size(1) == 3,
-                "fdgs: xyz must be a float32 CUDA tensor [n,3]");
-    const c10::cuda::CUDAGuard guard(xyz.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    TORCH_CHECK(xyz.scalar_type() == torch::kFloat32, "fdgs: xyz must be ", dtype_name(torch::kFloat32));
+    TORCH_CHECK(xyz.dim() == 2 && xyz.size(1) == 3, "fdgs: xyz must be [n,3]");
+    TORCH_CHECK(xyz.is_cuda(), "fdgs: xyz must be a CUDA tensor");
+    const DeviceStream on(xyz);
     const auto x = xyz.contiguous();
     const int n = x.size(0);
     torch::Tensor idx = torch::empty({n, k}, x.options().dtype(torch::kInt32));
     torch::Tensor d2 = torch::empty({n, k}, x.options());
     torch::Tensor scratch = torch::empty({(int64_t)(brute_force ? 16 : fdgs_knn_scratch_bytes(n))}, x.options().dtype(torch::kByte));
     check(fdgs_knn(n, (int)k, x.data_ptr<float>(), reinterpret_cast<char*>(scratch.data_ptr()), idx.data_ptr<int>(),
-                   d2.data_ptr<float>(), brute_force, (void*)stream),
+                   d2.data_ptr<float>(), brute_force, (void*)on.stream),
           "knn");
     return std::make_tuple(idx, d2);
 }
 
 // ---- rigidity and motion regularisers (include/fdgs.h: fdgs_rigid_*) -----------------------------------------------
-// Every tensor is checked for dtype, layout, shape and device before the device is touched.  An undefined or empty
-// optional tensor is "not provided".
-static const void* rigid_ptr(const torch::Tensor& t, torch::ScalarType dtype, int64_t rows, int64_t numel, const char* name) {
-    TORCH_CHECK(t.defined(), "fdgs: ", name, " is required");
-    TORCH_CHECK(t.scalar_type() == dtype, "fdgs: ", name, " must be ", c10::toString(dtype));
-    TORCH_CHECK(t.is_contiguous(), "fdgs: ", name, " must be contiguous");
-    TORCH_CHECK(t.dim() >= 1 && t.size(0) == rows && t.numel() == numel, "fdgs: ", name, " has the wrong shape");
-    return t.data_ptr();
-}
-
-static void rigid_same_device(std::initializer_list<const torch::Tensor*> ts) {
-    const torch::Tensor* first = nullptr;
-    for (const torch::Tensor* t : ts) {
-        if (!t->defined() || t->numel() == 0) continue;
-        TORCH_CHECK(t->is_cuda(), "fdgs: regulariser tensors must be CUDA tensors");
-        if (!first) first = t;
-        TORCH_CHECK(t->device() == first->device(), "fdgs: regulariser tensors on different devices");
-    }
-}
-
 // params = [t [n,1], scaling [n,3], scaling_t [n,1], rotation [n,4], rotation_r [n,4]] (the raw parameters)
 static fdgs_rigid_args rigid_args(const std::vector<torch::Tensor>& params, int64_t k) {
     TORCH_CHECK(params.size() == 5, "fdgs: five parameter tensors (t, scaling, scaling_t, rotation, rotation_r)");
@@ -834,24 +776,18 @@ static fdgs_rigid_args rigid_args(const std::vector<torch::Tensor>& params, int6
     memset(&a, 0, sizeof(a));
     a.n = (int)n;
     a.k = (int)k;
-    a.t = static_cast<const float*>(rigid_ptr(params[0], torch::kFloat32, n, n, "t"));
-    a.scaling = static_cast<const float*>(rigid_ptr(params[1], torch::kFloat32, n, 3 * n, "scaling"));
-    a.scaling_t = static_cast<const float*>(rigid_ptr(params[2], torch::kFloat32, n, n, "scaling_t"));
-    a.rotation = static_cast<const float*>(rigid_ptr(params[3], torch::kFloat32, n, 4 * n, "rotation"));
-    a.rotation_r = static_cast<const float*>(rigid_ptr(params[4], torch::kFloat32, n, 4 * n, "rotation_r"));
+    a.t = arg<float>(params[0], "t", n, n, REQUIRED);
+    a.scaling = arg<float>(params[1], "scaling", n, 3 * n, REQUIRED);
+    a.scaling_t = arg<float>(params[2], "scaling_t", n, n, REQUIRED);
+    a.rotation = arg<float>(params[3], "rotation", n, 4 * n, REQUIRED);
+    a.rotation_r = arg<float>(params[4], "rotation_r", n, 4 * n, REQUIRED);
     return a;
 }
 
 static void rigid_list(fdgs_rigid_args& a, const torch::Tensor& idx, const torch::Tensor& weight) {
     const int64_t n = a.n, k = a.k;
-    a.idx = static_cast<const int*>(rigid_ptr(idx, torch::kInt32, n, n * k, "idx"));
-    a.weight = static_cast<const float*>(rigid_ptr(weight, torch::kFloat32, n, n * k, "weight"));
-}
-
-static const float* rigid_scalar(const torch::Tensor& g, const char* name) {
-    if (!g.defined() || g.numel() == 0) return nullptr;
-    TORCH_CHECK(g.scalar_type() == torch::kFloat32 && g.numel() == 1, "fdgs: ", name, " must be one float32 element");
-    return g.data_ptr<float>();
+    a.idx = arg<int>(idx, "idx", n, n * k, REQUIRED);
+    a.weight = arg<float>(weight, "weight", n, n * k, REQUIRED);
 }
 
 // (weight, in_offsets, in_edges) of fdgs_knn's (idx, dist2)
@@ -859,18 +795,17 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> RigidNeighbours(const to
     TORCH_CHECK(idx.defined() && idx.dim() == 2, "fdgs: idx must be [n,k]");
     const int64_t n = idx.size(0), k = idx.size(1);
     TORCH_CHECK(n > 0 && k >= 1 && k <= 32, "fdgs: bad n / k (n > 0, 1 <= k <= 32)");
-    const int* ip = static_cast<const int*>(rigid_ptr(idx, torch::kInt32, n, n * k, "idx"));
-    const float* dp = static_cast<const float*>(rigid_ptr(dist2, torch::kFloat32, n, n * k, "dist2"));
-    rigid_same_device({&idx, &dist2});
-    const c10::cuda::CUDAGuard guard(idx.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    const int* ip = arg<int>(idx, "idx", n, n * k, REQUIRED);
+    const float* dp = arg<float>(dist2, "dist2", n, n * k, REQUIRED);
+    same_cuda_device("regulariser", {idx, dist2});
+    const DeviceStream on(idx);
     auto opts = dist2.options();
     torch::Tensor weight = torch::empty({n, k}, opts);
     torch::Tensor in_offsets = torch::empty({n + 1}, opts.dtype(torch::kInt32));
     torch::Tensor in_edges = torch::empty({n * k}, opts.dtype(torch::kInt32));
     torch::Tensor scratch = torch::empty({(int64_t)fdgs_rigid_scratch_bytes((int)n, (int)k) + 256}, opts.dtype(torch::kByte));
     check(fdgs_rigid_neighbours((int)n, (int)k, ip, dp, reinterpret_cast<char*>(scratch.data_ptr()), weight.data_ptr<float>(),
-                                in_offsets.data_ptr<int>(), in_edges.data_ptr<int>(), (void*)stream),
+                                in_offsets.data_ptr<int>(), in_edges.data_ptr<int>(), (void*)on.stream),
           "rigid_neighbours");
     return std::make_tuple(weight, in_offsets, in_edges);
 }
@@ -881,10 +816,9 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> RigidForward(const std::
                                                                      const bool want_rigid, const bool want_motion) {
     fdgs_rigid_args a = rigid_args(params, k);
     if (want_rigid) rigid_list(a, idx, weight);
-    rigid_same_device({&params[0], &params[1], &params[2], &params[3], &params[4], &idx, &weight});
+    same_cuda_device("regulariser", {params[0], params[1], params[2], params[3], params[4], idx, weight});
     TORCH_CHECK(params[1].is_cuda(), "fdgs: regulariser tensors must be CUDA tensors");
-    const c10::cuda::CUDAGuard guard(params[1].device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    const DeviceStream on(params[1]);
     auto opts = params[1].options();
     torch::Tensor velocity = torch::empty({params[1].size(0), 3}, opts);
     torch::Tensor lr = want_rigid ? torch::empty({}, opts) : torch::zeros({}, opts);
@@ -893,7 +827,7 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> RigidForward(const std::
     torch::Tensor scratch = torch::empty({(int64_t)sb + 256}, opts.dtype(torch::kByte));
     a.velocity = velocity.data_ptr<float>();
     check(fdgs_rigid_forward(&a, reinterpret_cast<char*>(scratch.data_ptr()), want_rigid ? lr.data_ptr<float>() : nullptr,
-                             want_motion ? lm.data_ptr<float>() : nullptr, (void*)stream),
+                             want_motion ? lm.data_ptr<float>() : nullptr, (void*)on.stream),
           "rigid_forward");
     return std::make_tuple(velocity, lr, lm);
 }
@@ -906,23 +840,22 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor> RigidBack
     const torch::Tensor& grad_motion) {
     fdgs_rigid_args a = rigid_args(params, k);
     const int64_t n = a.n;
-    a.velocity = static_cast<float*>(const_cast<void*>(rigid_ptr(velocity, torch::kFloat32, n, 3 * n, "velocity")));
-    const float* gr = rigid_scalar(grad_rigid, "grad_rigid");
-    const float* gm = rigid_scalar(grad_motion, "grad_motion");
+    a.velocity = arg<float>(velocity, "velocity", n, 3 * n, REQUIRED);
+    const float* gr = arg<float>(grad_rigid, "grad_rigid", -1, 1);
+    const float* gm = arg<float>(grad_motion, "grad_motion", -1, 1);
     if (gr) {
         rigid_list(a, idx, weight);
-        a.in_offsets = static_cast<const int*>(rigid_ptr(in_offsets, torch::kInt32, n + 1, n + 1, "in_offsets"));
-        a.in_edges = static_cast<const int*>(rigid_ptr(in_edges, torch::kInt32, n * k, n * k, "in_edges"));
+        a.in_offsets = arg<int>(in_offsets, "in_offsets", n + 1, n + 1, REQUIRED);
+        a.in_edges = arg<int>(in_edges, "in_edges", n * k, n * k, REQUIRED);
     }
-    rigid_same_device({&params[0], &params[1], &params[2], &params[3], &params[4], &velocity, &idx, &weight, &in_offsets, &in_edges,
-                       &grad_rigid, &grad_motion});
+    same_cuda_device("regulariser", {params[0], params[1], params[2], params[3], params[4], velocity, idx, weight, in_offsets,
+                                     in_edges, grad_rigid, grad_motion});
     TORCH_CHECK(params[1].is_cuda(), "fdgs: regulariser tensors must be CUDA tensors");
-    const c10::cuda::CUDAGuard guard(params[1].device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    const DeviceStream on(params[1]);
     torch::Tensor ds = torch::empty_like(params[1]), dst = torch::empty_like(params[2]);
     torch::Tensor dr = torch::empty_like(params[3]), drr = torch::empty_like(params[4]);
     check(fdgs_rigid_backward(&a, gr, gm, ds.data_ptr<float>(), dst.data_ptr<float>(), dr.data_ptr<float>(), drr.data_ptr<float>(),
-                              (void*)stream),
+                              (void*)on.stream),
           "rigid_backward");
     return std::make_tuple(ds, dst, dr, drr);
 }
@@ -931,45 +864,34 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor> RigidBack
 // x, y: [B,C,H,W] float32 contiguous CUDA tensors; accum: float64 [5] on the same device, or empty = none.
 // Returns out [B,4] float64 (l1, psnr, ssim, msssim per view).  Checks dtype, layout and shape before the device.
 torch::Tensor ImageMetrics(const torch::Tensor& x, const torch::Tensor& y, const bool clamp, const torch::Tensor& accum) {
-    TORCH_CHECK(x.defined() && y.defined(), "fdgs: image_metrics needs two images");
-    TORCH_CHECK(x.scalar_type() == torch::kFloat32 && y.scalar_type() == torch::kFloat32, "fdgs: images must be Float (float32)");
-    TORCH_CHECK(x.is_contiguous() && y.is_contiguous(), "fdgs: images must be contiguous");
-    TORCH_CHECK(x.dim() == 4 && x.sizes() == y.sizes(), "fdgs: images must be [B,C,H,W] of equal shape");
-    const bool has_accum = accum.defined() && accum.numel() > 0;
-    if (has_accum) {
-        TORCH_CHECK(accum.scalar_type() == torch::kFloat64 && accum.is_contiguous() && accum.numel() == 5,
-                    "fdgs: accum must be a contiguous Double (float64) tensor of 5 elements");
-    }
-    TORCH_CHECK(x.is_cuda() && y.is_cuda() && x.device() == y.device() && (!has_accum || accum.device() == x.device()),
-                "fdgs: image_metrics tensors must be CUDA tensors on one device");
     fdgs_metrics_args a;
     memset(&a, 0, sizeof(a));
+    a.x = arg<float>(x, "images", -1, -1, REQUIRED);
+    a.y = arg<float>(y, "images", -1, -1, REQUIRED);
+    TORCH_CHECK(x.dim() == 4 && x.sizes() == y.sizes(), "fdgs: images must be [B,C,H,W] of equal shape");
+    a.accum = arg<double>(accum, "accum", -1, 5);
+    same_cuda_device("image_metrics", {x, y, accum});
     a.B = (int)x.size(0); a.C = (int)x.size(1); a.H = (int)x.size(2); a.W = (int)x.size(3);
     TORCH_CHECK(x.size(0) == a.B && x.size(1) == a.C && x.size(2) == a.H && x.size(3) == a.W, "fdgs: image size overflow");
     const size_t sb = fdgs_metrics_scratch_bytes(a.B, a.C, a.H, a.W);
-    const c10::cuda::CUDAGuard guard(x.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    const DeviceStream on(x);
     torch::Tensor out = torch::empty({x.size(0), 4}, x.options().dtype(torch::kFloat64));
     torch::Tensor scratch = torch::empty({(int64_t)sb}, x.options().dtype(torch::kByte));
-    a.x = x.data_ptr<float>();
-    a.y = y.data_ptr<float>();
     a.clamp = clamp ? 1 : 0;
     a.out = out.data_ptr<double>();
-    a.accum = has_accum ? accum.data_ptr<double>() : nullptr;
-    check(fdgs_image_metrics(&a, reinterpret_cast<char*>(scratch.data_ptr()), (void*)stream), "image_metrics");
+    check(fdgs_image_metrics(&a, reinterpret_cast<char*>(scratch.data_ptr()), (void*)on.stream), "image_metrics");
     return out;
 }
 
 std::tuple<torch::Tensor, torch::Tensor, torch::Tensor> DebugActivate(const torch::Tensor& log_s, const torch::Tensor& logit,
                                                                       const torch::Tensor& quat, const int64_t mode) {
-    const c10::cuda::CUDAGuard guard(log_s.device());
-    cudaStream_t stream = c10::cuda::getCurrentCUDAStream().stream();
+    const DeviceStream on(log_s);
     const auto a = log_s.contiguous(), b = logit.contiguous(), q = quat.contiguous();
     const int n = (int)a.numel();
     TORCH_CHECK(b.numel() == n && q.numel() == 4 * (int64_t)n, "fdgs: debug_activate shapes");
     torch::Tensor s = torch::empty_like(a), o = torch::empty_like(b), qo = torch::empty_like(q);
     check(fdgs_debug_activate(n, a.data_ptr<float>(), b.data_ptr<float>(), q.data_ptr<float>(), (int)mode, s.data_ptr<float>(),
-                              o.data_ptr<float>(), qo.data_ptr<float>(), (void*)stream),
+                              o.data_ptr<float>(), qo.data_ptr<float>(), (void*)on.stream),
           "debug_activate");
     return std::make_tuple(s, o, qo);
 }
@@ -992,13 +914,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("unpack_rows", &UnpackRows);
     m.def("rasterize_gaussians", &RasterizeGaussiansCUDA);
     m.def("rasterize_gaussians_backward", &RasterizeGaussiansBackwardCUDA);
-    m.def("rasterize_gaussians_backward_factors", &RasterizeGaussiansBackwardFactors);
-    m.def("rasterize_gaussians_raw", &RasterizeGaussiansRaw);
-    m.def("rasterize_gaussians_backward_raw", &RasterizeGaussiansBackwardRaw);
-    m.def("rasterize_gaussians_bg", &RasterizeGaussiansBg);
-    m.def("rasterize_gaussians_backward_bg", &RasterizeGaussiansBackwardBg);
-    m.def("rasterize_gaussians_raw_bg", &RasterizeGaussiansRawBg);
-    m.def("rasterize_gaussians_backward_raw_bg", &RasterizeGaussiansBackwardRawBg);
+    m.def("rasterize_gaussians_ext", &RasterizeGaussiansExt);
+    m.def("rasterize_gaussians_backward_ext", &RasterizeGaussiansBackwardExt);
     m.def("sky_forward", &SkyForward);
     m.def("sky_backward", &SkyBackward);
     m.def("sh_outer_sum", &ShOuterSum);

@@ -1,8 +1,10 @@
 """fdgs -- loader for the H100-native 4D Gaussian rasterizer libraries.
 
-`fdgs.C` is the torch extension module (`fdgs_C.so`) exposing exactly the reference's
+`fdgs.C` is the torch extension module (`fdgs_C.so`) exposing the reference's
 `_C.rasterize_gaussians / rasterize_gaussians_backward / mark_visible`
-(reference: diff-gaussian-rasterization/ext.cpp:15-19); `fdgs.lib()` is the raw C-ABI
+(reference: diff-gaussian-rasterization/ext.cpp:15-19), the extended pair
+`rasterize_gaussians_ext / rasterize_gaussians_backward_ext` (raw parameters, per-pixel background,
+view-parallel colour factors) and the training-step bindings; `fdgs.lib()` is the raw C-ABI
 (`libfdgs.so`, include/fdgs.h) through ctypes.
 
 There is NO fallback: if the CUDA libraries have not been built (run

@@ -1,8 +1,9 @@
 """In-tree build of the native pieces (explicit nvcc / g++ command lines, no JIT cache).
 
   libfdgs.so   the product: CUDA kernels + C-ABI (include/fdgs.h), sm_90a only
-  fdgs_C.so    thin torch extension over the C-ABI (same three entry points as the
-               reference's `_C`, reference: diff-gaussian-rasterization/ext.cpp:15-19)
+  fdgs_C.so    thin torch extension over the C-ABI (the three entry points of the reference's
+               `_C`, reference: diff-gaussian-rasterization/ext.cpp:15-19, their extended pair
+               rasterize_gaussians_ext / _backward_ext, and the training-step bindings)
 
 Both land in `4d-gaussian-splatting_b200/fdgs/lib/` (git-ignored).  Nothing here falls back to a CPU or PyTorch implementation: if the libraries are
 missing, importing `fdgs` raises.

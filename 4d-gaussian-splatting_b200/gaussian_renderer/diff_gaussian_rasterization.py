@@ -10,7 +10,11 @@ reference's `train.py` run unchanged.
 What differs is underneath: the reference JIT-compiles diff-gaussian-rasterization at import
 (`:17-28`); here `_C` is the prebuilt sm_90a extension `fdgs_C.so` sitting on the C-ABI of
 include/fdgs.h.  Importing this module fails loudly when that library has not been built --
-there is no PyTorch or CPU fallback path.
+there is no PyTorch or CPU fallback path.  Both entries (`GaussianRasterizer.forward` and the
+raw-parameter `forward_raw`) run through one autograd Function, which calls `_C.rasterize_gaussians_ext`
+and `_C.rasterize_gaussians_backward_ext`: the reference's 30 / 37 positional arguments followed by
+the extensions.  So under `debug` a failing call's snapshot holds that extended argument tuple; its
+first 30 (forward) or 37 (backward) entries are the reference's layout.
 """
 from typing import NamedTuple
 
@@ -20,6 +24,9 @@ from torch import nn
 import fdgs
 
 _C = fdgs.ext()
+
+# an empty tensor is "not provided" (a null pointer in C) everywhere in _C; never given a gradient or written to
+_NONE = torch.Tensor([])
 
 _SNAPSHOT_MSG = {
     "snapshot_fw.dump": "\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.",
@@ -93,31 +100,36 @@ class GaussianRasterizationSettings(NamedTuple):
 
 
 class _RasterizeGaussians(torch.autograd.Function):
-    """reference: :67-225.  Inputs, in order: means3D, means2D, sh, colors_precomp, flow_2d, opacities,
-    ts, scales, scales_t, rotations, rotations_r, cov3Ds_precomp, prefilter_var, raster_settings, bg_image (a per-pixel
-    background [3,H,W] behind the Gaussians, or None)."""
+    """reference: :67-225.  Inputs, in order: means3D, means2D, sh, sh_rest, colors_precomp, flow_2d, opacities, ts,
+    scales, scales_t, rotations, rotations_r, cov3Ds_precomp, prefilter_var, raster_settings, raw, bg_image.
+
+    raw: the raw-parameter entry (no reference counterpart; SURVEY.md section 8(f) row 1).  The inputs are then the
+    optimiser's RAW parameters -- log-scales, un-normalised quaternions, opacity logits, and the SH row as the two tensors
+    sh = features_dc [P,1,3] / sh_rest = features_rest [P,M-1,3] -- and the gradients come back w.r.t. exactly those, so
+    the exp / F.normalize x2 / sigmoid kernels and the 1.15 GB torch.cat of the reference's getters
+    (scene/gaussian_model.py:179-219), with their autograd mirror images, disappear from the frame.  Otherwise sh_rest is
+    empty.  bg_image: a per-pixel background [3,H,W] behind the Gaussians, or None."""
 
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, flow_2d, opacities, ts, scales, scales_t,
-                rotations, rotations_r, cov3Ds_precomp, prefilter_var, raster_settings, bg_image=None):
+    def forward(ctx, means3D, means2D, sh, sh_rest, colors_precomp, flow_2d, opacities, ts, scales, scales_t,
+                rotations, rotations_r, cov3Ds_precomp, prefilter_var, raster_settings, raw, bg_image):
         s = raster_settings
-        # positional layout of _C.rasterize_gaussians (reference: :88-119, rasterize_points.h:18-49)
+        # _C.rasterize_gaussians' positional layout (reference: :88-119, rasterize_points.h:18-49) + the extensions
         args = (s.bg, means3D, colors_precomp, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
                 s.scale_modifier, cov3Ds_precomp, prefilter_var, s.viewmatrix, s.projmatrix, s.tanfovx, s.tanfovy,
                 s.image_height, s.image_width, sh, s.sh_degree, s.sh_degree_t, s.campos, s.timestamp,
-                s.time_duration, s.rot_4d, s.gaussian_dim, s.force_sh_3d, s.prefiltered, s.debug)
-        if bg_image is None:
-            fw = _invoke(_C.rasterize_gaussians, args, s.debug, "snapshot_fw.dump")
-        else:
-            fw = _invoke(_C.rasterize_gaussians_bg, args + (bg_image,), s.debug, "snapshot_fw.dump")
-        (num_rendered, color, flow, depth, T, radii, geom_buf, binning_buf, img_buf, covs_com, out_means3D) = fw
+                s.time_duration, s.rot_4d, s.gaussian_dim, s.force_sh_3d, s.prefiltered, s.debug,
+                sh_rest, raw, _NONE if bg_image is None else bg_image)
+        (num_rendered, color, flow, depth, T, radii, geom_buf, binning_buf, img_buf, covs_com,
+         out_means3D) = _invoke(_C.rasterize_gaussians_ext, args, s.debug, "snapshot_fw.dump")
 
         _notify_forward(radii)
         ctx.bg_image = bg_image
+        ctx.raw = raw
         ctx.raster_settings = s
         ctx.num_rendered = num_rendered
         ctx.prefilter_var = prefilter_var
-        ctx.save_for_backward(colors_precomp, means3D, out_means3D, scales, rotations, cov3Ds_precomp, radii, sh,
+        ctx.save_for_backward(colors_precomp, means3D, out_means3D, scales, rotations, cov3Ds_precomp, radii, sh, sh_rest,
                               flow_2d, opacities, ts, scales_t, rotations_r, geom_buf, binning_buf, img_buf)
         ctx.mark_non_differentiable(radii)
         # outputs the loss does not touch arrive as None in backward() instead of zero images; the
@@ -130,7 +142,7 @@ class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_out_color, grad_radii, grad_depth, grad_alpha, grad_flow, grad_covs_com):
         s = ctx.raster_settings
-        (colors_precomp, means3D, out_means3D, scales, rotations, cov3Ds_precomp, radii, sh, flow_2d, opacities,
+        (colors_precomp, means3D, out_means3D, scales, rotations, cov3Ds_precomp, radii, sh, sh_rest, flow_2d, opacities,
          ts, scales_t, rotations_r, geom_buf, binning_buf, img_buf) = ctx.saved_tensors
         if grad_out_color is None:
             grad_out_color = torch.zeros(ctx.image_shape, dtype=torch.float32, device=means3D.device)
@@ -138,128 +150,41 @@ class _RasterizeGaussians(torch.autograd.Function):
         grad_depth = none if grad_depth is None else grad_depth
         grad_alpha = none if grad_alpha is None else grad_alpha
         grad_flow = none if grad_flow is None else grad_flow
-        # positional layout of _C.rasterize_gaussians_backward (reference: :154-190, rasterize_points.h:51-89)
-        args = (s.bg, means3D, out_means3D, radii, colors_precomp, flow_2d, opacities, ts, scales, scales_t,
-                rotations, rotations_r, s.scale_modifier, cov3Ds_precomp, ctx.prefilter_var, s.viewmatrix,
-                s.projmatrix, s.tanfovx, s.tanfovy, grad_out_color, grad_depth, grad_alpha, grad_flow, sh,
-                s.sh_degree, s.sh_degree_t, s.campos, s.timestamp, s.time_duration, s.rot_4d, s.gaussian_dim,
-                s.force_sh_3d, geom_buf, ctx.num_rendered, binning_buf, img_buf, s.debug)
         # View-parallel step (fdgs/dist.py, multi-GPU): the dense dL_dsh of this view is not produced; the backward
         # emits the [P,3] colour factor of its rank-one rows and the step rebuilds / sums the rows of all views after
         # the exchange.  No reference counterpart (its views are sequential on one GPU, train.py:104-166).
         from fdgs.dist import ViewParallelStep
         step = ViewParallelStep.current()
-        factors = step is not None and step.wants_factors(sh, cov3Ds_precomp) and ctx.needs_input_grad[2]
-        g_bg = None
-        if ctx.bg_image is not None:
-            want_bg = ctx.needs_input_grad[14]
-            out = _invoke(_C.rasterize_gaussians_backward_bg, args + (ctx.bg_image, bool(factors), bool(want_bg)), s.debug,
-                          "snapshot_bw.dump")
-            (g_means2D, g_colors, g_opacities, g_means3D, g_cov3D, g_sh, g_flows, g_ts, g_scales, g_scales_t,
-             g_rot, g_rot_r, sh_factors, g_bg) = out
-            g_bg = g_bg if want_bg else None
-            if factors:
-                step.record_view(sh_factors, s, dict(means3D=means3D, ts=ts, scales=scales, scales_t=scales_t,
-                                                     rotations=rotations, rotations_r=rotations_r))
-                g_sh = None
-        elif factors:
-            out = _invoke(_C.rasterize_gaussians_backward_factors, args, s.debug, "snapshot_bw.dump")
-            (g_means2D, g_colors, g_opacities, g_means3D, g_cov3D, _no_sh, g_flows, g_ts, g_scales, g_scales_t,
-             g_rot, g_rot_r, factors) = out
-            step.record_view(factors, s, dict(means3D=means3D, ts=ts, scales=scales, scales_t=scales_t,
-                                              rotations=rotations, rotations_r=rotations_r))
-            g_sh = None
-        else:
-            (g_means2D, g_colors, g_opacities, g_means3D, g_cov3D, g_sh, g_flows, g_ts, g_scales, g_scales_t,
-             g_rot, g_rot_r) = _invoke(_C.rasterize_gaussians_backward, args, s.debug, "snapshot_bw.dump")
+        factors = (step is not None and step.wants_factors(sh, cov3Ds_precomp)
+                   and (ctx.needs_input_grad[2] or ctx.needs_input_grad[3]))
+        want_bg = ctx.needs_input_grad[16]
+        # _C.rasterize_gaussians_backward's positional layout (reference: :154-190, rasterize_points.h:51-89) + the
+        # extensions
+        args = (s.bg, means3D, out_means3D, radii, colors_precomp, flow_2d, opacities, ts, scales, scales_t,
+                rotations, rotations_r, s.scale_modifier, cov3Ds_precomp, ctx.prefilter_var, s.viewmatrix,
+                s.projmatrix, s.tanfovx, s.tanfovy, grad_out_color, grad_depth, grad_alpha, grad_flow, sh,
+                s.sh_degree, s.sh_degree_t, s.campos, s.timestamp, s.time_duration, s.rot_4d, s.gaussian_dim,
+                s.force_sh_3d, geom_buf, ctx.num_rendered, binning_buf, img_buf, s.debug,
+                sh_rest, ctx.raw, _NONE if ctx.bg_image is None else ctx.bg_image, bool(factors), bool(want_bg))
+        (g_means2D, g_colors, g_opacities, g_means3D, g_cov3D, g_sh, g_flows, g_ts, g_scales, g_scales_t, g_rot, g_rot_r,
+         sh_factors, g_sh_rest, g_bg) = _invoke(_C.rasterize_gaussians_backward_ext, args, s.debug, "snapshot_bw.dump")
+        if factors:
+            inputs = dict(means3D=means3D, ts=ts, scales=scales, scales_t=scales_t, rotations=rotations,
+                          rotations_r=rotations_r)
+            if ctx.raw:
+                inputs["raw"] = True
+            step.record_view(sh_factors, s, inputs)
+            g_sh = g_sh_rest = None
 
         def for_input(grad, inp):
             # inputs passed as the empty "not provided" placeholder take no gradient
             return grad if (inp.numel() > 0 and grad is not None) else None
 
-        # one entry per forward input (reference: :208-223); prefilter_var / settings get None
-        return (g_means3D, g_means2D, for_input(g_sh, sh), for_input(g_colors, colors_precomp),
+        # one entry per forward input (reference: :208-223); prefilter_var / settings / raw get None
+        return (g_means3D, g_means2D, for_input(g_sh, sh), for_input(g_sh_rest, sh_rest), for_input(g_colors, colors_precomp),
                 for_input(g_flows, flow_2d), g_opacities, for_input(g_ts, ts), for_input(g_scales, scales),
                 for_input(g_scales_t, scales_t), for_input(g_rot, rotations), for_input(g_rot_r, rotations_r),
-                for_input(g_cov3D, cov3Ds_precomp), None, None, g_bg)
-
-
-class _RasterizeGaussiansRaw(torch.autograd.Function):
-    """Raw-parameter entry (no reference counterpart; SURVEY.md section 8(f) row 1): the inputs are the optimiser's RAW
-    parameters -- log-scales, un-normalised quaternions, opacity logits, and the SH row as the two tensors
-    features_dc [P,1,3] / features_rest [P,M-1,3] -- and the gradients come back w.r.t. exactly those, so the
-    exp / F.normalize x2 / sigmoid kernels and the 1.15 GB torch.cat of the reference's getters
-    (scene/gaussian_model.py:179-219), with their autograd mirror images, disappear from the frame.
-    Inputs, in order: means3D, means2D, features_dc, features_rest, flow_2d, opacity_logits, ts, log_scales,
-    log_scales_t, rotations_raw, rotations_r_raw, prefilter_var, raster_settings, bg_image (or None)."""
-
-    @staticmethod
-    def forward(ctx, means3D, means2D, sh_dc, sh_rest, flow_2d, opacities, ts, scales, scales_t, rotations,
-                rotations_r, prefilter_var, raster_settings, bg_image=None):
-        s = raster_settings
-        none = torch.Tensor([])
-        args = (s.bg, means3D, none, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
-                s.scale_modifier, none, prefilter_var, s.viewmatrix, s.projmatrix, s.tanfovx, s.tanfovy,
-                s.image_height, s.image_width, sh_dc, s.sh_degree, s.sh_degree_t, s.campos, s.timestamp,
-                s.time_duration, s.rot_4d, s.gaussian_dim, s.force_sh_3d, s.prefiltered, s.debug, sh_rest, True)
-        if bg_image is None:
-            fw = _invoke(_C.rasterize_gaussians_raw, args, s.debug, "snapshot_fw.dump")
-        else:
-            fw = _invoke(_C.rasterize_gaussians_raw_bg, args + (bg_image,), s.debug, "snapshot_fw.dump")
-        (num_rendered, color, flow, depth, T, radii, geom_buf, binning_buf, img_buf, covs_com, out_means3D) = fw
-        _notify_forward(radii)
-        ctx.bg_image = bg_image
-        ctx.raster_settings = s
-        ctx.num_rendered = num_rendered
-        ctx.prefilter_var = prefilter_var
-        ctx.save_for_backward(means3D, out_means3D, scales, rotations, radii, sh_dc, sh_rest, flow_2d, opacities, ts,
-                              scales_t, rotations_r, geom_buf, binning_buf, img_buf)
-        ctx.mark_non_differentiable(radii)
-        ctx.set_materialize_grads(False)
-        ctx.image_shape = tuple(color.shape)
-        return color, radii, depth, 1 - T, flow, covs_com
-
-    @staticmethod
-    def backward(ctx, grad_out_color, grad_radii, grad_depth, grad_alpha, grad_flow, grad_covs_com):
-        s = ctx.raster_settings
-        (means3D, out_means3D, scales, rotations, radii, sh_dc, sh_rest, flow_2d, opacities, ts, scales_t, rotations_r,
-         geom_buf, binning_buf, img_buf) = ctx.saved_tensors
-        if grad_out_color is None:
-            grad_out_color = torch.zeros(ctx.image_shape, dtype=torch.float32, device=means3D.device)
-        none = torch.empty(0, dtype=torch.float32, device=means3D.device)
-        grad_depth = none if grad_depth is None else grad_depth
-        grad_alpha = none if grad_alpha is None else grad_alpha
-        grad_flow = none if grad_flow is None else grad_flow
-        from fdgs.dist import ViewParallelStep
-        step = ViewParallelStep.current()
-        factors = step is not None and step.wants_factors(sh_dc, none) and (ctx.needs_input_grad[2] or ctx.needs_input_grad[3])
-        e = torch.Tensor([])
-        args = (s.bg, means3D, out_means3D, radii, e, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
-                s.scale_modifier, e, ctx.prefilter_var, s.viewmatrix, s.projmatrix, s.tanfovx, s.tanfovy, grad_out_color,
-                grad_depth, grad_alpha, grad_flow, sh_dc, s.sh_degree, s.sh_degree_t, s.campos, s.timestamp,
-                s.time_duration, s.rot_4d, s.gaussian_dim, s.force_sh_3d, geom_buf, ctx.num_rendered, binning_buf,
-                img_buf, s.debug, sh_rest, True, bool(factors))
-        g_bg = None
-        if ctx.bg_image is None:
-            out = _invoke(_C.rasterize_gaussians_backward_raw, args, s.debug, "snapshot_bw.dump")
-        else:
-            want_bg = ctx.needs_input_grad[13]
-            out = _invoke(_C.rasterize_gaussians_backward_raw_bg, args + (ctx.bg_image, bool(want_bg)), s.debug,
-                          "snapshot_bw.dump")
-            g_bg = out[14] if want_bg else None
-        (g_means2D, g_colors, g_opacities, g_means3D, g_cov3D, g_sh, g_flows, g_ts, g_scales, g_scales_t, g_rot, g_rot_r,
-         sh_factors, g_sh_rest) = out[:14]
-        if factors:
-            step.record_view(sh_factors, s, dict(means3D=means3D, ts=ts, scales=scales, scales_t=scales_t,
-                                                 rotations=rotations, rotations_r=rotations_r, raw=True))
-            g_sh = g_sh_rest = None
-
-        def for_input(grad, inp):
-            return grad if (inp.numel() > 0 and grad is not None) else None
-
-        return (g_means3D, g_means2D, for_input(g_sh, sh_dc), for_input(g_sh_rest, sh_rest), for_input(g_flows, flow_2d),
-                g_opacities, for_input(g_ts, ts), for_input(g_scales, scales), for_input(g_scales_t, scales_t),
-                for_input(g_rot, rotations), for_input(g_rot_r, rotations_r), None, None, g_bg)
+                for_input(g_cov3D, cov3Ds_precomp), None, None, None, g_bg if want_bg else None)
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, flow_2d, opacities, ts, scales, scales_t,
@@ -268,9 +193,9 @@ def rasterize_gaussians(means3D, means2D, sh, colors_precomp, flow_2d, opacities
     Gaussians' device) behind the Gaussians; the image is then `rendered + (1 - alpha) * bg_image`, bit for bit, and
     bg_image receives a gradient when it requires one."""
     _check_bg_image(bg_image, raster_settings, means3D)
-    return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, flow_2d, opacities, ts, scales,
+    return _RasterizeGaussians.apply(means3D, means2D, sh, _NONE, colors_precomp, flow_2d, opacities, ts, scales,
                                      scales_t, rotations, rotations_r, cov3Ds_precomp, prefilter_var,
-                                     raster_settings, bg_image)
+                                     raster_settings, False, bg_image)
 
 
 class GaussianRasterizer(nn.Module):
@@ -287,7 +212,7 @@ class GaussianRasterizer(nn.Module):
 
     def forward_raw(self, means3D, means2D, opacity_logits, features_dc, features_rest, log_scales, rotations_raw,
                     flow_2d=None, ts=None, log_scales_t=None, rotations_r_raw=None, prefilter_var=-1.0, bg_image=None):
-        """Same 6-tuple as forward(), from the optimiser's RAW parameters (see _RasterizeGaussiansRaw): activations and
+        """Same 6-tuple as forward(), from the optimiser's RAW parameters (see _RasterizeGaussians): activations and
         the SH concatenation happen inside the kernels, gradients arrive at the raw leaves directly.  bg_image: as in
         rasterize_gaussians."""
         if self.raster_settings.rot_4d and (rotations_r_raw is None or log_scales_t is None or ts is None):
@@ -298,9 +223,9 @@ class GaussianRasterizer(nn.Module):
             return torch.Tensor([]) if t is None else t
 
         _check_bg_image(bg_image, self.raster_settings, means3D)
-        return _RasterizeGaussiansRaw.apply(means3D, means2D, features_dc, opt(features_rest), opt(flow_2d), opacity_logits,
-                                            opt(ts), log_scales, opt(log_scales_t), rotations_raw, opt(rotations_r_raw),
-                                            prefilter_var, self.raster_settings, bg_image)
+        return _RasterizeGaussians.apply(means3D, means2D, features_dc, opt(features_rest), _NONE, opt(flow_2d),
+                                         opacity_logits, opt(ts), log_scales, opt(log_scales_t), rotations_raw,
+                                         opt(rotations_r_raw), _NONE, prefilter_var, self.raster_settings, True, bg_image)
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, flow_2d=None, ts=None,
                 scales=None, scales_t=None, rotations=None, rotations_r=None, cov3D_precomp=None,

@@ -36,12 +36,14 @@ def test_new_entries_reject_null_arguments():
     assert lib.fdgs_last_error() == b""
 
 
-def test_extension_exposes_the_new_bindings():
+def test_extension_exposes_the_extended_bindings():
     import fdgs
     C = fdgs.ext()
-    for name in ("rasterize_gaussians_bg", "rasterize_gaussians_backward_bg", "rasterize_gaussians_raw_bg",
-                 "rasterize_gaussians_backward_raw_bg", "sky_forward", "sky_backward"):
+    for name in ("rasterize_gaussians_ext", "rasterize_gaussians_backward_ext", "sky_forward", "sky_backward"):
         assert hasattr(C, name), name
+    # the per-variant bindings the two extended entries replace
+    for suffix in ("bg", "raw", "raw_bg", "backward_bg", "backward_raw", "backward_raw_bg", "backward_factors"):
+        assert not hasattr(C, "rasterize_gaussians_" + suffix), suffix
 
 
 def test_bg_image_is_validated_before_any_gpu_work():

@@ -17,6 +17,16 @@ CHAIN = {"scales", "scales_t", "rotations", "rotations_r", "ts"}
 RAW_CHAIN = {"scaling", "scaling_t", "rotation", "rotation_r", "t"}     # the same leaves under RawModel's names
 
 
+def _fwd_bg(C, args, bgi):
+    """rasterize_gaussians' 30 arguments with a per-pixel background: the extended entry without raw parameters"""
+    return C.rasterize_gaussians_ext(*args, torch.empty(0), False, bgi)
+
+
+def _bwd_bg(C, args, bgi):
+    """rasterize_gaussians_backward's 37 arguments with a per-pixel background, dL/dbg_image wanted (index 14)"""
+    return C.rasterize_gaussians_backward_ext(*args, torch.empty(0), False, bgi, False, True)
+
+
 def _bg_image(cfg):
     return torch.rand(3, cfg["H"], cfg["W"], generator=torch.Generator().manual_seed(cfg["seed"] + 7)).to(DEV)
 
@@ -28,11 +38,11 @@ def C():
 
 
 @pytest.mark.parametrize("name", CASES)
-def test_forward_is_the_torch_composition_bit_for_bit(C, name):
+def test_extended_forward_is_the_torch_composition_bit_for_bit(C, name):
     cfg, cam, sc, st = helpers.build(name, device=DEV)
     bgi = _bg_image(cfg)
     fw0 = C.rasterize_gaussians(*helpers.fwd_args(st, sc, cfg))
-    fw1 = C.rasterize_gaussians_bg(*helpers.fwd_args(st, sc, cfg), bgi)
+    fw1 = _fwd_bg(C, helpers.fwd_args(st, sc, cfg), bgi)
     alpha = 1 - fw0[4]
     assert torch.equal(fw1[1], fw0[1] + (1 - alpha) * bgi)
     assert fw1[0] == fw0[0]
@@ -41,14 +51,14 @@ def test_forward_is_the_torch_composition_bit_for_bit(C, name):
     vis = fw0[5] > 0             # covs_com: the rows of culled Gaussians are never written
     assert torch.equal(fw1[9][vis], fw0[9][vis])
     # an empty bg_image is "none"
-    fw2 = C.rasterize_gaussians_bg(*helpers.fwd_args(st, sc, cfg), torch.empty(0, device=DEV))
+    fw2 = _fwd_bg(C, helpers.fwd_args(st, sc, cfg), torch.empty(0, device=DEV))
     assert torch.equal(fw2[1], fw0[1])
 
     # dL/dbg_image on every pixel, including the tiles with empty lists
     gc, gd, ga, gf = helpers.pixel_grads(cfg, device=DEV)
     none = torch.empty(0, device=DEV)
-    bw = C.rasterize_gaussians_backward_bg(*helpers.bwd_args(st, sc, cfg, fw1, (gc, none, none, none)), bgi, False, True)
-    assert torch.equal(bw[13], (1 - alpha) * gc)
+    bw = _bwd_bg(C, helpers.bwd_args(st, sc, cfg, fw1, (gc, none, none, none)), bgi)
+    assert torch.equal(bw[14], (1 - alpha) * gc)
 
 
 def _leaves(sc):
@@ -144,7 +154,7 @@ def test_raw_entry_with_background_image(name):
     assert helpers.l2_rel(helpers.to_np(out["native"][3]), helpers.to_np(out["torch"][3])) <= 1e-4
 
 
-def test_no_gaussians_background_only(C):
+def test_extended_entry_with_no_gaussians_is_the_background(C):
     """P = 0: the image is the background and dL/dbg_image is the whole image gradient times T = 1."""
     cfg, cam, sc, st = helpers.build("ragged", device=DEV)
     bgi = _bg_image(cfg)
@@ -152,19 +162,19 @@ def test_no_gaussians_background_only(C):
     for i, t in enumerate(a):
         if isinstance(t, torch.Tensor) and t.dim() >= 1 and t.shape[0] == cfg["P"] and t.device.type == "cuda":
             a[i] = t[:0].contiguous()
-    fw = C.rasterize_gaussians_bg(*a, bgi)
+    fw = _fwd_bg(C, a, bgi)
     assert fw[0] == 0 and bool((fw[4] == 1).all())
     assert torch.equal(fw[1], (fw[1] - fw[1]) + st["bg"].view(3, 1, 1) + (1 - (1 - fw[4])) * bgi)
     gc = helpers.pixel_grads(cfg, device=DEV)[0]
     e = torch.empty(0, device=DEV)
     b = list(helpers.bwd_args(st, sc, cfg, fw, (gc, e, e, e)))
     b[1] = a[1]
-    bw = C.rasterize_gaussians_backward_bg(*b, bgi, False, True)
-    assert torch.equal(bw[13], (1 - (1 - fw[4])) * gc)
+    bw = _bwd_bg(C, b, bgi)
+    assert torch.equal(bw[14], (1 - (1 - fw[4])) * gc)
 
 
 @pytest.mark.parametrize("name", ["small", "rotcam"])
-def test_ctypes_forward_bg(C, name):
+def test_ctypes_forward_bg_matches_the_extended_entry(C, name):
     """fdgs_forward_bg through ctypes: NULL is fdgs_forward bit for bit, an image is the extension's result."""
     import fdgs
     from test_gpu_ctypes_abi import FwdArgs, FwdResult, ALLOC_FN, _p
@@ -208,7 +218,7 @@ def test_ctypes_forward_bg(C, name):
     plain = run(lib.fdgs_forward)
     null = run(lib.fdgs_forward_bg, _p(None))
     img = run(lib.fdgs_forward_bg, _p(bgi))
-    fw = C.rasterize_gaussians_bg(*helpers.fwd_args(st, sc, cfg), bgi)
+    fw = _fwd_bg(C, helpers.fwd_args(st, sc, cfg), bgi)
     for k in plain:
         assert torch.equal(plain[k], null[k]), k
     assert torch.equal(img["color"], fw[1])

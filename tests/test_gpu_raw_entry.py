@@ -76,26 +76,33 @@ def test_raw_entry_vs_reference_render_at_cfg3():
 
 
 def test_view_parallel_step_with_raw_entry():
-    """factor mode + raw entry on one GPU: 3 views, gradients at the raw leaves == sequential autograd accumulation"""
+    """factor mode + raw entry on one GPU: 3 views, gradients at the raw leaves == sequential autograd accumulation,
+    without and with an environment-map sky behind the Gaussians"""
     from fdgs.dist import ViewParallelStep
     from gaussian_renderer import render
     import test_gpu_view_parallel as vp
+    from test_gpu_sky import SkyModel, SkyPipe
     cfg, cam, sc, st = helpers.build("n3v", device=DEV)
-    cams = vp._views(cfg, 3, DEV)
     bg = torch.zeros(3, device=DEV)
-    A = RawModel(sc, seed=4, requires_grad=True)
-    B = RawModel(sc, seed=4, requires_grad=True)
     Gs = [torch.randn(3, cfg["H"], cfg["W"], generator=torch.Generator().manual_seed(50 + k)).to(DEV) for k in range(3)]
-    for k, c in enumerate(cams):
-        ((render(c, A, Pipe(), bg)["render"] * Gs[k]).sum() / 3).backward()
-    step = ViewParallelStep(sc.P, DEV)
-    with step:
+    for sky in (False, True):
+        cams = vp._views(cfg, 3, DEV, sky)
+        if sky:
+            A, B, pipe = SkyModel(sc, vp._env(), seed=4, requires_grad=True), SkyModel(sc, vp._env(), seed=4, requires_grad=True), SkyPipe()
+        else:
+            A, B, pipe = RawModel(sc, seed=4, requires_grad=True), RawModel(sc, seed=4, requires_grad=True), Pipe()
         for k, c in enumerate(cams):
-            pkg = render(c, B, Pipe(), bg)
-            ((pkg["render"] * Gs[k]).sum() / 3).backward()
-            step.add_view_stats(pkg["viewspace_points"].grad, pkg["radii"])
-    lv = B.leaves()
-    step.finish([lv[k] for k in ("xyz", "t", "scaling", "scaling_t", "rotation", "rotation_r", "opacity")],
-                [lv["features_dc"], lv["features_rest"]])
-    for k, a in A.leaves().items():
-        assert helpers.l2_rel(helpers.to_np(lv[k].grad), helpers.to_np(a.grad)) < (2e-6 if k.startswith("features") else 1e-4), k
+            ((render(c, A, pipe, bg)["render"] * Gs[k]).sum() / 3).backward()
+        step = ViewParallelStep(sc.P, DEV)
+        with step:
+            for k, c in enumerate(cams):
+                pkg = render(c, B, pipe, bg)
+                ((pkg["render"] * Gs[k]).sum() / 3).backward()
+                step.add_view_stats(pkg["viewspace_points"].grad, pkg["radii"])
+        lv = B.leaves()
+        step.finish([lv[k] for k in ("xyz", "t", "scaling", "scaling_t", "rotation", "rotation_r", "opacity")],
+                    [lv["features_dc"], lv["features_rest"]])
+        for k, a in A.leaves().items():
+            assert helpers.l2_rel(helpers.to_np(lv[k].grad), helpers.to_np(a.grad)) < (2e-6 if k.startswith("features") else 1e-4), (sky, k)
+        if sky:
+            assert helpers.l2_rel(helpers.to_np(B.env_map.grad), helpers.to_np(A.env_map.grad)) < 1e-4

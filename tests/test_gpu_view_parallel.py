@@ -2,8 +2,8 @@
 
   1. one GPU: the SH colour-factor backward + sh_outer_sum reconstruction equals the dense dL_dsh of the ordinary
      backward (one view), and the sum over several views equals accumulating the views' dL_dsh one after the other
-     (what the reference's sequential loop does, train.py:104-166);  the reconstruction kernel against its PyTorch
-     fp32 reference (tests/sh_outer_ref.py);
+     (what the reference's sequential loop does, train.py:104-166), also with an environment-map sky behind the
+     Gaussians;  the reconstruction kernel against its PyTorch fp32 reference (tests/sh_outer_ref.py);
   2. two GPUs (skipped on a one-GPU box): N NCCL ranks through ViewParallelStep reproduce the gradients and the
      densification statistics of the sequential single-GPU loop over the same views.
 """
@@ -23,8 +23,10 @@ class _Model:
     """GaussianModel stand-in over activated parameters; SH optionally split like the reference's
     features_dc / features_rest (scene/gaussian_model.py:210-214)."""
 
-    def __init__(self, sc, split_sh=False):
+    def __init__(self, sc, split_sh=False, env=None):
         leaf = lambda t: t.clone().requires_grad_(True)
+        if env is not None:
+            self.env_map = leaf(env)
         self.get_xyz, self.get_opacity = leaf(sc.means3D), leaf(sc.opacities)
         self.get_scaling, self.get_scaling_t = leaf(sc.scales), leaf(sc.scales_t)
         self.get_rotation, self.get_rotation_r, self.get_t = leaf(sc.rotations), leaf(sc.rotations_r), leaf(sc.ts)
@@ -51,28 +53,47 @@ class _Pipe:
     env_map_res = 0
 
 
-def _views(cfg, n, device):
-    """n cameras around the configuration's base camera, each with its own timestamp."""
+class _SkyPipe(_Pipe):
+    env_map_res = 500
+
+
+def _pipe(pc):
+    return _SkyPipe() if hasattr(pc, "env_map") else _Pipe()
+
+
+def _env():
+    """an environment map for the sky cases"""
+    return torch.rand(3, 500, 500, generator=torch.Generator().manual_seed(5)).to(DEV)
+
+
+def _views(cfg, n, device, sky=False):
+    """n cameras around the configuration's base camera, each with its own timestamp; sky: cameras with the pinhole
+    intrinsics the environment-map sampler needs (tests/sky_ref.py)."""
     from fdgs import synth
+    import sky_ref
     out = []
     for v in range(n):
         pose = cfg.get("pose", (0.0, 0.0, 0.0, 0.0, 0.0, 0.0))
         R, T = synth.pose_from_euler(pose[0] + 2.0 * v, pose[1] - 1.0 * v, pose[2], pose[3] + 0.05 * v, pose[4], pose[5] - 0.03 * v)
         dur = cfg.get("time_duration", 1.0)
-        out.append(synth.make_camera(cfg["W"], cfg["H"], timestamp=cfg.get("timestamp", 0.5) + 0.07 * dur * (v - 0.5 * n),
-                                     negative_fov=cfg.get("negative_fov", False), R=R, T=T).to(device))
+        timestamp = cfg.get("timestamp", 0.5) + 0.07 * dur * (v - 0.5 * n)
+        if sky:
+            out.append(sky_ref.SkyCamera(cfg["W"], cfg["H"], R=R, T=T, timestamp=timestamp, device=device))
+        else:
+            out.append(synth.make_camera(cfg["W"], cfg["H"], timestamp=timestamp, negative_fov=cfg.get("negative_fov", False),
+                                         R=R, T=T).to(device))
     return out
 
 
-def _sequential(cfg, sc, cams, device, split_sh):
+def _sequential(cfg, sc, cams, device, split_sh, env=None):
     """the reference's loop: render every view in turn, autograd accumulates (train.py:104-183)"""
     from gaussian_renderer import render
     from fdgs.dist import ViewBatchStats
-    pc = _Model(sc, split_sh)
+    pc = _Model(sc, split_sh, env)
     stats = ViewBatchStats(sc.P, device)
     bg = torch.zeros(3, device=device)
     for k, cam in enumerate(cams):
-        pkg = render(cam, pc, _Pipe(), bg)
+        pkg = render(cam, pc, _pipe(pc), bg)
         g = torch.Generator(device="cpu").manual_seed(1000 + k)
         G = torch.randn(3, cfg["H"], cfg["W"], generator=g).to(device)
         ((pkg["render"] * G).sum() / len(cams)).backward()
@@ -80,15 +101,15 @@ def _sequential(cfg, sc, cams, device, split_sh):
     return pc, stats
 
 
-def _view_parallel(cfg, sc, cams, view_ids, device, split_sh, group=None, views_per_rank=None):
+def _view_parallel(cfg, sc, cams, view_ids, device, split_sh, group=None, views_per_rank=None, env=None):
     from gaussian_renderer import render
     from fdgs.dist import ViewParallelStep
-    pc = _Model(sc, split_sh)
+    pc = _Model(sc, split_sh, env)
     step = ViewParallelStep(sc.P, device, group=group)
     bg = torch.zeros(3, device=device)
     with step:
         for k in view_ids:
-            pkg = render(cams[k], pc, _Pipe(), bg)
+            pkg = render(cams[k], pc, _pipe(pc), bg)
             g = torch.Generator(device="cpu").manual_seed(1000 + k)
             G = torch.randn(3, cfg["H"], cfg["W"], generator=g).to(device)
             ((pkg["render"] * G).sum() / len(cams)).backward()
@@ -112,21 +133,30 @@ def _cmp(pa, pb, sa, sb, tol_sh, tol_geo, tol_chain=None):
     for i, (a, b) in enumerate(zip(pa.geometry(), pb.geometry())):
         err = helpers.l2_rel(helpers.to_np(a.grad), helpers.to_np(b.grad))
         assert err <= (tol_geo if i == 6 else tol_chain), (i, err)
+    if hasattr(pa, "env_map"):
+        # both sides hand the sky sampler the same dL/dsky; its backward's atomics differ in the last bits
+        assert helpers.l2_rel(helpers.to_np(pa.env_map.grad), helpers.to_np(pb.env_map.grad)) <= tol_geo
     assert helpers.l2_rel(helpers.to_np(sa.grad_norm_sum), helpers.to_np(sb.grad_norm_sum)) <= tol_geo
     assert torch.equal(sa.visibility_count.view(-1), sb.visibility_count.view(-1))
     assert torch.equal(sa.max_radii, sb.max_radii)
 
 
-@pytest.mark.parametrize("name,nviews,split", [("small", 1, False), ("rotcam", 1, True), ("dur10", 3, False),
-                                               ("n3v", 4, True), ("sh3d", 2, False), ("mid", 3, True)])
-def test_factor_mode_equals_dense_backward_one_gpu(name, nviews, split):
+# sky: render() with an environment map, i.e. the rasterizer with a per-pixel background image
+ONE_GPU = [("small", 1, False, False), ("rotcam", 1, True, False), ("dur10", 3, False, False), ("n3v", 4, True, False),
+           ("sh3d", 2, False, False), ("mid", 3, True, False), ("small", 2, False, True), ("mid", 3, True, True)]
+
+
+@pytest.mark.parametrize("name,nviews,split,sky", ONE_GPU,
+                         ids=["%s-%d-%s%s" % (n, v, s, "-sky" if k else "") for n, v, s, k in ONE_GPU])
+def test_factor_mode_equals_dense_backward_one_gpu(name, nviews, split, sky):
     """world = 1: the factor path (no dense dL_dsh) against ordinary autograd accumulation over the same views.
     Same backward kernels for everything but the SH rows, so the geometry matches to the blend's atomic noise; the SH
     rows are rebuilt with the same device functions and summed in view order."""
     cfg, cam, sc, st = helpers.build(name, device=DEV)
-    cams = _views(cfg, nviews, DEV)
-    ref, rs = _sequential(cfg, sc, cams, DEV, split)
-    got, gs, info = _view_parallel(cfg, sc, cams, list(range(nviews)), DEV, split)
+    cams = _views(cfg, nviews, DEV, sky)
+    env = _env() if sky else None
+    ref, rs = _sequential(cfg, sc, cams, DEV, split, env)
+    got, gs, info = _view_parallel(cfg, sc, cams, list(range(nviews)), DEV, split, env=env)
     assert info["views_total"] == nviews
     # the blend backward's RED order differs from run to run -> dL_dcolor (the factor) carries ~1e-7 noise
     _cmp(got, ref, gs, rs, tol_sh=2e-6, tol_geo=1e-4, tol_chain=1e-3 if cfg["P"] < 50000 else 5e-3)
