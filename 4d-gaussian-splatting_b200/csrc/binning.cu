@@ -54,13 +54,21 @@ constexpr size_t BIN_SMEM_LIMIT = 200 * 1024;
 // SCATTER = true : row[t] holds the column prefix on entry; keys are written to
 //                  tile_offset[t] + row[t] + (arrival order inside the CTA).
 // SMEM: histogram lives in shared memory; otherwise (very large tile grids) the CTA-private global row is used in place.
-template <bool SCATTER, bool SMEM>
-__global__ void __launch_bounds__(BIN_THREADS) bin_pass_kernel(int P, int chunk, const uint4* __restrict__ binrec, int grid_x,
+// BATCH: blockIdx.y = view; binrec is a [views][P] stack and view v owns the columns v * num_tiles .. of matrix rows of
+// views * num_tiles columns (the shared-memory histogram stays one image's tiles)
+template <bool SCATTER, bool SMEM, bool BATCH>
+__device__ __forceinline__ void bin_pass_body(int P, int chunk, const uint4* __restrict__ binrec, int grid_x,
                                                                int num_tiles, uint32_t* __restrict__ matrix,
                                                                const uint32_t* __restrict__ tile_offset,
                                                                uint64_t* __restrict__ keys) {
     extern __shared__ uint32_t hist_smem[];
     uint32_t* row = matrix + (size_t)blockIdx.x * num_tiles;
+    if (BATCH) {
+        const size_t v = blockIdx.y;
+        row = matrix + ((size_t)blockIdx.x * gridDim.y + v) * num_tiles;
+        binrec += v * (size_t)P;
+        if (SCATTER) tile_offset += v * (size_t)num_tiles;
+    }
     uint32_t* hist = SMEM ? hist_smem : row;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     for (int t = tid; t < num_tiles; t += BIN_THREADS) {
@@ -122,6 +130,23 @@ __global__ void __launch_bounds__(BIN_THREADS) bin_pass_kernel(int P, int chunk,
         __syncthreads();
         for (int t = tid; t < num_tiles; t += BIN_THREADS) row[t] = hist[t];
     }
+}
+
+template <bool SCATTER, bool SMEM>
+__global__ void __launch_bounds__(BIN_THREADS) bin_pass_kernel(int P, int chunk, const uint4* __restrict__ binrec, int grid_x,
+                                                               int num_tiles, uint32_t* __restrict__ matrix,
+                                                               const uint32_t* __restrict__ tile_offset,
+                                                               uint64_t* __restrict__ keys) {
+    bin_pass_body<SCATTER, SMEM, false>(P, chunk, binrec, grid_x, num_tiles, matrix, tile_offset, keys);
+}
+
+// the batched entry (fdgs_forward_batch / fdgs_backward_batch): one view per blockIdx.y
+template <bool SCATTER, bool SMEM>
+__global__ void __launch_bounds__(BIN_THREADS) bin_pass_batch_kernel(int P, int chunk, const uint4* __restrict__ binrec, int grid_x,
+                                                               int num_tiles, uint32_t* __restrict__ matrix,
+                                                               const uint32_t* __restrict__ tile_offset,
+                                                               uint64_t* __restrict__ keys) {
+    bin_pass_body<SCATTER, SMEM, true>(P, chunk, binrec, grid_x, num_tiles, matrix, tile_offset, keys);
 }
 
 // ---- 2. offsets ------------------------------------------------------------------------------------
@@ -377,14 +402,16 @@ constexpr int SORT_LARGE_THREADS = 1024, SORT_LARGE_KEYS = 16384;    // 139 KB o
 
 // One CTA per tile.  LARGE = false handles the tiles with n <= 2048, LARGE = true those above (launched
 // only if the largest tile needs it); tiles above 16384 instances sort in place in global memory.
-template <bool LARGE>
-__global__ void __launch_bounds__(LARGE ? SORT_LARGE_THREADS : SORT_SMALL_THREADS)
-tile_sort_kernel(const uint2* __restrict__ ranges, uint64_t* __restrict__ keys, uint32_t* __restrict__ point_list,
-                 const InstRec* __restrict__ grec, StageRec* __restrict__ recs) {
+// BATCH: one CTA per (view, tile); the keys hold Gaussian indices in [0, P) and the records are gathered from the view's
+// slice of grec, a [views][P] stack
+template <bool LARGE, bool BATCH>
+__device__ __forceinline__ void tile_sort_body(const uint2* __restrict__ ranges, uint64_t* __restrict__ keys, uint32_t* __restrict__ point_list,
+                 const InstRec* __restrict__ grec, StageRec* __restrict__ recs, int tiles_per_view, int P) {
     extern __shared__ uint64_t skeys[];
     const uint2 range = ranges[blockIdx.x];
     const int n = (int)(range.y - range.x);
     if (n <= 0) return;
+    if (BATCH) grec += (size_t)(blockIdx.x / tiles_per_view) * (size_t)P;
     uint64_t* gk = keys + range.x;
     uint32_t* ids = point_list + range.x;
     if (!LARGE) {
@@ -403,6 +430,19 @@ tile_sort_kernel(const uint2* __restrict__ ranges, uint64_t* __restrict__ keys, 
             gather_records<SORT_LARGE_THREADS>(ids, n, grec, recs + range.x);
         }
     }
+}
+
+template <bool LARGE>
+__global__ void __launch_bounds__(LARGE ? SORT_LARGE_THREADS : SORT_SMALL_THREADS) tile_sort_kernel(const uint2* __restrict__ ranges, uint64_t* __restrict__ keys, uint32_t* __restrict__ point_list,
+                 const InstRec* __restrict__ grec, StageRec* __restrict__ recs, int tiles_per_view, int P) {
+    tile_sort_body<LARGE, false>(ranges, keys, point_list, grec, recs, tiles_per_view, P);
+}
+
+// the batched entry (fdgs_forward_batch / fdgs_backward_batch): one view per (view, tile) CTA
+template <bool LARGE>
+__global__ void __launch_bounds__(LARGE ? SORT_LARGE_THREADS : SORT_SMALL_THREADS) tile_sort_batch_kernel(const uint2* __restrict__ ranges, uint64_t* __restrict__ keys, uint32_t* __restrict__ point_list,
+                 const InstRec* __restrict__ grec, StageRec* __restrict__ recs, int tiles_per_view, int P) {
+    tile_sort_body<LARGE, true>(ranges, keys, point_list, grec, recs, tiles_per_view, P);
 }
 
 // test hook: unpack the per-Gaussian records into the reference's plain arrays; `radii` is any
@@ -440,8 +480,8 @@ int device_sm_count() {
 
 int bin_ctas() { return bin_cta_count(); }
 
-template <bool SCATTER>
-static cudaError_t launch_bin_pass(int P, const uint4* binrec, int grid_x, int grid_y,
+template <bool SCATTER, bool BATCH>
+static cudaError_t launch_bin_pass(int P, int views, const uint4* binrec, int grid_x, int grid_y,
                                    uint32_t* matrix, const uint32_t* tile_offset, uint64_t* keys, cudaStream_t stream) {
     if (P <= 0) return cudaSuccess;
     const int num_tiles = grid_x * grid_y;
@@ -449,22 +489,26 @@ static cudaError_t launch_bin_pass(int P, const uint4* binrec, int grid_x, int g
     int chunk = (P + ctas - 1) / ctas;
     chunk = (chunk + 31) & ~31;
     const size_t smem = (size_t)num_tiles * sizeof(uint32_t);
+    const dim3 grid(ctas, BATCH ? views : 1);
     if (smem <= BIN_SMEM_LIMIT) {
+        const auto k = BATCH ? bin_pass_batch_kernel<SCATTER, true> : bin_pass_kernel<SCATTER, true>;
         static PerDeviceOnce once;
-        cudaError_t e = ensure_dynamic_smem(bin_pass_kernel<SCATTER, true>, (int)BIN_SMEM_LIMIT, once);
+        cudaError_t e = ensure_dynamic_smem(k, (int)BIN_SMEM_LIMIT, once);
         if (e != cudaSuccess) return e;
-        bin_pass_kernel<SCATTER, true><<<ctas, BIN_THREADS, smem, stream>>>(P, chunk, binrec, grid_x, num_tiles, matrix,
-                                                                            tile_offset, keys);
+        k<<<grid, BIN_THREADS, smem, stream>>>(P, chunk, binrec, grid_x, num_tiles, matrix, tile_offset, keys);
     } else {
-        bin_pass_kernel<SCATTER, false><<<ctas, BIN_THREADS, 0, stream>>>(P, chunk, binrec, grid_x, num_tiles, matrix,
-                                                                          tile_offset, keys);
+        const auto k = BATCH ? bin_pass_batch_kernel<SCATTER, false> : bin_pass_kernel<SCATTER, false>;
+        k<<<grid, BIN_THREADS, 0, stream>>>(P, chunk, binrec, grid_x, num_tiles, matrix, tile_offset, keys);
     }
     return cudaGetLastError();
 }
 
-cudaError_t launch_bin_count(int P, const uint4* binrec, int grid_x, int grid_y, uint32_t* matrix, cudaStream_t stream) {
-    if (P <= 0) return cudaMemsetAsync(matrix, 0, (size_t)bin_cta_count() * grid_x * grid_y * sizeof(uint32_t), stream);
-    return launch_bin_pass<false>(P, binrec, grid_x, grid_y, matrix, nullptr, nullptr, stream);
+cudaError_t launch_bin_count(int P, const uint4* binrec, int grid_x, int grid_y, uint32_t* matrix, cudaStream_t stream,
+                             int views, bool batch) {
+    if (P <= 0)
+        return cudaMemsetAsync(matrix, 0, (size_t)bin_cta_count() * views * grid_x * grid_y * sizeof(uint32_t), stream);
+    if (batch) return launch_bin_pass<false, true>(P, views, binrec, grid_x, grid_y, matrix, nullptr, nullptr, stream);
+    return launch_bin_pass<false, false>(P, 1, binrec, grid_x, grid_y, matrix, nullptr, nullptr, stream);
 }
 
 cudaError_t launch_tile_scan(int num_tiles, uint32_t* matrix, uint32_t* tile_total, uint32_t* tile_offset, uint2* ranges,
@@ -475,25 +519,37 @@ cudaError_t launch_tile_scan(int num_tiles, uint32_t* matrix, uint32_t* tile_tot
 }
 
 cudaError_t launch_bin_scatter(int P, const uint4* binrec, int grid_x, int grid_y, uint32_t* matrix,
-                               const uint32_t* tile_offset, uint64_t* keys, cudaStream_t stream) {
-    return launch_bin_pass<true>(P, binrec, grid_x, grid_y, matrix, tile_offset, keys, stream);
+                               const uint32_t* tile_offset, uint64_t* keys, cudaStream_t stream, int views, bool batch) {
+    if (batch) return launch_bin_pass<true, true>(P, views, binrec, grid_x, grid_y, matrix, tile_offset, keys, stream);
+    return launch_bin_pass<true, false>(P, 1, binrec, grid_x, grid_y, matrix, tile_offset, keys, stream);
 }
 
 int tile_sort_pack_kernel_count(int max_count) { return max_count > SORT_SMALL_KEYS ? 2 : 1; }
 
-cudaError_t launch_tile_sort_pack(int num_tiles, int max_count, int R, const uint2* ranges, uint64_t* keys,
-                                  const InstRec* grec, StageRec* recs, uint32_t* point_list, cudaStream_t stream) {
-    if (num_tiles <= 0 || R <= 0) return cudaSuccess;
+template <bool BATCH>
+static cudaError_t tile_sort_pack(int num_tiles, int max_count, const uint2* ranges, uint64_t* keys, const InstRec* grec,
+                                  StageRec* recs, uint32_t* point_list, int tiles_per_view, int P, cudaStream_t stream) {
     constexpr size_t small_smem = (size_t)(SORT_SMALL_KEYS + SORT_SMALL_KEYS / 8) * sizeof(uint64_t);
     constexpr size_t large_smem = (size_t)(SORT_LARGE_KEYS + SORT_LARGE_KEYS / 16) * sizeof(uint64_t);
-    tile_sort_kernel<false><<<num_tiles, SORT_SMALL_THREADS, small_smem, stream>>>(ranges, keys, point_list, grec, recs);
+    const auto small = BATCH ? tile_sort_batch_kernel<false> : tile_sort_kernel<false>;
+    small<<<num_tiles, SORT_SMALL_THREADS, small_smem, stream>>>(ranges, keys, point_list, grec, recs, tiles_per_view, P);
     if (max_count > SORT_SMALL_KEYS) {
+        const auto large = BATCH ? tile_sort_batch_kernel<true> : tile_sort_kernel<true>;
         static PerDeviceOnce once;
-        cudaError_t e = ensure_dynamic_smem(tile_sort_kernel<true>, (int)large_smem, once);
+        cudaError_t e = ensure_dynamic_smem(large, (int)large_smem, once);
         if (e != cudaSuccess) return e;
-        tile_sort_kernel<true><<<num_tiles, SORT_LARGE_THREADS, large_smem, stream>>>(ranges, keys, point_list, grec, recs);
+        large<<<num_tiles, SORT_LARGE_THREADS, large_smem, stream>>>(ranges, keys, point_list, grec, recs, tiles_per_view, P);
     }
     return cudaGetLastError();
+}
+
+cudaError_t launch_tile_sort_pack(int num_tiles, int max_count, int R, const uint2* ranges, uint64_t* keys,
+                                  const InstRec* grec, StageRec* recs, uint32_t* point_list, cudaStream_t stream,
+                                  int tiles_per_view, int P) {
+    if (num_tiles <= 0 || R <= 0) return cudaSuccess;
+    if (tiles_per_view > 0)
+        return tile_sort_pack<true>(num_tiles, max_count, ranges, keys, grec, recs, point_list, tiles_per_view, P, stream);
+    return tile_sort_pack<false>(num_tiles, max_count, ranges, keys, grec, recs, point_list, 0, 0, stream);
 }
 
 cudaError_t launch_unpack_grec(int P, const InstRec* grec, const int* radii, float* depths, float* means2D,

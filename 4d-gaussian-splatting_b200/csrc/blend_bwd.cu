@@ -59,9 +59,34 @@ __device__ __forceinline__ void background_image_terms(const BlendBwdParams& p, 
     }
 }
 
-template <bool AUX>
-__global__ void __launch_bounds__(BB_THREADS, AUX ? 3 : 4) blend_bwd_kernel(const BlendBwdParams p) {
+// view v of a batch (blockIdx.z): the same kernel on the view's slices of ranges, of every image and of the five
+// per-Gaussian gradients (their rows keep the Gaussian indices [0, P) of the instance records)
+__device__ __forceinline__ BlendBwdParams blend_bwd_view(BlendBwdParams p, int v) {
+    const size_t HW = (size_t)p.W * p.H, P = (size_t)p.P;
+    p.ranges += (size_t)v * p.grid_x * p.grid_y;
+    p.final_T += v * HW;
+    p.n_contrib += v * HW;
+    p.dL_dpix += 3 * v * HW;
+    if (p.dL_depths) p.dL_depths += v * HW;
+    if (p.dL_masks) p.dL_masks += v * HW;
+    if (p.dL_dpix_flow) p.dL_dpix_flow += 2 * v * HW;
+    p.dL_dmean2D += 3 * v * P;
+    p.dL_dconic += 4 * v * P;
+    p.dL_dopacity += v * P;
+    p.dL_dcolor += 3 * v * P;
+    p.dL_dflows += 2 * v * P;
+    if (p.bg_image) p.bg_image += 3 * v * HW;
+    if (p.dL_dbg_image) p.dL_dbg_image += 3 * v * HW;
+    return p;
+}
+
+template <bool AUX, bool BATCH>
+__device__ __forceinline__ void blend_bwd_body(const BlendBwdParams& p_) {
     __shared__ BlendBwdSmem sm;
+    // an lvalue on both sides: the single-view instantiation reads its parameters in place, no copy
+    BlendBwdParams view_;
+    if (BATCH) view_ = blend_bwd_view(p_, blockIdx.z);
+    const BlendBwdParams& p = BATCH ? view_ : p_;
     const int tile = blockIdx.y * p.grid_x + blockIdx.x;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int wx0 = blockIdx.x * TILE_X + (warp & 1) * 8;
@@ -309,6 +334,17 @@ __global__ void __launch_bounds__(BB_THREADS, AUX ? 3 : 4) blend_bwd_kernel(cons
     }
 }
 
+template <bool AUX>
+__global__ void __launch_bounds__(BB_THREADS, AUX ? 3 : 4) blend_bwd_kernel(const BlendBwdParams p_) {
+    blend_bwd_body<AUX, false>(p_);
+}
+
+// the batched entry (fdgs_forward_batch / fdgs_backward_batch): one view per blockIdx.z
+template <bool AUX>
+__global__ void __launch_bounds__(BB_THREADS, AUX ? 3 : 4) blend_bwd_batch_kernel(const BlendBwdParams p_) {
+    blend_bwd_body<AUX, true>(p_);
+}
+
 
 // =====================================================================================================
 // v2: colour-only backward (no upstream gradient for flow / depth / alpha), the training default.
@@ -396,8 +432,12 @@ __device__ __forceinline__ uint32_t tf32_hi(float x) { return __float_as_uint(x)
 // the tensor core reads only the upper 19 bits of a tf32 operand, so the remainder needs no masking
 __device__ __forceinline__ uint32_t tf32_lo(float x, uint32_t hi) { return __float_as_uint(x - __uint_as_float(hi)); }
 
-template <int STAGES, bool ACOL_SMEM, bool AUX>
-__global__ void __launch_bounds__(B2_THREADS, (ACOL_SMEM && !AUX) ? 4 : 3) blend_bwd2_kernel(const BlendBwdParams p) {
+template <int STAGES, bool ACOL_SMEM, bool AUX, bool BATCH>
+__device__ __forceinline__ void blend_bwd2_body(const BlendBwdParams& p_) {
+    // an lvalue on both sides: the single-view instantiation reads its parameters in place, no copy
+    BlendBwdParams view_;
+    if (BATCH) view_ = blend_bwd_view(p_, blockIdx.z);
+    const BlendBwdParams& p = BATCH ? view_ : p_;
     static_assert(!AUX || ACOL_SMEM, "the AUX instantiation keeps its A fragments in shared memory");
     constexpr int B2_STAGES = STAGES;
     extern __shared__ __align__(128) unsigned char b2_smem_raw[];
@@ -695,6 +735,17 @@ __global__ void __launch_bounds__(B2_THREADS, (ACOL_SMEM && !AUX) ? 4 : 3) blend
     if (ncol > 0) flush(ncol);
 }
 
+template <int STAGES, bool ACOL_SMEM, bool AUX>
+__global__ void __launch_bounds__(B2_THREADS, (ACOL_SMEM && !AUX) ? 4 : 3) blend_bwd2_kernel(const BlendBwdParams p_) {
+    blend_bwd2_body<STAGES, ACOL_SMEM, AUX, false>(p_);
+}
+
+// the batched entry (fdgs_forward_batch / fdgs_backward_batch): one view per blockIdx.z
+template <int STAGES, bool ACOL_SMEM, bool AUX>
+__global__ void __launch_bounds__(B2_THREADS, (ACOL_SMEM && !AUX) ? 4 : 3) blend_bwd2_batch_kernel(const BlendBwdParams p_) {
+    blend_bwd2_body<STAGES, ACOL_SMEM, AUX, true>(p_);
+}
+
 }  // namespace
 
 bool blend_bwd_is_raw(const BlendBwdParams&) {
@@ -704,30 +755,37 @@ bool blend_bwd_is_raw(const BlendBwdParams&) {
     return !force_v1;
 }
 
-cudaError_t launch_blend_bwd(const BlendBwdParams& p, cudaStream_t stream) {
-    dim3 grid(p.grid_x, p.grid_y, 1);
+template <bool BATCH>
+static cudaError_t blend_bwd(const BlendBwdParams& p, cudaStream_t stream) {
+    const dim3 grid(p.grid_x, p.grid_y, BATCH ? p.views : 1);
     const bool aux = p.dL_depths || p.dL_masks || p.dL_dpix_flow;
     if (blend_bwd_is_raw(p)) {
         if (!aux) {
             // colour fragments in shared memory + 3 stages: 64 registers, 53 KB -> 4 CTAs / SM.  (Keeping them in
             // registers costs 80 registers -> 3 CTAs / SM and measured 8 % slower.)
+            const auto k = BATCH ? blend_bwd2_batch_kernel<3, true, false> : blend_bwd2_kernel<3, true, false>;
             static PerDeviceOnce once;
-            cudaError_t e = ensure_dynamic_smem(blend_bwd2_kernel<3, true, false>, (int)sizeof(B2Smem<3, true, false>), once);
+            cudaError_t e = ensure_dynamic_smem(k, (int)sizeof(B2Smem<3, true, false>), once);
             if (e != cudaSuccess) return e;
-            blend_bwd2_kernel<3, true, false><<<grid, B2_THREADS, sizeof(B2Smem<3, true, false>), stream>>>(p);
+            k<<<grid, B2_THREADS, sizeof(B2Smem<3, true, false>), stream>>>(p);
         } else {
             // upstream gradients for the depth / alpha / flow images too: 6 a1-weighted rows (16-row A tile), 3 CTAs / SM
+            const auto k = BATCH ? blend_bwd2_batch_kernel<3, true, true> : blend_bwd2_kernel<3, true, true>;
             static PerDeviceOnce once_aux;
-            cudaError_t e = ensure_dynamic_smem(blend_bwd2_kernel<3, true, true>, (int)sizeof(B2Smem<3, true, true>), once_aux);
+            cudaError_t e = ensure_dynamic_smem(k, (int)sizeof(B2Smem<3, true, true>), once_aux);
             if (e != cudaSuccess) return e;
-            blend_bwd2_kernel<3, true, true><<<grid, B2_THREADS, sizeof(B2Smem<3, true, true>), stream>>>(p);
+            k<<<grid, B2_THREADS, sizeof(B2Smem<3, true, true>), stream>>>(p);
         }
-    } else if (!aux) {
-        blend_bwd_kernel<false><<<grid, BB_THREADS, 0, stream>>>(p);
     } else {
-        blend_bwd_kernel<true><<<grid, BB_THREADS, 0, stream>>>(p);
+        const auto k = aux ? (BATCH ? blend_bwd_batch_kernel<true> : blend_bwd_kernel<true>)
+                           : (BATCH ? blend_bwd_batch_kernel<false> : blend_bwd_kernel<false>);
+        k<<<grid, BB_THREADS, 0, stream>>>(p);
     }
     return cudaGetLastError();
+}
+
+cudaError_t launch_blend_bwd(const BlendBwdParams& p, cudaStream_t stream) {
+    return p.views > 0 ? blend_bwd<true>(p, stream) : blend_bwd<false>(p, stream);
 }
 
 }  // namespace fdgs

@@ -32,8 +32,27 @@ struct __align__(128) BlendFwdSmem {
     int done_warps;
 };
 
-__global__ void __launch_bounds__(BF_THREADS) blend_fwd_kernel(const BlendFwdParams p) {
+// view v of a batch (blockIdx.z): the same kernel on the view's slices of ranges and of every image
+__device__ __forceinline__ BlendFwdParams blend_fwd_view(BlendFwdParams p, int v) {
+    const size_t HW = (size_t)p.W * p.H;
+    p.ranges += (size_t)v * p.grid_x * p.grid_y;
+    p.final_T += v * HW;
+    p.n_contrib += v * HW;
+    p.out_color += 3 * v * HW;
+    p.out_flow += 2 * v * HW;
+    p.out_depth += v * HW;
+    p.out_T += v * HW;
+    if (p.bg_image) p.bg_image += 3 * v * HW;
+    return p;
+}
+
+template <bool BATCH>
+__device__ __forceinline__ void blend_fwd_body(const BlendFwdParams& p_) {
     __shared__ BlendFwdSmem sm;
+    // an lvalue on both sides: the single-view instantiation reads its parameters in place, no copy
+    BlendFwdParams view_;
+    if (BATCH) view_ = blend_fwd_view(p_, blockIdx.z);
+    const BlendFwdParams& p = BATCH ? view_ : p_;
     const int tile = blockIdx.y * p.grid_x + blockIdx.x;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // 8x4 footprint per warp: warps tile the 16x16 block as 2 (x) by 4 (y)
@@ -186,11 +205,20 @@ __global__ void __launch_bounds__(BF_THREADS) blend_fwd_kernel(const BlendFwdPar
     }
 }
 
+__global__ void __launch_bounds__(BF_THREADS) blend_fwd_kernel(const BlendFwdParams p_) {
+    blend_fwd_body<false>(p_);
+}
+
+// the batched entry (fdgs_forward_batch / fdgs_backward_batch): one view per blockIdx.z
+__global__ void __launch_bounds__(BF_THREADS) blend_fwd_batch_kernel(const BlendFwdParams p_) {
+    blend_fwd_body<true>(p_);
+}
+
 }  // namespace
 
 cudaError_t launch_blend_fwd(const BlendFwdParams& p, cudaStream_t stream) {
-    dim3 grid(p.grid_x, p.grid_y, 1);
-    blend_fwd_kernel<<<grid, BF_THREADS, 0, stream>>>(p);
+    if (p.views > 0) blend_fwd_batch_kernel<<<dim3(p.grid_x, p.grid_y, p.views), BF_THREADS, 0, stream>>>(p);
+    else blend_fwd_kernel<<<dim3(p.grid_x, p.grid_y, 1), BF_THREADS, 0, stream>>>(p);
     return cudaGetLastError();
 }
 

@@ -120,7 +120,7 @@ struct GeomState {
     uint32_t* tiles_touched; // [P]
     uint4* binrec;           // [P] tile rectangle + depth bits of every Gaussian, for the binning passes
     size_t bytes;
-    static GeomState carve(char* base, int P) {
+    static GeomState carve(char* base, long long P) {
         GeomState g;
         Carver c(base);
         const size_t p = (size_t)(P > 0 ? P : 0);
@@ -144,11 +144,12 @@ struct ImageState {
     uint32_t* bin_info;      // [4] total instances, largest tile, overflow flag, spare
     size_t tiles;
     size_t bytes;
-    static ImageState carve(char* base, int W, int H) {
+    // views > 1: the batched entry's [views] stacks of every per-pixel and per-tile array (tiles = all views' tiles)
+    static ImageState carve(char* base, int W, int H, int views = 1) {
         ImageState s;
         Carver c(base);
-        const size_t N = (size_t)W * H;
-        s.tiles = (size_t)((W + fdgs::TILE_X - 1) / fdgs::TILE_X) * ((H + fdgs::TILE_Y - 1) / fdgs::TILE_Y);
+        const size_t N = (size_t)W * H * (size_t)views;
+        s.tiles = (size_t)((W + fdgs::TILE_X - 1) / fdgs::TILE_X) * ((H + fdgs::TILE_Y - 1) / fdgs::TILE_Y) * (size_t)views;
         s.final_T = c.take<float>(N);
         s.n_contrib = c.take<uint32_t>(N);
         s.ranges = c.take<uint2>(s.tiles);
@@ -175,6 +176,62 @@ struct BinningState {
         b.keys = c.take<uint64_t>(r);
         b.bytes = c.total();
         return b;
+    }
+};
+
+// The batched entry's geometry buffer: the [B][P] stacks of GeomState, then the per-view scalars
+struct BatchGeomState {
+    GeomState g;
+    fdgs::ViewScalars* scalars;   // [B]
+    size_t bytes;
+    static BatchGeomState carve(char* base, int P, int B) {
+        BatchGeomState s;
+        s.g = GeomState::carve(base, (long long)(P > 0 ? P : 0) * (B > 0 ? B : 0));
+        const size_t off = (s.g.bytes + 127) & ~(size_t)127;
+        s.scalars = base ? reinterpret_cast<fdgs::ViewScalars*>(base + off) : nullptr;
+        s.bytes = off + (size_t)(B > 0 ? B : 0) * sizeof(fdgs::ViewScalars) + 128;
+        return s;
+    }
+};
+
+// The batched backward's scratch: per-view gradients before their view sums, and the sh_outer_sum table
+struct BatchBwdScratch {
+    float* dL_dconic;     // [B,P,4] accumulated by the blend (zeroed by the backward)
+    float* dL_dcolor;     // [B,P,3] accumulated
+    float* dL_dflows;     // [B,P,2] accumulated
+    float* dL_dopacity;   // [B,P]   accumulated
+    float* dL_dmean3D;    // [B,P,3]
+    float* dL_dcov3D;     // [B,P,6]
+    float* dL_dts;        // [B,P]
+    float* dL_dscale;     // [B,P,3]
+    float* dL_dscale_t;   // [B,P]
+    float* dL_drot;       // [B,P,4]
+    float* dL_drot_r;     // [B,P,4]
+    float* table;         // [B][3P + 4] colour factors + view metadata
+    float* dirs;          // [B][P][8]
+    size_t zero_bytes;    // the accumulated arrays lead the buffer
+    size_t bytes;
+    static long long factor_stride(int P) { return 3ll * P + 4; }
+    static BatchBwdScratch carve(char* base, int P, int B) {
+        BatchBwdScratch s;
+        Carver c(base);
+        const size_t n = (size_t)(P > 0 ? P : 0) * (size_t)(B > 0 ? B : 0);
+        s.dL_dconic = c.take<float>(4 * n);
+        s.dL_dcolor = c.take<float>(3 * n);
+        s.dL_dflows = c.take<float>(2 * n);
+        s.dL_dopacity = c.take<float>(n);
+        s.zero_bytes = c.off;
+        s.dL_dmean3D = c.take<float>(3 * n);
+        s.dL_dcov3D = c.take<float>(6 * n);
+        s.dL_dts = c.take<float>(n);
+        s.dL_dscale = c.take<float>(3 * n);
+        s.dL_dscale_t = c.take<float>(n);
+        s.dL_drot = c.take<float>(4 * n);
+        s.dL_drot_r = c.take<float>(4 * n);
+        s.table = c.take<float>((size_t)factor_stride(P > 0 ? P : 0) * (size_t)(B > 0 ? B : 0));
+        s.dirs = c.take<float>(8 * n);
+        s.bytes = c.total();
+        return s;
     }
 };
 
@@ -207,19 +264,17 @@ const char* fdgs_last_error(void) { return g_last_error.c_str(); }
 size_t fdgs_geom_bytes(int P) { return GeomState::carve(nullptr, P).bytes + 128; }
 size_t fdgs_image_bytes(int width, int height) { return ImageState::carve(nullptr, width, height).bytes + 128; }
 size_t fdgs_binning_bytes(int num_rendered, int, int) { return BinningState::carve(nullptr, num_rendered).bytes + 128; }
+size_t fdgs_geom_batch_bytes(int P, int B) { return BatchGeomState::carve(nullptr, P, B).bytes + 128; }
+size_t fdgs_image_batch_bytes(int width, int height, int B) {
+    return ImageState::carve(nullptr, width, height, B > 0 ? B : 0).bytes + 128;
+}
+size_t fdgs_backward_batch_scratch_bytes(int P, int B) { return BatchBwdScratch::carve(nullptr, P, B).bytes + 128; }
 
 }  // extern "C"
 
 namespace {
 
-int forward_impl(const fdgs_forward_args* a, const float* bg_image, fdgs_alloc_fn geom_alloc, void* geom_ctx,
-                 fdgs_alloc_fn binning_alloc, void* binning_ctx, fdgs_alloc_fn image_alloc, void* image_ctx, void* stream_v,
-                 fdgs_forward_result* res) {
-    g_last_error.clear();
-    if (!a || !res || !geom_alloc || !binning_alloc || !image_alloc) return fail(FDGS_ERR_INVALID_ARG, "null argument");
-    memset(res, 0, sizeof(*res));
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
-    const bool debug = a->debug != 0;
+int check_forward_args(const fdgs_forward_args* a) {
     const int P = a->P, W = a->width, H = a->height;
     if (P < 0 || W <= 0 || H <= 0) return fail(FDGS_ERR_INVALID_ARG, "bad P / width / height");
     // the blend kernel writes every pixel of every image even when nothing is rendered (P == 0: background only)
@@ -251,6 +306,23 @@ int forward_impl(const fdgs_forward_args* a, const float* bg_image, fdgs_alloc_f
     const int grid_x = (W + fdgs::TILE_X - 1) / fdgs::TILE_X, grid_y = (H + fdgs::TILE_Y - 1) / fdgs::TILE_Y;
     // tile coordinates travel as 16-bit fields of the per-Gaussian bin record (preprocess_fwd.cu / binning.cu)
     if (grid_x > 65535 || grid_y > 65535) return fail(FDGS_ERR_UNSUPPORTED, "image larger than 1048560 pixels on a side");
+    if (P > 0 && a->shs_rest && !a->colors_precomp && a->M < 2) return fail(FDGS_ERR_INVALID_ARG, "split SH rows need M >= 2");
+    if (P > 0 && a->raw_params && a->cov3D_precomp)
+        return fail(FDGS_ERR_INVALID_ARG, "raw_params needs scales / rotations, not cov3D_precomp");
+    return FDGS_OK;
+}
+
+int forward_impl(const fdgs_forward_args* a, const float* bg_image, fdgs_alloc_fn geom_alloc, void* geom_ctx,
+                 fdgs_alloc_fn binning_alloc, void* binning_ctx, fdgs_alloc_fn image_alloc, void* image_ctx, void* stream_v,
+                 fdgs_forward_result* res) {
+    g_last_error.clear();
+    if (!a || !res || !geom_alloc || !binning_alloc || !image_alloc) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    memset(res, 0, sizeof(*res));
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
+    const bool debug = a->debug != 0;
+    const int P = a->P, W = a->width, H = a->height;
+    if (int rc = check_forward_args(a)) return rc;
+    const int grid_x = (W + fdgs::TILE_X - 1) / fdgs::TILE_X, grid_y = (H + fdgs::TILE_Y - 1) / fdgs::TILE_Y;
     const size_t N = (size_t)W * H;
 
     // scratch: geometry + image
@@ -288,8 +360,6 @@ int forward_impl(const fdgs_forward_args* a, const float* bg_image, fdgs_alloc_f
         sh_staging(a->colors_precomp ? nullptr : a->shs, a->M, true, &pp.sh_bulk_ok, &pp.sh_row_stride_floats);
         pp.raw_params = a->raw_params; pp.quat_norm_mode = g_quat_norm_mode;
         pp.shs_rest = a->colors_precomp ? nullptr : a->shs_rest;
-        if (pp.shs_rest && a->M < 2) return fail(FDGS_ERR_INVALID_ARG, "split SH rows need M >= 2");
-        if (a->raw_params && a->cov3D_precomp) return fail(FDGS_ERR_INVALID_ARG, "raw_params needs scales / rotations, not cov3D_precomp");
         pp.flows = a->flows_precomp;
         pp.out_means3D = a->out_means3D; pp.radii = a->radii; pp.cov3D = geom.cov3D; pp.grec = geom.grec;
         pp.clamped = geom.clamped; pp.tiles_touched = geom.tiles_touched; pp.binrec = geom.binrec;
@@ -335,6 +405,7 @@ int forward_impl(const fdgs_forward_args* a, const float* bg_image, fdgs_alloc_f
     bp.final_T = img.final_T; bp.n_contrib = img.n_contrib;
     bp.out_color = a->out_color; bp.out_flow = a->out_flow; bp.out_depth = a->out_depth; bp.out_T = a->out_T;
     bp.bg_image = bg_image;
+    bp.views = 0;
     (void)N;
     FDGS_STAGE(5, 1, fdgs::launch_blend_fwd(bp, stream), "blend_fwd");
     return FDGS_OK;
@@ -388,6 +459,7 @@ int backward_impl(const fdgs_backward_args* a, const float* bg_image, float* dL_
         bp.dL_dmean2D = a->dL_dmean2D; bp.dL_dconic = a->dL_dconic; bp.dL_dopacity = a->dL_dopacity;
         bp.dL_dcolor = a->dL_dcolor; bp.dL_dflows = a->dL_dflows;
         bp.bg_image = bg_image; bp.dL_dbg_image = dL_dbg_image;
+        bp.views = 0; bp.P = P;
         blend_raw = R > 0 && fdgs::blend_bwd_is_raw(bp);
         FDGS_STAGE(6, 1, fdgs::launch_blend_bwd(bp, stream), "blend_bwd");
     }
@@ -420,6 +492,232 @@ int backward_impl(const fdgs_backward_args* a, const float* bg_image, float* dL_
     if (pb.has_scales && pb.rot_4d && (!a->rotations_r || !a->scales_t || !a->ts || !a->opacities))
         return fail(FDGS_ERR_INVALID_ARG, "rot_4d backward needs rotations_r, scales_t, ts, opacities");
     FDGS_STAGE(7, fdgs::preprocess_bwd_kernel_count(pb), fdgs::launch_preprocess_bwd(pb, stream), "preprocess_bwd");
+    return FDGS_OK;
+}
+
+// ---- batched views: B cameras of the same Gaussians in one pass per stage (include/fdgs.h: fdgs_forward_batch) -------
+constexpr int kMaxViews = 65535;   // views run along gridDim.y / gridDim.z
+
+int check_batch_views(int B, const float* bg_image, int bg_views) {
+    if (B < 1 || B > kMaxViews) return fail(FDGS_ERR_INVALID_ARG, "bad view count B (1 <= B <= 65535)");
+    if (bg_image && bg_views != B) return fail(FDGS_ERR_INVALID_ARG, "bg_image view count does not match B");
+    return FDGS_OK;
+}
+
+int forward_batch_impl(const fdgs_forward_batch_args* b, fdgs_alloc_fn geom_alloc, void* geom_ctx, fdgs_alloc_fn binning_alloc,
+                       void* binning_ctx, fdgs_alloc_fn image_alloc, void* image_ctx, void* stream_v, fdgs_forward_result* res) {
+    g_last_error.clear();
+    if (!b || !res || !geom_alloc || !binning_alloc || !image_alloc) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    memset(res, 0, sizeof(*res));
+    const fdgs_forward_args* a = &b->view;
+    const int B = b->B;
+    if (int rc = check_batch_views(B, b->bg_image, b->bg_views)) return rc;
+    if (!a->viewmatrix || !a->projmatrix || !a->cam_pos || !b->timestamps || !b->tan_fovx || !b->tan_fovy)
+        return fail(FDGS_ERR_INVALID_ARG, "the per-view camera table (viewmatrix / projmatrix / cam_pos / timestamps / tan_fovx / "
+                                          "tan_fovy) must be set");
+    if (int rc = check_forward_args(a)) return rc;
+    if (a->P > 0 && (a->colors_precomp || a->cov3D_precomp))
+        return fail(FDGS_ERR_INVALID_ARG, "the batched entry takes SH and scales / rotations, not precomputed colours or covariances");
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
+    const bool debug = a->debug != 0;
+    const int P = a->P, W = a->width, H = a->height;
+    const int grid_x = (W + fdgs::TILE_X - 1) / fdgs::TILE_X, grid_y = (H + fdgs::TILE_Y - 1) / fdgs::TILE_Y;
+    const int tiles = grid_x * grid_y;
+    if ((long long)tiles * B > 0x7fffffffLL || (long long)P * B > 0x7fffffffLL)
+        return fail(FDGS_ERR_UNSUPPORTED, "B * tiles or B * P exceeds 2^31 - 1");
+
+    const size_t geom_bytes = fdgs_geom_batch_bytes(P, B);
+    char* geom_raw = geom_alloc(geom_ctx, geom_bytes);
+    if (!geom_raw) return fail(FDGS_ERR_ALLOC, "geometry buffer allocation failed");
+    BatchGeomState geom = BatchGeomState::carve(align128(geom_raw), P, B);
+    const size_t img_bytes = fdgs_image_batch_bytes(W, H, B);
+    char* img_raw = image_alloc(image_ctx, img_bytes);
+    if (!img_raw) return fail(FDGS_ERR_ALLOC, "image buffer allocation failed");
+    ImageState img = ImageState::carve(align128(img_raw), W, H, B);
+    res->geom_buffer = geom_raw;
+    res->geom_bytes = geom_bytes;
+    res->image_buffer = img_raw;
+    res->image_bytes = img_bytes;
+    res->cov3D = geom.g.cov3D;
+
+    // the per-view scalars, focal lengths computed as the single-view entry computes them (reference: rasterizer_impl.cu:235-236);
+    // a pageable host-to-device copy is staged before the call returns and does not synchronise
+    std::vector<fdgs::ViewScalars> vs((size_t)B);
+    for (int v = 0; v < B; ++v) {
+        memset(&vs[v], 0, sizeof(vs[v]));
+        vs[v].timestamp = b->timestamps[v];
+        vs[v].tan_fovx = b->tan_fovx[v];
+        vs[v].tan_fovy = b->tan_fovy[v];
+        vs[v].focal_y = H / (2.0f * b->tan_fovy[v]);
+        vs[v].focal_x = W / (2.0f * b->tan_fovx[v]);
+    }
+    FDGS_CUDA(cudaMemcpyAsync(geom.scalars, vs.data(), vs.size() * sizeof(vs[0]), cudaMemcpyHostToDevice, stream), "view table copy");
+
+    if (P > 0) {
+        fdgs::PreprocessFwdParams pp;
+        memset(&pp, 0, sizeof(pp));
+        pp.P = P; pp.D = a->D; pp.D_t = a->D_t; pp.M = a->M;
+        pp.means3D = a->means3D; pp.ts = a->ts; pp.scales = a->scales; pp.scales_t = a->scales_t;
+        pp.scale_modifier = a->scale_modifier; pp.rotations = a->rotations; pp.rotations_r = a->rotations_r;
+        pp.opacities = a->opacities; pp.shs = a->shs; pp.prefilter_var = a->prefilter_var;
+        pp.viewmatrix = a->viewmatrix; pp.projmatrix = a->projmatrix; pp.cam_pos = a->cam_pos;
+        pp.time_duration = a->time_duration;
+        pp.rot_4d = a->rot_4d; pp.gaussian_dim = a->gaussian_dim; pp.force_sh_3d = a->force_sh_3d;
+        pp.W = W; pp.H = H; pp.grid_x = grid_x; pp.grid_y = grid_y; pp.prefiltered = a->prefiltered;
+        sh_staging(a->shs, a->M, true, &pp.sh_bulk_ok, &pp.sh_row_stride_floats);
+        pp.raw_params = a->raw_params; pp.quat_norm_mode = g_quat_norm_mode; pp.shs_rest = a->shs_rest;
+        pp.flows = a->flows_precomp;
+        pp.out_means3D = a->out_means3D; pp.radii = a->radii; pp.cov3D = geom.g.cov3D; pp.grec = geom.g.grec;
+        pp.clamped = geom.g.clamped; pp.tiles_touched = geom.g.tiles_touched; pp.binrec = geom.g.binrec;
+        pp.tile_cull = g_tile_cull.load();
+        pp.vb.B = B; pp.vb.scalars = geom.scalars;
+        FDGS_STAGE(0, 1, fdgs::launch_preprocess_fwd(pp, stream), "preprocess_fwd (batch)");
+    }
+    FDGS_STAGE(1, (P > 0 ? 1 : 0) + 2,
+               [&]() {
+                   cudaError_t e = fdgs::launch_bin_count(P, geom.g.binrec, grid_x, grid_y, img.bin_matrix, stream, B, true);
+                   if (e != cudaSuccess) return e;
+                   return fdgs::launch_tile_scan((int)img.tiles, img.bin_matrix, img.tile_total, img.tile_offset, img.ranges,
+                                                 img.bin_info, stream);
+               }(),
+               "bin_count + tile_scan (batch)");
+    // the one host synchronisation of the batch: R over all views, the largest tile of any view, the overflow flag
+    int bin_info[4] = {0, 0, 0, 0};
+    FDGS_CUDA(cudaMemcpyAsync(bin_info, img.bin_info, sizeof(bin_info), cudaMemcpyDeviceToHost, stream), "num_rendered copy");
+    FDGS_CUDA(cudaStreamSynchronize(stream), "num_rendered sync");
+    const int num_rendered = bin_info[0];
+    if (num_rendered < 0 || bin_info[2] != 0) return fail(FDGS_ERR_UNSUPPORTED, "more than 2^31 - 1 tile instances");
+    res->num_rendered = num_rendered;
+
+    const size_t bin_bytes = fdgs_binning_bytes(num_rendered, W, H);
+    char* bin_raw = binning_alloc(binning_ctx, bin_bytes);
+    if (!bin_raw) return fail(FDGS_ERR_ALLOC, "binning buffer allocation failed");
+    BinningState bin = BinningState::carve(align128(bin_raw), num_rendered);
+    res->binning_buffer = bin_raw;
+    res->binning_bytes = bin_bytes;
+
+    if (num_rendered > 0) {
+        FDGS_STAGE(2, 1,
+                   fdgs::launch_bin_scatter(P, geom.g.binrec, grid_x, grid_y, img.bin_matrix, img.tile_offset, bin.keys, stream,
+                                            B, true),
+                   "bin_scatter (batch)");
+        FDGS_STAGE(3, fdgs::tile_sort_pack_kernel_count(bin_info[1]),
+                   fdgs::launch_tile_sort_pack((int)img.tiles, bin_info[1], num_rendered, img.ranges, bin.keys, geom.g.grec,
+                                               bin.recs, bin.point_list, stream, tiles, P),
+                   "tile_sort_pack (batch)");
+    }
+    fdgs::BlendFwdParams bp;
+    bp.W = W; bp.H = H; bp.grid_x = grid_x; bp.grid_y = grid_y;
+    bp.ranges = img.ranges; bp.recs = bin.recs; bp.background = a->background;
+    bp.final_T = img.final_T; bp.n_contrib = img.n_contrib;
+    bp.out_color = a->out_color; bp.out_flow = a->out_flow; bp.out_depth = a->out_depth; bp.out_T = a->out_T;
+    bp.bg_image = b->bg_image;
+    bp.views = B;
+    FDGS_STAGE(5, 1, fdgs::launch_blend_fwd(bp, stream), "blend_fwd (batch)");
+    return FDGS_OK;
+}
+
+int backward_batch_impl(const fdgs_backward_batch_args* b, void* stream_v) {
+    g_last_error.clear();
+    if (!b) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    const fdgs_backward_args* a = &b->view;
+    const int B = b->B;
+    if (int rc = check_batch_views(B, b->bg_image, b->bg_views)) return rc;
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
+    const bool debug = a->debug != 0;
+    const int P = a->P, W = a->width, H = a->height, R = a->R;
+    if (P < 0 || W <= 0 || H <= 0 || R < 0) return fail(FDGS_ERR_INVALID_ARG, "bad P / width / height / R");
+    if (!a->image_buffer || !a->geom_buffer || !a->dL_dpix || !a->background)
+        return fail(FDGS_ERR_INVALID_ARG, "scratch buffers of the forward pass / colour image gradient / background required");
+    const int grid_x = (W + fdgs::TILE_X - 1) / fdgs::TILE_X, grid_y = (H + fdgs::TILE_Y - 1) / fdgs::TILE_Y;
+    if ((long long)grid_x * grid_y * B > 0x7fffffffLL || (long long)P * B > 0x7fffffffLL)
+        return fail(FDGS_ERR_UNSUPPORTED, "B * tiles or B * P exceeds 2^31 - 1");
+    ImageState img = ImageState::carve(align128(const_cast<char*>(a->image_buffer)), W, H, B);
+    fdgs::BlendBwdParams bp;
+    memset(&bp, 0, sizeof(bp));
+    bp.W = W; bp.H = H; bp.grid_x = grid_x; bp.grid_y = grid_y;
+    bp.ranges = img.ranges; bp.background = a->background; bp.final_T = img.final_T; bp.n_contrib = img.n_contrib;
+    bp.dL_dpix = a->dL_dpix; bp.dL_depths = a->dL_depths; bp.dL_masks = a->dL_masks; bp.dL_dpix_flow = a->dL_dpix_flow;
+    bp.bg_image = b->bg_image; bp.dL_dbg_image = b->dL_dbg_image;
+    bp.views = B; bp.P = P;
+    if (P == 0) {
+        // nothing was rendered: the background image takes the whole colour gradient
+        if (b->dL_dbg_image) FDGS_STAGE(6, 1, fdgs::launch_blend_bwd(bp, stream), "blend_bwd (batch)");
+        return FDGS_OK;
+    }
+    if (R > 0 && !a->binning_buffer) return fail(FDGS_ERR_INVALID_ARG, "scratch buffers of the forward pass required");
+    if (!a->radii || !a->out_means3D || !a->viewmatrix || !a->projmatrix || !a->campos)
+        return fail(FDGS_ERR_INVALID_ARG, "radii / out_means3D / viewmatrix / projmatrix / campos required");
+    if (!a->shs || a->M <= 0 || a->colors_precomp || a->cov3D_precomp || !a->scales || !a->rotations)
+        return fail(FDGS_ERR_INVALID_ARG, "the batched entry takes SH and scales / rotations, not precomputed colours or covariances");
+    if (a->rot_4d && (!a->rotations_r || !a->scales_t || !a->ts || !a->opacities))
+        return fail(FDGS_ERR_INVALID_ARG, "rot_4d backward needs rotations_r, scales_t, ts, opacities");
+    if (!a->dL_dmean2D || !a->dL_dopacity || !a->dL_dmean3D || !a->dL_dsh || !a->dL_dts || !a->dL_dscale || !a->dL_dscale_t ||
+        !a->dL_drot || !a->dL_drot_r || !b->scratch)
+        return fail(FDGS_ERR_INVALID_ARG, "gradient outputs and scratch required");
+    if (a->shs_rest && !a->dL_dsh_rest) return fail(FDGS_ERR_INVALID_ARG, "split SH rows need dL_dsh_rest");
+    if (!a->shs_rest && a->dL_dsh_rest) return fail(FDGS_ERR_INVALID_ARG, "dL_dsh_rest without shs_rest");
+
+    BatchGeomState geom = BatchGeomState::carve(align128(const_cast<char*>(a->geom_buffer)), P, B);
+    BinningState bin = BinningState::carve(a->binning_buffer ? align128(const_cast<char*>(a->binning_buffer)) : nullptr, R);
+    BatchBwdScratch sc = BatchBwdScratch::carve(align128(b->scratch), P, B);
+    FDGS_CUDA(cudaMemsetAsync(sc.dL_dconic, 0, sc.zero_bytes, stream), "zero the accumulated gradients");
+
+    bool blend_raw = false;
+    if (R > 0 || b->dL_dbg_image) {
+        bp.recs = bin.recs;
+        bp.dL_dmean2D = a->dL_dmean2D; bp.dL_dconic = sc.dL_dconic; bp.dL_dopacity = sc.dL_dopacity;
+        bp.dL_dcolor = sc.dL_dcolor; bp.dL_dflows = sc.dL_dflows;
+        blend_raw = R > 0 && fdgs::blend_bwd_is_raw(bp);
+        FDGS_STAGE(6, 1, fdgs::launch_blend_bwd(bp, stream), "blend_bwd (batch)");
+    }
+    fdgs::PreprocessBwdParams pb;
+    memset(&pb, 0, sizeof(pb));
+    pb.P = P; pb.D = a->D; pb.D_t = a->D_t; pb.M = a->M;
+    pb.means3D = a->out_means3D; pb.radii = a->radii; pb.shs = a->shs; pb.ts = a->ts; pb.opacities = a->opacities;
+    pb.clamped = geom.g.clamped; pb.tiles_touched = geom.g.tiles_touched;
+    pb.scales = a->scales; pb.scales_t = a->scales_t; pb.rotations = a->rotations; pb.rotations_r = a->rotations_r;
+    pb.scale_modifier = a->scale_modifier; pb.cov3D = geom.g.cov3D;
+    pb.prefilter_var = a->prefilter_var; pb.viewmatrix = a->viewmatrix; pb.projmatrix = a->projmatrix; pb.campos = a->campos;
+    pb.time_duration = a->time_duration;
+    pb.rot_4d = a->rot_4d; pb.gaussian_dim = a->gaussian_dim; pb.force_sh_3d = a->force_sh_3d;
+    pb.has_scales = 1;
+    pb.grec = geom.g.grec; pb.blend_raw = blend_raw ? 1 : 0; pb.W = W; pb.H = H;
+    sh_staging(a->shs, a->M, false, &pb.sh_bulk_ok, &pb.sh_row_stride_floats);
+    pb.raw_params = a->raw_params; pb.quat_norm_mode = g_quat_norm_mode; pb.shs_rest = a->shs_rest;
+    pb.dL_dmean2D = a->dL_dmean2D; pb.dL_dconic = sc.dL_dconic; pb.dL_dopacity = sc.dL_dopacity; pb.dL_dcolor = sc.dL_dcolor;
+    pb.dL_dmean3D = sc.dL_dmean3D; pb.dL_dcov3D = sc.dL_dcov3D; pb.sh_factors = sc.table; pb.dL_dts = sc.dL_dts;
+    pb.dL_dscale = sc.dL_dscale; pb.dL_dscale_t = sc.dL_dscale_t; pb.dL_drot = sc.dL_drot; pb.dL_drot_r = sc.dL_drot_r;
+    pb.vb.B = B; pb.vb.scalars = geom.scalars; pb.factor_stride = BatchBwdScratch::factor_stride(P);
+    FDGS_STAGE(7, fdgs::preprocess_bwd_kernel_count(pb), fdgs::launch_preprocess_bwd(pb, stream), "preprocess_bwd (batch)");
+
+    // every per-Gaussian gradient but the SH rows: summed over the views in view order
+    fdgs::ViewSumParams vsum;
+    memset(&vsum, 0, sizeof(vsum));
+    vsum.B = B;
+    const struct { const float* src; float* dst; int width; } sums[] = {
+        {sc.dL_dmean3D, a->dL_dmean3D, 3}, {sc.dL_dopacity, a->dL_dopacity, 1}, {sc.dL_dts, a->dL_dts, 1},
+        {sc.dL_dscale, a->dL_dscale, 3},   {sc.dL_dscale_t, a->dL_dscale_t, 1}, {sc.dL_drot, a->dL_drot, 4},
+        {sc.dL_drot_r, a->dL_drot_r, 4}};
+    for (const auto& t : sums) {
+        vsum.src[vsum.n] = t.src;
+        vsum.dst[vsum.n] = t.dst;
+        vsum.count[vsum.n] = (long long)t.width * P;
+        ++vsum.n;
+    }
+    FDGS_STAGE(7, 1, fdgs::launch_view_sum(vsum, stream), "view_sum (batch)");
+
+    // the SH rows: the views' rank-one rows summed straight into dL_dsh (| dL_dsh_rest), every row (K = P)
+    fdgs::ShSumParams sp;
+    memset(&sp, 0, sizeof(sp));
+    sp.P = P; sp.V = B; sp.K = P; sp.table = sc.table; sp.view_stride = BatchBwdScratch::factor_stride(P); sp.meta_off = 3ll * P;
+    sp.slot_of = nullptr; sp.union_idx = nullptr; sp.dirs = sc.dirs; sp.means3D = a->out_means3D; sp.ts = a->ts;
+    sp.scales = a->scales; sp.scales_t = a->scales_t; sp.rotations = a->rotations; sp.rotations_r = a->rotations_r;
+    sp.scale_modifier = a->scale_modifier; sp.time_duration = a->time_duration; sp.rot_4d = a->rot_4d;
+    sp.gaussian_dim = a->gaussian_dim; sp.force_sh_3d = a->force_sh_3d; sp.D = a->D; sp.D_t = a->D_t; sp.M = a->M;
+    sp.out0 = a->dL_dsh; sp.m0 = a->shs_rest ? 1 : a->M; sp.out1 = a->shs_rest ? a->dL_dsh_rest : nullptr; sp.accumulate = 0;
+    sp.view_means = a->out_means3D;
+    FDGS_STAGE(7, 2, fdgs::launch_sh_outer_sum(sp, stream), "sh_outer_sum (batch)");
     return FDGS_OK;
 }
 
@@ -461,6 +759,14 @@ int fdgs_backward(const fdgs_backward_args* a, void* stream) { return backward_i
 int fdgs_backward_bg(const fdgs_backward_args* a, const float* bg_image, float* dL_dbg_image, void* stream) {
     return backward_impl(a, bg_image, dL_dbg_image, stream);
 }
+
+int fdgs_forward_batch(const fdgs_forward_batch_args* args, fdgs_alloc_fn geom_alloc, void* geom_ctx,
+                       fdgs_alloc_fn binning_alloc, void* binning_ctx, fdgs_alloc_fn image_alloc, void* image_ctx, void* stream,
+                       fdgs_forward_result* res) {
+    return forward_batch_impl(args, geom_alloc, geom_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, stream, res);
+}
+
+int fdgs_backward_batch(const fdgs_backward_batch_args* args, void* stream) { return backward_batch_impl(args, stream); }
 
 int fdgs_sky_forward(const fdgs_sky_args* a, float* out_sky, int* miss_flag, void* stream_v) {
     g_last_error.clear();
@@ -535,6 +841,7 @@ int fdgs_sh_outer_sum(const fdgs_sh_sum_args* a, void* stream_v) {
     p.time_duration = a->time_duration; p.rot_4d = a->rot_4d; p.gaussian_dim = a->gaussian_dim;
     p.force_sh_3d = a->force_sh_3d; p.D = a->D; p.D_t = a->D_t; p.M = a->M;
     p.out0 = a->out0; p.m0 = a->m0; p.out1 = (a->m0 < a->M) ? a->out1 : nullptr; p.accumulate = a->accumulate;
+    p.view_means = nullptr;
     FDGS_CUDA(fdgs::launch_sh_outer_sum(p, reinterpret_cast<cudaStream_t>(stream_v)), "sh_outer_sum");
     g_kernel_launches += 1;
     return FDGS_OK;
@@ -892,6 +1199,23 @@ int fdgs_debug_export_binning(const char* binning_buffer, const char* image_buff
     if (ranges) FDGS_CUDA(cudaMemcpyAsync(ranges, img.ranges, tiles * 8, cudaMemcpyDeviceToDevice, stream), "export ranges");
     if (n_contrib)
         FDGS_CUDA(cudaMemcpyAsync(n_contrib, img.n_contrib, (size_t)W * H * 4, cudaMemcpyDeviceToDevice, stream),
+                  "export n_contrib");
+    return FDGS_OK;
+}
+
+int fdgs_debug_export_binning_view(const char* image_buffer, int width, int height, int B, int view, unsigned int* ranges,
+                                   unsigned int* n_contrib, void* stream_v) {
+    g_last_error.clear();
+    if (!image_buffer || width <= 0 || height <= 0 || B < 1 || view < 0 || view >= B)
+        return fail(FDGS_ERR_INVALID_ARG, "bad image buffer / size / view");
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
+    ImageState img = ImageState::carve(align128(const_cast<char*>(image_buffer)), width, height, B);
+    const size_t tiles = img.tiles / (size_t)B, N = (size_t)width * height;
+    if (ranges)
+        FDGS_CUDA(cudaMemcpyAsync(ranges, img.ranges + (size_t)view * tiles, tiles * 8, cudaMemcpyDeviceToDevice, stream),
+                  "export ranges");
+    if (n_contrib)
+        FDGS_CUDA(cudaMemcpyAsync(n_contrib, img.n_contrib + (size_t)view * N, N * 4, cudaMemcpyDeviceToDevice, stream),
                   "export n_contrib");
     return FDGS_OK;
 }

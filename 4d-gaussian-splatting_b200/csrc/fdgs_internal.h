@@ -30,6 +30,19 @@ inline cudaError_t ensure_dynamic_smem(Kernel kernel, int bytes, PerDeviceOnce& 
 // SM count of the current device (132 on an H100), cached per device ordinal
 int device_sm_count();
 
+// ---- batched views (fdgs_forward_batch / fdgs_backward_batch) --------------------------------------------------
+// The per-view scalars of a batch, one 32-byte row per view in device memory (uploaded by the forward into the geometry
+// buffer).  focal_x / focal_y are computed on the host exactly as the single-view entry computes them.
+struct ViewScalars {
+    float timestamp, tan_fovx, tan_fovy, focal_x, focal_y, pad[3];
+};
+// Batched kernels run one view per blockIdx.y (per-Gaussian kernels) or blockIdx.z (tile kernels); every per-view
+// array is a [B][...] stack with the stride of one view's array.  The single-view instantiations never read these.
+struct ViewBatch {
+    int B;                      // views
+    const ViewScalars* scalars; // [B] device
+};
+
 // ---- forward preprocess ---------------------------------------------------------------------
 struct PreprocessFwdParams {
     int P, D, D_t, M;
@@ -69,6 +82,9 @@ struct PreprocessFwdParams {
     uint32_t* tiles_touched;
     uint4* binrec;          // [P] compact bin record of EVERY Gaussian (see launch_bin_count)
     int tile_cull;          // != 0: list a Gaussian only in the tiles its alpha >= 1/255 footprint reaches (fdgs_set_tile_cull)
+    // batched entry (vb.scalars != NULL): viewmatrix / projmatrix / cam_pos are [B,16] / [B,16] / [B,3] tables, the
+    // camera scalars come from vb.scalars, and every output above is a [B][P] stack
+    ViewBatch vb;
 };
 cudaError_t launch_preprocess_fwd(const PreprocessFwdParams& p, cudaStream_t stream);
 cudaError_t launch_debug_activate(int n, const float* log_s, const float* logit, const float* quat, int mode, float* s_out,
@@ -79,16 +95,22 @@ cudaError_t launch_debug_activate(int n, const float* log_s, const float* logit,
 int bin_ctas();                                 // rows of the [bin_ctas()][num_tiles] count matrix
 // binrec[i] = { x0 | y0 << 16, x1 | y1 << 16, depth bits, tile mask }: tile rectangle (empty = not listed anywhere) of
 // Gaussian i; for rectangles of up to 32 tiles bit j of the mask = tile j (row-major) takes an instance
-cudaError_t launch_bin_count(int P, const uint4* binrec, int grid_x, int grid_y, uint32_t* matrix, cudaStream_t stream);
+// views > 1 (the batched entry, any views >= 1 with batch = true): binrec is a [views][P] stack, the matrix has
+// views * grid_x * grid_y columns and view v's tiles are the columns v * tiles .. v * tiles + tiles - 1
+cudaError_t launch_bin_count(int P, const uint4* binrec, int grid_x, int grid_y, uint32_t* matrix, cudaStream_t stream,
+                             int views = 1, bool batch = false);
 // matrix -> per-CTA column prefixes; tile_offset / ranges; info[0] = total instances R, info[1] = largest tile
 cudaError_t launch_tile_scan(int num_tiles, uint32_t* matrix, uint32_t* tile_total, uint32_t* tile_offset, uint2* ranges,
                              uint32_t* info, cudaStream_t stream);
 cudaError_t launch_bin_scatter(int P, const uint4* binrec, int grid_x, int grid_y, uint32_t* matrix,
-                               const uint32_t* tile_offset, uint64_t* keys, cudaStream_t stream);
-// sorts every tile's keys and writes the 64-byte instance records + the sorted index list
+                               const uint32_t* tile_offset, uint64_t* keys, cudaStream_t stream, int views = 1,
+                               bool batch = false);
+// sorts every tile's keys and writes the 64-byte instance records + the sorted index list.  tiles_per_view > 0 (the
+// batched entry): num_tiles = views * tiles_per_view and tile t gathers from grec's view slice t / tiles_per_view
 int tile_sort_pack_kernel_count(int max_count);
 cudaError_t launch_tile_sort_pack(int num_tiles, int max_count, int R, const uint2* ranges, uint64_t* keys,
-                                  const InstRec* grec, StageRec* recs, uint32_t* point_list, cudaStream_t stream);
+                                  const InstRec* grec, StageRec* recs, uint32_t* point_list, cudaStream_t stream,
+                                  int tiles_per_view = 0, int P = 0);
 cudaError_t launch_unpack_grec(int P, const InstRec* grec, const int* radii, float* depths, float* means2D,
                                float* conic_opacity, float* rgb, cudaStream_t stream);
 
@@ -105,6 +127,7 @@ struct BlendFwdParams {
     float* out_depth;      // [H,W]
     float* out_T;          // [H,W]
     const float* bg_image; // [3,H,W] per-pixel background behind the Gaussians, or NULL
+    int views;             // > 0: batched entry, blockIdx.z = view; ranges and every image are [views] stacks
 };
 cudaError_t launch_blend_fwd(const BlendFwdParams& p, cudaStream_t stream);
 
@@ -126,6 +149,8 @@ struct BlendBwdParams {
     float* dL_dflows;     // [P,2]
     const float* bg_image;   // [3,H,W] or NULL (BlendFwdParams::bg_image)
     float* dL_dbg_image;     // [3,H,W] overwritten for every pixel, or NULL
+    int views;               // > 0: batched entry, blockIdx.z = view; images and the five gradients are [views] stacks
+    int P;                   // Gaussians per view (the batched entry's gradient stride)
 };
 cudaError_t launch_blend_bwd(const BlendBwdParams& p, cudaStream_t stream);
 // true when launch_blend_bwd(p) leaves RAW moment sums (W10, W01 | W20, W11, W02 | W00 of w = G dL/dalpha
@@ -179,9 +204,24 @@ struct PreprocessBwdParams {
     float* dL_dscale_t;
     float* dL_drot;
     float* dL_drot_r;
+    // batched entry (vb.scalars != NULL): cameras as in PreprocessFwdParams, every per-Gaussian input of the forward and
+    // every output above is a [B][P] stack, sh_factors a [B][factor_stride] stack whose view block ends with the
+    // view's timestamp and camera position at offset 3 P (the ShSumParams table)
+    ViewBatch vb;
+    long long factor_stride;
 };
 cudaError_t launch_preprocess_bwd(const PreprocessBwdParams& p, cudaStream_t stream);
 int preprocess_bwd_kernel_count(const PreprocessBwdParams& p);
+// dst_i[e] = ((src_i[0][e] + src_i[1][e]) + src_i[2][e]) + ... in fp32, view order: the order in which autograd's
+// AccumulateGrad builds .grad over a sequential loop of views.  src_i is a [B][n_i] stack.
+constexpr int VIEW_SUM_MAX = 8;
+struct ViewSumParams {
+    int n, B;
+    const float* src[VIEW_SUM_MAX];
+    float* dst[VIEW_SUM_MAX];
+    long long count[VIEW_SUM_MAX];   // elements per view
+};
+cudaError_t launch_view_sum(const ViewSumParams& p, cudaStream_t stream);
 
 // ---- view-parallel SH gradient (preprocess_bwd.cu: sh_outer_sum_kernel) -----------------------------------------
 struct ShSumParams {
@@ -204,6 +244,9 @@ struct ShSumParams {
     int m0;                   // coefficients 0 .. m0-1 of a row live in out0 ...
     float* out1;              // ... the rest in out1 [P, M - m0, 3] (NULL when m0 == M)
     int accumulate;           // add to the tensors' contents instead of overwriting them
+    // batched entry: view_means != NULL takes view v's direction from the shifted means the forward wrote,
+    // view_means[v][3 P]; union_idx / slot_of may then be NULL, meaning every row (K = P, the identity map)
+    const float* view_means;
 };
 cudaError_t launch_sh_outer_sum(const ShSumParams& p, cudaStream_t stream);
 // flag[0] |= 1 if any row r with mask[r] == 0 of any of the n tensors has a non-zero element

@@ -209,8 +209,48 @@ __device__ __forceinline__ void sh_row_inplace(float4* rowq, int nq, const ShCtx
 // read: the direction / time gradients need sum_k dbasis_k (sh_k . dRGB).
 // STAGE as in preprocess_fwd_kernel: 0 = global memory coefficient by coefficient, 1 = cp.async.bulk rows in and out,
 // 2 = cooperative coalesced copies of split rows (features_dc | features_rest in, their two gradient tensors out).
-template <int STAGE, bool FACTORS>
-__global__ void __launch_bounds__(SB_THREADS, 6) sh_bwd_kernel(const PreprocessBwdParams a) {
+// view v of a batch (blockIdx.y): the view's camera and its slices of the forward's per-Gaussian state and of every
+// gradient (see PreprocessBwdParams::vb)
+__device__ __forceinline__ PreprocessBwdParams preprocess_bwd_view(PreprocessBwdParams a, int v) {
+    const size_t P = (size_t)a.P;
+    const ViewScalars vs = a.vb.scalars[v];
+    a.viewmatrix += 16 * v;
+    a.projmatrix += 16 * v;
+    a.campos += 3 * v;
+    a.timestamp = vs.timestamp;
+    a.tan_fovx = vs.tan_fovx;
+    a.tan_fovy = vs.tan_fovy;
+    a.focal_x = vs.focal_x;
+    a.focal_y = vs.focal_y;
+    a.means3D += 3 * v * P;
+    a.radii += v * P;
+    a.clamped += v * P;
+    a.tiles_touched += v * P;
+    a.cov3D += 6 * v * P;
+    a.grec += v * P;
+    a.dL_dmean2D += 3 * v * P;
+    a.dL_dconic += 4 * v * P;
+    a.dL_dopacity += v * P;
+    a.dL_dcolor += 3 * v * P;
+    a.dL_dmean3D += 3 * v * P;
+    a.dL_dcov3D += 6 * v * P;
+    if (a.sh_factors) a.sh_factors += v * a.factor_stride;
+    a.dL_dts += v * P;
+    a.dL_dscale += 3 * v * P;
+    a.dL_dscale_t += v * P;
+    a.dL_drot += 4 * v * P;
+    a.dL_drot_r += 4 * v * P;
+    return a;
+}
+
+// BATCH: one view per blockIdx.y (FACTORS only: the SH rows of a batch are summed over its views by sh_outer_sum)
+template <int STAGE, bool FACTORS, bool BATCH>
+__device__ __forceinline__ void sh_bwd_body(const PreprocessBwdParams& a_) {
+    static_assert(!BATCH || FACTORS, "a batch emits colour factors");
+    // an lvalue on both sides: the single-view instantiation reads its parameters in place, no copy
+    PreprocessBwdParams view_;
+    if (BATCH) view_ = preprocess_bwd_view(a_, blockIdx.y);
+    const PreprocessBwdParams& a = BATCH ? view_ : a_;
     constexpr bool BULK = STAGE == 1;
     constexpr bool SPLIT = STAGE == 2;
     __shared__ int slot_idx[SB_CAP];   // STAGE 2: Gaussian whose row occupies each slot
@@ -244,6 +284,14 @@ __global__ void __launch_bounds__(SB_THREADS, 6) sh_bwd_kernel(const PreprocessB
     slot_of[tid] = (short)my_rank;
     __syncthreads();
 
+    if (BATCH && blockIdx.x == 0 && tid == 0) {
+        // the view's metadata row of the sh_outer_sum table, after its P colour factors
+        float* meta = a.sh_factors + 3 * (size_t)a.P;
+        meta[0] = a.timestamp;
+        meta[1] = a.campos[0];
+        meta[2] = a.campos[1];
+        meta[3] = a.campos[2];
+    }
     // zero rows: every float4 of every non-rendered row of this CTA, coalesced
     if (FACTORS) {
         if (in_range && !vis) {
@@ -387,6 +435,17 @@ __global__ void __launch_bounds__(SB_THREADS, 6) sh_bwd_kernel(const PreprocessB
     }
 }
 
+template <int STAGE, bool FACTORS>
+__global__ void __launch_bounds__(SB_THREADS, 6) sh_bwd_kernel(const PreprocessBwdParams a_) {
+    sh_bwd_body<STAGE, FACTORS, false>(a_);
+}
+
+// the batched entry (fdgs_forward_batch / fdgs_backward_batch): one view per blockIdx.y
+template <int STAGE>
+__global__ void __launch_bounds__(SB_THREADS, 6) sh_bwd_batch_kernel(const PreprocessBwdParams a_) {
+    sh_bwd_body<STAGE, true, true>(a_);
+}
+
 // ---- view-parallel SH gradient: rebuild and sum the rows of all views -------------------------------------------
 // dL_dsh of ONE view is rank one per Gaussian: row[k][ch] = w_k(view direction, time) * dRGB[ch]  (sh_row_inplace
 // above).  With the views of a step spread over ranks (fdgs/dist.py) only dRGB travels (3 floats per Gaussian and
@@ -405,7 +464,7 @@ __global__ void __launch_bounds__(256) sh_outer_dir_kernel(const ShSumParams a) 
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (long long)a.K * a.V) return;
     const int k = (int)(t / a.V), v = (int)(t - (long long)k * a.V);
-    const long long idx = a.union_idx[k];
+    const long long idx = a.union_idx ? a.union_idx[k] : k;
     const float* blk = a.table + (size_t)v * a.view_stride;
     const float r = blk[3 * (size_t)k + 0], g = blk[3 * (size_t)k + 1], b = blk[3 * (size_t)k + 2];
     float4 o0 = make_float4(0.f, 0.f, 1.f, 0.f), o1 = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -415,7 +474,11 @@ __global__ void __launch_bounds__(256) sh_outer_dir_kernel(const ShSumParams a) 
         const float timestamp = meta[0];
         const float t_g = (a.ts != nullptr) ? a.ts[idx] : 0.f;
         float mx = a.means3D[3 * idx + 0], my = a.means3D[3 * idx + 1], mz = a.means3D[3 * idx + 2];
-        if (a.rot_4d) {
+        if (a.view_means) {
+            // the shifted mean this view's forward wrote: exactly what sh_ctx_init() read
+            const float* vm = a.view_means + (size_t)v * 3 * a.P + 3 * idx;
+            mx = vm[0]; my = vm[1]; mz = vm[2];
+        } else if (a.rot_4d) {
             // the forward's mean shift (preprocess_fwd.cu), same intrinsics, same order
             const float mod = a.scale_modifier;
             Sigma4 S;
@@ -536,7 +599,7 @@ __global__ void __launch_bounds__(128) sh_outer_sum_kernel(const ShSumParams a, 
         else if (kg == 1) sh_outer_accumulate<1>(a, k, acc);
         else if (kg == 2) sh_outer_accumulate<2>(a, k, acc);
         else sh_outer_accumulate<3>(a, k, acc);
-        my_idx = a.union_idx[k];     // the destination row of lane `lane`'s Gaussian (shuffled to the storing warp below)
+        my_idx = a.union_idx ? a.union_idx[k] : k;     // the destination row of lane `lane`'s Gaussian (shuffled to the storing warp below)
     }
     // stage: coefficients 16 b + 4 kg + j of the row -> floats 48 b + 12 kg + 3 j + ch
     {
@@ -566,7 +629,12 @@ __device__ __forceinline__ void mat3_mul(const float A[3][3], const float B[3][3
 }
 
 // ---- geometry backward ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(GB_THREADS, 8) geom_bwd_kernel(const PreprocessBwdParams a, const int has_sh_part) {
+template <bool BATCH>
+__device__ __forceinline__ void geom_bwd_body(const PreprocessBwdParams& a_, const int has_sh_part) {
+    // an lvalue on both sides: the single-view instantiation reads its parameters in place, no copy
+    PreprocessBwdParams view_;
+    if (BATCH) view_ = preprocess_bwd_view(a_, blockIdx.y);
+    const PreprocessBwdParams& a = BATCH ? view_ : a_;
     const int idx = blockIdx.x * GB_THREADS + threadIdx.x;
     if (idx >= a.P) return;
     const bool vis = (a.radii[idx] > 0) && (a.tiles_touched[idx] != 0u);
@@ -808,6 +876,27 @@ __global__ void __launch_bounds__(GB_THREADS, 8) geom_bwd_kernel(const Preproces
     reinterpret_cast<float4*>(a.dL_drot_r)[idx] = make_float4(g_rotr[0], g_rotr[1], g_rotr[2], g_rotr[3]);
 }
 
+__global__ void __launch_bounds__(GB_THREADS, 8) geom_bwd_kernel(const PreprocessBwdParams a_, const int has_sh_part) {
+    geom_bwd_body<false>(a_, has_sh_part);
+}
+
+// the batched entry (fdgs_forward_batch / fdgs_backward_batch): one view per blockIdx.y
+__global__ void __launch_bounds__(GB_THREADS, 8) geom_bwd_batch_kernel(const PreprocessBwdParams a_, const int has_sh_part) {
+    geom_bwd_body<true>(a_, has_sh_part);
+}
+
+// one thread per element of a tensor (blockIdx.y), its B view rows added in view order with round-to-nearest adds
+__global__ void __launch_bounds__(256) view_sum_kernel(const ViewSumParams p) {
+    const int i = blockIdx.y;
+    const long long n = p.count[i];
+    const float* __restrict__ src = p.src[i];
+    for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
+        float s = src[e];
+        for (int v = 1; v < p.B; ++v) s = __fadd_rn(s, src[(size_t)v * n + e]);
+        p.dst[i][e] = s;
+    }
+}
+
 // reference: rasterizer_impl.cu:54-67 checkFrustum + auxiliary.h:140-163
 __global__ void mark_visible_kernel(int P, const float* __restrict__ means, const float* __restrict__ V,
                                     unsigned char* __restrict__ present) {
@@ -823,37 +912,54 @@ int preprocess_bwd_kernel_count(const PreprocessBwdParams& p) {
     return (p.shs != nullptr && p.M > 0 && (p.dL_dsh != nullptr || p.sh_factors != nullptr)) ? 2 : 1;
 }
 
-cudaError_t launch_preprocess_bwd(const PreprocessBwdParams& p, cudaStream_t stream) {
-    if (p.P <= 0) return cudaSuccess;
+using PreprocessBwdKernel = void (*)(const PreprocessBwdParams);
+using PreprocessBwdKernelG = void (*)(const PreprocessBwdParams, const int);
+
+// the SH backward of one staging mode: dense rows or colour factors, or the batched entry's per-view factors
+template <int STAGE, bool BATCH>
+static PreprocessBwdKernel sh_bwd_for(bool factors) {
+    if (BATCH) return sh_bwd_batch_kernel<STAGE>;
+    return factors ? sh_bwd_kernel<STAGE, true> : sh_bwd_kernel<STAGE, false>;
+}
+
+template <bool BATCH>
+static cudaError_t preprocess_bwd(const PreprocessBwdParams& p, cudaStream_t stream) {
     const bool factors = p.sh_factors != nullptr;
     const bool has_sh = p.shs != nullptr && p.M > 0 && (p.dL_dsh != nullptr || factors);
+    const unsigned views = BATCH ? (unsigned)p.vb.B : 1u;
     if (has_sh) {
-        const int blocks = (p.P + SB_THREADS - 1) / SB_THREADS;
+        const dim3 blocks((p.P + SB_THREADS - 1) / SB_THREADS, views);
         const bool split = p.shs_rest != nullptr;
         if (p.sh_bulk_ok && (!split || p.M % 16 == 0)) {
             const size_t smem = (size_t)SB_CAP * p.sh_row_stride_floats * sizeof(float);
             static PerDeviceOnce once[4];
-            cudaError_t e0;
-            if (split) e0 = factors ? ensure_dynamic_smem(sh_bwd_kernel<2, true>, 200 * 1024, once[3])
-                                    : ensure_dynamic_smem(sh_bwd_kernel<2, false>, 200 * 1024, once[2]);
-            else e0 = factors ? ensure_dynamic_smem(sh_bwd_kernel<1, true>, 200 * 1024, once[1])
-                              : ensure_dynamic_smem(sh_bwd_kernel<1, false>, 200 * 1024, once[0]);
+            const PreprocessBwdKernel k = split ? sh_bwd_for<2, BATCH>(factors) : sh_bwd_for<1, BATCH>(factors);
+            cudaError_t e0 = ensure_dynamic_smem(k, 200 * 1024, once[2 * split + factors]);
             if (e0 != cudaSuccess) return e0;
-            if (split) {
-                if (factors) sh_bwd_kernel<2, true><<<blocks, SB_THREADS, smem, stream>>>(p);
-                else sh_bwd_kernel<2, false><<<blocks, SB_THREADS, smem, stream>>>(p);
-            } else {
-                if (factors) sh_bwd_kernel<1, true><<<blocks, SB_THREADS, smem, stream>>>(p);
-                else sh_bwd_kernel<1, false><<<blocks, SB_THREADS, smem, stream>>>(p);
-            }
+            k<<<blocks, SB_THREADS, smem, stream>>>(p);
         } else {
-            if (factors) sh_bwd_kernel<0, true><<<blocks, SB_THREADS, 0, stream>>>(p);
-            else sh_bwd_kernel<0, false><<<blocks, SB_THREADS, 0, stream>>>(p);
+            sh_bwd_for<0, BATCH>(factors)<<<blocks, SB_THREADS, 0, stream>>>(p);
         }
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
-    geom_bwd_kernel<<<(p.P + GB_THREADS - 1) / GB_THREADS, GB_THREADS, 0, stream>>>(p, has_sh ? 1 : 0);
+    const PreprocessBwdKernelG g = BATCH ? geom_bwd_batch_kernel : geom_bwd_kernel;
+    g<<<dim3((p.P + GB_THREADS - 1) / GB_THREADS, views), GB_THREADS, 0, stream>>>(p, has_sh ? 1 : 0);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_preprocess_bwd(const PreprocessBwdParams& p, cudaStream_t stream) {
+    if (p.P <= 0) return cudaSuccess;
+    return p.vb.scalars ? preprocess_bwd<true>(p, stream) : preprocess_bwd<false>(p, stream);
+}
+
+cudaError_t launch_view_sum(const ViewSumParams& p, cudaStream_t stream) {
+    if (p.n <= 0) return cudaSuccess;
+    long long most = 0;
+    for (int i = 0; i < p.n; ++i) most = p.count[i] > most ? p.count[i] : most;
+    if (most <= 0) return cudaSuccess;
+    const long long blocks = (most + 255) / 256;
+    view_sum_kernel<<<dim3((unsigned)(blocks < 65535 * 16 ? blocks : 65535 * 16), p.n), 256, 0, stream>>>(p);
     return cudaGetLastError();
 }
 
@@ -862,7 +968,8 @@ cudaError_t launch_sh_outer_sum(const ShSumParams& p, cudaStream_t stream) {
     if ((long long)p.K * p.V > 0)
         sh_outer_dir_kernel<<<(unsigned)(((long long)p.K * p.V + 255) / 256), 256, 0, stream>>>(p);
     const int union_blocks = (int)(((long long)p.K + SO_ROWS - 1) / SO_ROWS);
-    const int zero_blocks = (int)(((long long)p.P + 127) / 128);
+    // without slot_of every row is in the union (K = P): no zero rows
+    const int zero_blocks = p.slot_of ? (int)(((long long)p.P + 127) / 128) : 0;
     sh_outer_sum_kernel<<<(unsigned)(union_blocks + zero_blocks), 128, 0, stream>>>(p, union_blocks);
     return cudaGetLastError();
 }

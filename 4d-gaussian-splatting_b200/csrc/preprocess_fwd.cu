@@ -191,8 +191,34 @@ __device__ __forceinline__ void sh_color_3d(const Row& row, int M, int deg, floa
 // coefficient by coefficient: odd row sizes), 1: one cp.async.bulk per row (TMA 1-D; contiguous 16-byte-aligned rows),
 // 2: cooperative coalesced copy by the whole CTA (split rows features_dc | features_rest of the raw-parameter entry:
 // 12-byte and 564-byte pieces, which the bulk-copy engine cannot address).
-template <int STAGE>
-__global__ void __launch_bounds__(PRE_THREADS, 5) preprocess_fwd_kernel(const PreprocessFwdParams a) {
+// view v of a batch (blockIdx.y): the view's camera and its slices of every per-Gaussian output
+__device__ __forceinline__ PreprocessFwdParams preprocess_fwd_view(PreprocessFwdParams a, int v) {
+    const size_t P = (size_t)a.P;
+    const ViewScalars vs = a.vb.scalars[v];
+    a.viewmatrix += 16 * v;
+    a.projmatrix += 16 * v;
+    a.cam_pos += 3 * v;
+    a.timestamp = vs.timestamp;
+    a.tan_fovx = vs.tan_fovx;
+    a.tan_fovy = vs.tan_fovy;
+    a.focal_x = vs.focal_x;
+    a.focal_y = vs.focal_y;
+    a.out_means3D += 3 * v * P;
+    a.radii += v * P;
+    a.cov3D += 6 * v * P;
+    a.grec += v * P;
+    a.clamped += v * P;
+    a.tiles_touched += v * P;
+    a.binrec += v * P;
+    return a;
+}
+
+template <int STAGE, bool BATCH>
+__device__ __forceinline__ void preprocess_fwd_body(const PreprocessFwdParams& a_) {
+    // an lvalue on both sides: the single-view instantiation reads its parameters in place, no copy
+    PreprocessFwdParams view_;
+    if (BATCH) view_ = preprocess_fwd_view(a_, blockIdx.y);
+    const PreprocessFwdParams& a = BATCH ? view_ : a_;
     constexpr bool BULK = STAGE == 1;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ __align__(8) uint64_t bar;
@@ -517,6 +543,17 @@ __global__ void __launch_bounds__(PRE_THREADS, 5) preprocess_fwd_kernel(const Pr
     }
 }
 
+template <int STAGE>
+__global__ void __launch_bounds__(PRE_THREADS, 5) preprocess_fwd_kernel(const PreprocessFwdParams a_) {
+    preprocess_fwd_body<STAGE, false>(a_);
+}
+
+// the batched entry (fdgs_forward_batch / fdgs_backward_batch): one view per blockIdx.y
+template <int STAGE>
+__global__ void __launch_bounds__(PRE_THREADS, 5) preprocess_fwd_batch_kernel(const PreprocessFwdParams a_) {
+    preprocess_fwd_body<STAGE, true>(a_);
+}
+
 }  // namespace
 
 // test hook: the in-kernel activations of the raw-parameter entry, applied to plain arrays (tests compare them with
@@ -538,26 +575,32 @@ cudaError_t launch_debug_activate(int n, const float* log_s, const float* logit,
     return cudaGetLastError();
 }
 
+template <int STAGE, bool BATCH>
+static cudaError_t preprocess_fwd_stage(const PreprocessFwdParams& p, dim3 blocks, size_t smem, PerDeviceOnce* once,
+                                        cudaStream_t stream) {
+    const auto k = BATCH ? preprocess_fwd_batch_kernel<STAGE> : preprocess_fwd_kernel<STAGE>;
+    if (once) {
+        cudaError_t e = ensure_dynamic_smem(k, 200 * 1024, *once);
+        if (e != cudaSuccess) return e;
+    }
+    k<<<blocks, PRE_THREADS, smem, stream>>>(p);
+    return cudaGetLastError();
+}
+
+template <bool BATCH>
+static cudaError_t preprocess_fwd(const PreprocessFwdParams& p, cudaStream_t stream) {
+    const dim3 blocks((p.P + PRE_THREADS - 1) / PRE_THREADS, BATCH ? p.vb.B : 1);
+    const bool staged = p.sh_bulk_ok && p.colors_precomp == nullptr;   // shared-memory staging possible (see sh_staging)
+    if (!staged) return preprocess_fwd_stage<0, BATCH>(p, blocks, 0, nullptr, stream);
+    const size_t smem = (size_t)PRE_CAP * p.sh_row_stride_floats * sizeof(float);
+    static PerDeviceOnce once1, once2;
+    return p.shs_rest ? preprocess_fwd_stage<2, BATCH>(p, blocks, smem, &once2, stream)
+                      : preprocess_fwd_stage<1, BATCH>(p, blocks, smem, &once1, stream);
+}
+
 cudaError_t launch_preprocess_fwd(const PreprocessFwdParams& p, cudaStream_t stream) {
     if (p.P <= 0) return cudaSuccess;
-    const int blocks = (p.P + PRE_THREADS - 1) / PRE_THREADS;
-    const bool staged = p.sh_bulk_ok && p.colors_precomp == nullptr;   // shared-memory staging possible (see sh_staging)
-    if (staged) {
-        const size_t smem = (size_t)PRE_CAP * p.sh_row_stride_floats * sizeof(float);
-        static PerDeviceOnce once1, once2;
-        if (p.shs_rest) {
-            cudaError_t e = ensure_dynamic_smem(preprocess_fwd_kernel<2>, 200 * 1024, once2);
-            if (e != cudaSuccess) return e;
-            preprocess_fwd_kernel<2><<<blocks, PRE_THREADS, smem, stream>>>(p);
-        } else {
-            cudaError_t e = ensure_dynamic_smem(preprocess_fwd_kernel<1>, 200 * 1024, once1);
-            if (e != cudaSuccess) return e;
-            preprocess_fwd_kernel<1><<<blocks, PRE_THREADS, smem, stream>>>(p);
-        }
-    } else {
-        preprocess_fwd_kernel<0><<<blocks, PRE_THREADS, 0, stream>>>(p);
-    }
-    return cudaGetLastError();
+    return p.vb.scalars ? preprocess_fwd<true>(p, stream) : preprocess_fwd<false>(p, stream);
 }
 
 }  // namespace fdgs

@@ -16,6 +16,10 @@
 //   rasterize_gaussians_backward_ext(37 args, sh_rest, raw_params, bg_image, sh_factor_mode, want_dbg)
 //                                         -> [12 gradients, sh_factors, dL_dsh_rest, dL_dbg_image]
 //
+// and a batched pair over B cameras of the same Gaussians (include/fdgs.h: fdgs_forward_batch):
+//
+//   rasterize_gaussians_batch / rasterize_gaussians_backward_batch
+//
 // PyTorch is plumbing only: it owns the memory (tensors, the three growable byte buffers handed
 // to the library through the allocation callback) and supplies the current CUDA stream.  No
 // arithmetic happens here.  Differences from the reference shim, all performance-motivated and
@@ -334,6 +338,206 @@ RasterizeGaussiansBackwardCUDA(const torch::Tensor& background, const torch::Ten
         gaussian_dim, force_sh_3d, geomBuffer, R, binningBuffer, imageBuffer, debug, torch::Tensor(), false,
         torch::Tensor(), false, false);
     return std::make_tuple(o[0], o[1], o[2], o[3], o[4], o[5], o[6], o[7], o[8], o[9], o[10], o[11]);
+}
+
+// ---- batched views (include/fdgs.h: fdgs_forward_batch / fdgs_backward_batch) ---------------------------------------
+// The cameras are strict: viewmatrix / projmatrix [B,16] (or [B,4,4]) and campos [B,3] float32 CUDA tensors on the
+// Gaussians' device, timestamps / tanfovx / tanfovy [B] float32 CPU tensors; bg_image empty or [B,3,H,W].  Checked before
+// anything is allocated or launched.
+namespace {
+struct BatchCams {
+    int B;
+    const float *view, *proj, *campos, *timestamps, *tanfovx, *tanfovy;
+};
+
+BatchCams batch_cameras(const torch::Tensor& means3D, const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix,
+                        const torch::Tensor& campos, const torch::Tensor& timestamps, const torch::Tensor& tanfovx,
+                        const torch::Tensor& tanfovy) {
+    TORCH_CHECK(viewmatrix.defined() && viewmatrix.dim() >= 1, "fdgs: viewmatrix must be [B,16]");
+    BatchCams c;
+    const int64_t B = viewmatrix.size(0);
+    TORCH_CHECK(B >= 1 && B <= 65535, "fdgs: the view count B must be in [1, 65535]");
+    c.B = (int)B;
+    c.view = arg<float>(viewmatrix, "viewmatrix", B, 16 * B, REQUIRED);
+    c.proj = arg<float>(projmatrix, "projmatrix", B, 16 * B, REQUIRED);
+    c.campos = arg<float>(campos, "campos", B, 3 * B, REQUIRED);
+    c.timestamps = arg<float>(timestamps, "timestamps", B, B, REQUIRED);
+    c.tanfovx = arg<float>(tanfovx, "tanfovx", B, B, REQUIRED);
+    c.tanfovy = arg<float>(tanfovy, "tanfovy", B, B, REQUIRED);
+    TORCH_CHECK(!timestamps.is_cuda() && !tanfovx.is_cuda() && !tanfovy.is_cuda(),
+                "fdgs: timestamps / tanfovx / tanfovy must be CPU tensors");
+    TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor");
+    same_cuda_device("batched camera", {means3D, viewmatrix, projmatrix, campos});
+    return c;
+}
+
+const float* batch_bg_image(const torch::Tensor& bg_image, const torch::Tensor& means3D, int B, int H, int W) {
+    if (!bg_image.defined() || bg_image.numel() == 0) return nullptr;
+    TORCH_CHECK(bg_image.dim() == 4 && bg_image.size(0) == B && bg_image.size(1) == 3 && bg_image.size(2) == H &&
+                    bg_image.size(3) == W,
+                "fdgs: bg_image must be [B, 3, image_height, image_width]");
+    const float* p = arg<float>(bg_image, "bg_image");
+    same_cuda_device("bg_image", {means3D, bg_image});
+    return p;
+}
+}  // namespace
+
+// B views of the same Gaussians: (num_rendered, color [B,3,H,W], flow [B,2,H,W], depth [B,1,H,W], T [B,1,H,W],
+// radii [B,P], geomBuffer, binningBuffer, imgBuffer, out_means3D [B,P,3]).  Gaussian inputs as in rasterize_gaussians_ext
+// (SH and scales / rotations only: no precomputed colours or covariances).
+std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor,
+           torch::Tensor, torch::Tensor>
+RasterizeGaussiansBatch(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& flows,
+                        const torch::Tensor& opacity, const torch::Tensor& ts, const torch::Tensor& scales,
+                        const torch::Tensor& scales_t, const torch::Tensor& rotations, const torch::Tensor& rotations_r,
+                        const float scale_modifier, const float prefilter_var, const torch::Tensor& viewmatrix,
+                        const torch::Tensor& projmatrix, const torch::Tensor& campos, const torch::Tensor& timestamps,
+                        const torch::Tensor& tanfovx, const torch::Tensor& tanfovy, const int image_height,
+                        const int image_width, const torch::Tensor& sh, const torch::Tensor& sh_rest, const int degree,
+                        const int degree_t, const float time_duration, const bool rot_4d, const int gaussian_dim,
+                        const bool force_sh_3d, const bool prefiltered, const bool debug, const bool raw_params,
+                        const torch::Tensor& bg_image) {
+    TORCH_CHECK(means3D.dim() == 2 && means3D.size(1) == 3, "means3D must have dimensions (num_points, 3)");
+    const BatchCams cams = batch_cameras(means3D, viewmatrix, projmatrix, campos, timestamps, tanfovx, tanfovy);
+    const int B = cams.B, P = means3D.size(0), H = image_height, W = image_width;
+    TORCH_CHECK(H > 0 && W > 0, "fdgs: bad image size");
+    const float* bgi = batch_bg_image(bg_image, means3D, B, H, W);
+    const DeviceStream on(means3D);
+    auto fopts = means3D.options().dtype(torch::kFloat32);
+    auto bopts = means3D.options().dtype(torch::kByte);
+    torch::Tensor out_color = torch::empty({B, 3, H, W}, fopts);
+    torch::Tensor out_flow = torch::empty({B, 2, H, W}, fopts);
+    torch::Tensor out_depth = torch::empty({B, 1, H, W}, fopts);
+    torch::Tensor out_T = torch::empty({B, 1, H, W}, fopts);
+    torch::Tensor radii = torch::empty({B, P}, means3D.options().dtype(torch::kInt32));
+    torch::Tensor out_means3D = torch::empty({B, P, 3}, fopts);
+    torch::Tensor geomBuffer = torch::empty({0}, bopts), binningBuffer = torch::empty({0}, bopts),
+                  imgBuffer = torch::empty({0}, bopts);
+    const auto bg_c = contig(background), means_c = contig(means3D), flow_c = contig(flows), op_c = contig(opacity),
+               ts_c = contig(ts), sc_c = contig(scales), sct_c = contig(scales_t), rot_c = contig(rotations),
+               rotr_c = contig(rotations_r), sh_c = contig(sh), shr_c = contig(sh_rest);
+    fdgs_forward_batch_args b;
+    memset(&b, 0, sizeof(b));
+    fdgs_forward_args& a = b.view;
+    a.P = P; a.D = degree; a.D_t = degree_t;
+    a.M = (sh.defined() && sh.numel() != 0) ? (int)sh.size(1) : 0;
+    if (shr_c.defined() && shr_c.numel() != 0) {
+        TORCH_CHECK(a.M == 1 && shr_c.dim() == 3 && shr_c.size(0) == P, "fdgs: split SH rows are [P,1,3] + [P,M-1,3]");
+        a.M += (int)shr_c.size(1);
+        a.shs_rest = fptr(shr_c);
+    }
+    a.raw_params = raw_params;
+    a.background = fptr(bg_c); a.width = W; a.height = H;
+    a.means3D = fptr(means_c); a.shs = fptr(sh_c); a.flows_precomp = fptr(flow_c);
+    a.opacities = fptr(op_c); a.ts = fptr(ts_c); a.scales = fptr(sc_c); a.scales_t = fptr(sct_c);
+    a.scale_modifier = scale_modifier; a.rotations = fptr(rot_c); a.rotations_r = fptr(rotr_c);
+    a.prefilter_var = prefilter_var;
+    a.viewmatrix = cams.view; a.projmatrix = cams.proj; a.cam_pos = cams.campos;
+    a.time_duration = time_duration; a.rot_4d = rot_4d; a.gaussian_dim = gaussian_dim;
+    a.force_sh_3d = force_sh_3d; a.prefiltered = prefiltered; a.debug = debug;
+    a.out_means3D = out_means3D.data_ptr<float>(); a.out_color = out_color.data_ptr<float>();
+    a.out_flow = out_flow.data_ptr<float>(); a.out_depth = out_depth.data_ptr<float>();
+    a.out_T = out_T.data_ptr<float>(); a.radii = radii.data_ptr<int>();
+    b.B = B; b.timestamps = cams.timestamps; b.tan_fovx = cams.tanfovx; b.tan_fovy = cams.tanfovy;
+    b.bg_image = bgi; b.bg_views = bgi ? B : 0;
+    fdgs_forward_result r;
+    check(fdgs_forward_batch(&b, resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer, (void*)on.stream, &r),
+          "forward_batch");
+    return std::make_tuple(r.num_rendered, out_color, out_flow, out_depth, out_T, radii, geomBuffer, binningBuffer, imgBuffer,
+                           out_means3D);
+}
+
+// Backward of rasterize_gaussians_batch.  Returns 11 tensors: dL_dmeans2D [B,P,3] per view, then the view sums
+// dL_dopacity [P,1], dL_dmeans3D [P,3], dL_dsh ([P,M,3], or [P,1,3] with sh_rest), dL_dsh_rest, dL_dts [P,1],
+// dL_dscales [P,3], dL_dscales_t [P,1], dL_drotations [P,4], dL_drotations_r [P,4], and dL_dbg_image [B,3,H,W] (empty
+// unless want_dbg).
+std::vector<torch::Tensor>
+RasterizeGaussiansBackwardBatch(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& out_means3D,
+                                const torch::Tensor& radii, const torch::Tensor& flows, const torch::Tensor& opacities,
+                                const torch::Tensor& ts, const torch::Tensor& scales, const torch::Tensor& scales_t,
+                                const torch::Tensor& rotations, const torch::Tensor& rotations_r, const float scale_modifier,
+                                const float prefilter_var, const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix,
+                                const torch::Tensor& campos, const torch::Tensor& timestamps, const torch::Tensor& tanfovx,
+                                const torch::Tensor& tanfovy, const torch::Tensor& dL_dout_color,
+                                const torch::Tensor& dL_dout_depth, const torch::Tensor& dL_dout_mask,
+                                const torch::Tensor& dL_dout_flow, const torch::Tensor& sh, const torch::Tensor& sh_rest,
+                                const int degree, const int degree_t, const float time_duration, const bool rot_4d,
+                                const int gaussian_dim, const bool force_sh_3d, const torch::Tensor& geomBuffer, const int R,
+                                const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer, const bool debug,
+                                const bool raw_params, const torch::Tensor& bg_image, const bool want_dbg) {
+    TORCH_CHECK(means3D.dim() == 2 && means3D.size(1) == 3, "means3D must have dimensions (num_points, 3)");
+    const BatchCams cams = batch_cameras(means3D, viewmatrix, projmatrix, campos, timestamps, tanfovx, tanfovy);
+    const int B = cams.B, P = means3D.size(0);
+    TORCH_CHECK(dL_dout_color.dim() == 4 && dL_dout_color.size(0) == B && dL_dout_color.size(1) == 3,
+                "fdgs: the colour gradient must be [B,3,H,W]");
+    const int H = dL_dout_color.size(2), W = dL_dout_color.size(3);
+    const float* bgi = batch_bg_image(bg_image, means3D, B, H, W);
+    const float* om = arg<float>(out_means3D, "out_means3D", B, 3ll * B * P, REQUIRED);
+    const int* rad = arg<int>(radii, "radii", B, (int64_t)B * P, REQUIRED);
+    const auto gc_c = contig(dL_dout_color), gd_c = contig(dL_dout_depth), gm_c = contig(dL_dout_mask),
+               gf_c = contig(dL_dout_flow);
+    TORCH_CHECK(gd_c.numel() == 0 || gd_c.numel() == (int64_t)B * H * W, "fdgs: the depth gradient must be [B,1,H,W]");
+    TORCH_CHECK(gm_c.numel() == 0 || gm_c.numel() == (int64_t)B * H * W, "fdgs: the alpha gradient must be [B,1,H,W]");
+    TORCH_CHECK(gf_c.numel() == 0 || gf_c.numel() == 2ll * B * H * W, "fdgs: the flow gradient must be [B,2,H,W]");
+    const DeviceStream on(means3D);
+    const bool split = sh_rest.defined() && sh_rest.numel() != 0;
+    const int M = ((sh.defined() && sh.numel() != 0) ? (int)sh.size(1) : 0) + (split ? (int)sh_rest.size(1) : 0);
+    auto opts = means3D.options().dtype(torch::kFloat32);
+    torch::Tensor dL_dmeans2D = torch::zeros({B, P, 3}, opts);
+    torch::Tensor dL_dopacity = torch::empty({P, 1}, opts), dL_dmeans3D = torch::empty({P, 3}, opts);
+    torch::Tensor dL_dsh = torch::empty({P, split ? 1 : M, 3}, opts);
+    torch::Tensor dL_dsh_rest = split ? torch::empty({P, M - 1, 3}, opts) : torch::empty({0}, opts);
+    torch::Tensor dL_dts = torch::empty({P, 1}, opts), dL_dscales = torch::empty({P, 3}, opts),
+                  dL_dscales_t = torch::empty({P, 1}, opts), dL_drot = torch::empty({P, 4}, opts),
+                  dL_drot_r = torch::empty({P, 4}, opts);
+    torch::Tensor dL_dbg_image = want_dbg ? torch::empty({B, 3, H, W}, opts) : torch::empty({0}, opts);
+    torch::Tensor scratch = torch::empty({(int64_t)fdgs_backward_batch_scratch_bytes(P, B)}, means3D.options().dtype(torch::kByte));
+    const auto bg_c = contig(background), flow_c = contig(flows), op_c = contig(opacities), ts_c = contig(ts),
+               sc_c = contig(scales), sct_c = contig(scales_t), rot_c = contig(rotations), rotr_c = contig(rotations_r),
+               sh_c = contig(sh), shr_c = contig(sh_rest), geo_c = contig(geomBuffer), bin_c = contig(binningBuffer),
+               img_c = contig(imageBuffer);
+    fdgs_backward_batch_args b;
+    memset(&b, 0, sizeof(b));
+    fdgs_backward_args& a = b.view;
+    a.P = P; a.D = degree; a.D_t = degree_t; a.M = M; a.R = R;
+    a.background = fptr(bg_c); a.width = W; a.height = H;
+    a.out_means3D = om; a.shs = fptr(sh_c); a.flows_2d = fptr(flow_c);
+    a.opacities = fptr(op_c); a.ts = fptr(ts_c); a.scales = fptr(sc_c); a.scales_t = fptr(sct_c);
+    a.scale_modifier = scale_modifier; a.rotations = fptr(rot_c); a.rotations_r = fptr(rotr_c);
+    a.prefilter_var = prefilter_var;
+    a.viewmatrix = cams.view; a.projmatrix = cams.proj; a.campos = cams.campos;
+    a.time_duration = time_duration; a.rot_4d = rot_4d; a.gaussian_dim = gaussian_dim; a.force_sh_3d = force_sh_3d;
+    a.radii = rad;
+    a.geom_buffer = geo_c.numel() ? reinterpret_cast<const char*>(geo_c.data_ptr()) : nullptr;
+    a.binning_buffer = bin_c.numel() ? reinterpret_cast<const char*>(bin_c.data_ptr()) : nullptr;
+    a.image_buffer = img_c.numel() ? reinterpret_cast<const char*>(img_c.data_ptr()) : nullptr;
+    a.dL_dpix = fptr(gc_c); a.dL_depths = fptr(gd_c); a.dL_masks = fptr(gm_c); a.dL_dpix_flow = fptr(gf_c);
+    a.debug = debug; a.raw_params = raw_params;
+    a.dL_dmean2D = dL_dmeans2D.data_ptr<float>(); a.dL_dopacity = dL_dopacity.data_ptr<float>();
+    a.dL_dmean3D = dL_dmeans3D.data_ptr<float>(); a.dL_dsh = dL_dsh.data_ptr<float>();
+    a.shs_rest = split ? fptr(shr_c) : nullptr; a.dL_dsh_rest = split ? dL_dsh_rest.data_ptr<float>() : nullptr;
+    a.dL_dts = dL_dts.data_ptr<float>(); a.dL_dscale = dL_dscales.data_ptr<float>();
+    a.dL_dscale_t = dL_dscales_t.data_ptr<float>(); a.dL_drot = dL_drot.data_ptr<float>(); a.dL_drot_r = dL_drot_r.data_ptr<float>();
+    b.B = B; b.bg_image = bgi; b.bg_views = bgi ? B : 0;
+    b.dL_dbg_image = want_dbg ? dL_dbg_image.data_ptr<float>() : nullptr;
+    b.scratch = reinterpret_cast<char*>(scratch.data_ptr());
+    check(fdgs_backward_batch(&b, (void*)on.stream), "backward_batch");
+    return {dL_dmeans2D, dL_dopacity, dL_dmeans3D, dL_dsh, dL_dsh_rest, dL_dts, dL_dscales, dL_dscales_t, dL_drot, dL_drot_r,
+            dL_dbg_image};
+}
+
+// Test hook: view `view` of a batch's tile ranges [tiles,2] and n_contrib [H,W]
+std::tuple<torch::Tensor, torch::Tensor> DebugExportBinningView(const torch::Tensor& imgBuffer, const int W, const int H,
+                                                                const int B, const int view) {
+    const DeviceStream on(imgBuffer);
+    auto i32 = imgBuffer.options().dtype(torch::kInt32);
+    const int tiles = ((W + 15) / 16) * ((H + 15) / 16);
+    torch::Tensor ranges = torch::zeros({tiles, 2}, i32), n_contrib = torch::zeros({H, W}, i32);
+    check(fdgs_debug_export_binning_view(reinterpret_cast<const char*>(imgBuffer.data_ptr()), W, H, B, view,
+                                         reinterpret_cast<unsigned int*>(ranges.data_ptr<int>()),
+                                         reinterpret_cast<unsigned int*>(n_contrib.data_ptr<int>()), (void*)on.stream),
+          "debug_export_binning_view");
+    return std::make_tuple(ranges, n_contrib);
 }
 
 // ---- environment-map sky (include/fdgs.h: fdgs_sky_forward / fdgs_sky_backward) -----------------------------------
@@ -916,6 +1120,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("rasterize_gaussians_backward", &RasterizeGaussiansBackwardCUDA);
     m.def("rasterize_gaussians_ext", &RasterizeGaussiansExt);
     m.def("rasterize_gaussians_backward_ext", &RasterizeGaussiansBackwardExt);
+    m.def("rasterize_gaussians_batch", &RasterizeGaussiansBatch);
+    m.def("rasterize_gaussians_backward_batch", &RasterizeGaussiansBackwardBatch);
+    m.def("debug_export_binning_view", &DebugExportBinningView);
     m.def("sky_forward", &SkyForward);
     m.def("sky_backward", &SkyBackward);
     m.def("sh_outer_sum", &ShOuterSum);

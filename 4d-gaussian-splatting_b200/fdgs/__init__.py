@@ -4,7 +4,8 @@
 `_C.rasterize_gaussians / rasterize_gaussians_backward / mark_visible`
 (reference: diff-gaussian-rasterization/ext.cpp:15-19), the extended pair
 `rasterize_gaussians_ext / rasterize_gaussians_backward_ext` (raw parameters, per-pixel background,
-view-parallel colour factors) and the training-step bindings; `fdgs.lib()` is the raw C-ABI
+view-parallel colour factors), the batched pair `rasterize_gaussians_batch / rasterize_gaussians_backward_batch` (B views
+of the same Gaussians per call) and the training-step bindings; `fdgs.lib()` is the raw C-ABI
 (`libfdgs.so`, include/fdgs.h) through ctypes.
 
 There is NO fallback: if the CUDA libraries have not been built (run
@@ -31,6 +32,8 @@ ABI_SYMBOLS = (
     "fdgs_densify_scratch_bytes", "fdgs_densify_plan", "fdgs_densify_apply", "fdgs_reset_opacity", "fdgs_densify_stats",
     "fdgs_rigid_scratch_bytes", "fdgs_rigid_neighbours", "fdgs_rigid_forward", "fdgs_rigid_backward",
     "fdgs_metrics_scratch_bytes", "fdgs_image_metrics",
+    "fdgs_geom_batch_bytes", "fdgs_image_batch_bytes", "fdgs_backward_batch_scratch_bytes", "fdgs_forward_batch",
+    "fdgs_backward_batch", "fdgs_debug_export_binning_view",
 )
 
 STAGE_NAMES = ("preprocess_fwd", "bin_count_scan", "bin_scatter", "tile_sort_pack", "reserved", "blend_fwd", "blend_bwd",

@@ -15,11 +15,12 @@ import os
 import torch
 from torch.nn import functional as F
 
-from .diff_gaussian_rasterization import GaussianRasterizationSettings, GaussianRasterizer
+from .diff_gaussian_rasterization import (BatchRasterizationSettings, GaussianRasterizationSettings, GaussianRasterizer,
+                                          rasterize_gaussians_batch)
 from . import pyprep
 from fdgs.sky import sample_sky
 
-__all__ = ["render", "GaussianRasterizationSettings", "GaussianRasterizer"]
+__all__ = ["render", "render_batch", "GaussianRasterizationSettings", "GaussianRasterizer"]
 
 
 def _select(mask, *tensors):
@@ -193,3 +194,86 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
             "depth": depth,
             "alpha": alpha,
             "flow": flow}
+
+
+def render_batch(viewpoint_cameras, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None):
+    """Render B views of the scene in one rasterizer call per direction: one launch per stage and one host
+    synchronisation for the whole batch instead of one per view.
+
+    Returns render()'s seven keys, each stacked along a leading view dimension: "render" [B,3,H,W], "viewspace_points"
+    [B,P,3] (its .grad receives every view's screen-space gradient), "visibility_filter" / "radii" [B,P], "depth" /
+    "alpha" [B,1,H,W], "flow" [B,2,H,W].  View b's images and radii equal render(viewpoint_cameras[b], ...) bit for bit;
+    each Gaussian's parameter gradient is the sum of the views' gradients in view order, as a sequential loop with one
+    backward() per view would accumulate it.
+
+    The views must share the image size; precomputed colours or covariances (override_color, compute_cov3D_python,
+    convert_SHs_python) and a call inside an active ViewParallelStep are not supported (ValueError)."""
+    cams = list(viewpoint_cameras)
+    if not cams:
+        raise ValueError("render_batch needs at least one camera")
+    if override_color is not None:
+        raise ValueError("render_batch does not take override_color (precomputed colours); use render()")
+    if pipe.compute_cov3D_python:
+        raise ValueError("render_batch does not support compute_cov3D_python (precomputed covariances); use render()")
+    if pipe.convert_SHs_python:
+        raise ValueError("render_batch does not support convert_SHs_python (precomputed colours); use render()")
+    from fdgs.dist import ViewParallelStep
+    if ViewParallelStep.current() is not None:
+        raise ValueError("render_batch cannot run inside an active ViewParallelStep; render its views with render()")
+    H, W = int(cams[0].image_height), int(cams[0].image_width)
+    for c in cams[1:]:
+        if (int(c.image_height), int(c.image_width)) != (H, W):
+            raise ValueError("render_batch views must share the image size: %dx%d and %dx%d"
+                             % (W, H, int(c.image_width), int(c.image_height)))
+
+    xyz = pc.get_xyz
+    dev = xyz.device
+    B, P = len(cams), xyz.shape[0]
+    screenspace_points = torch.zeros((B, P, 3), dtype=xyz.dtype, requires_grad=True, device=dev) + 0
+    screenspace_points.retain_grad()
+
+    env_map_res = getattr(pipe, "env_map_res", 0)
+    settings = BatchRasterizationSettings(
+        image_height=H, image_width=W,
+        tanfovx=tuple(math.tan(c.FoVx * 0.5) for c in cams),
+        tanfovy=tuple(math.tan(c.FoVy * 0.5) for c in cams),
+        bg=bg_color if not env_map_res else torch.zeros(3, device=dev),
+        scale_modifier=scaling_modifier,
+        viewmatrix=torch.stack([c.world_view_transform for c in cams]),
+        projmatrix=torch.stack([c.full_proj_transform for c in cams]),
+        sh_degree=pc.active_sh_degree, sh_degree_t=pc.active_sh_degree_t,
+        campos=torch.stack([c.camera_center for c in cams]),
+        timestamp=tuple(float(c.timestamp) for c in cams),
+        time_duration=pc.time_duration[1] - pc.time_duration[0],
+        rot_4d=pc.rot_4d, gaussian_dim=pc.gaussian_dim, force_sh_3d=pc.force_sh_3d,
+        prefiltered=False, debug=pipe.debug)
+
+    sky = None
+    misses = []
+    if env_map_res:
+        assert pc.env_map is not None
+        skies = []
+        for c in cams:
+            s, miss = sample_sky(pc.env_map, c)
+            skies.append(s)
+            misses.append(miss)
+        sky = torch.stack(skies)
+
+    four_d = pc.gaussian_dim == 4
+    if _fused_prologue_ok(pc, pipe, None):
+        color, radii, depth, alpha, flow = rasterize_gaussians_batch(
+            xyz, screenspace_points, pc._opacity, pc._features_dc, pc._scaling, pc._rotation, settings,
+            sh_rest=pc._features_rest if pc._features_rest.numel() else None, flow_2d=torch.zeros_like(xyz[:, :2]),
+            ts=pc._t if four_d else None, scales_t=pc._scaling_t if four_d else None,
+            rotations_r=pc._rotation_r if pc.rot_4d else None,
+            prefilter_var=pc.prefilter_var if (four_d and pc.prefilter_var > 0.0) else -1.0, raw=True, bg_image=sky)
+    else:
+        color, radii, depth, alpha, flow = rasterize_gaussians_batch(
+            xyz, screenspace_points, pc.get_opacity, pc.get_features, pc.get_scaling, pc.get_rotation, settings,
+            flow_2d=torch.zeros_like(xyz[:, :2]), ts=pc.get_t if four_d else None,
+            scales_t=pc.get_scaling_t if four_d else None, rotations_r=pc.get_rotation_r if pc.rot_4d else None,
+            prefilter_var=pc.prefilter_var if (four_d and pc.prefilter_var > 0.0) else -1.0, bg_image=sky)
+    for miss in misses:
+        miss.check()
+    return {"render": color, "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii,
+            "depth": depth, "alpha": alpha, "flow": flow}

@@ -251,3 +251,113 @@ class GaussianRasterizer(nn.Module):
         return rasterize_gaussians(means3D, means2D, opt(shs), opt(colors_precomp), opt(flow_2d), opacities,
                                    opt(ts), opt(scales), opt(scales_t), opt(rotations), opt(rotations_r),
                                    opt(cov3D_precomp), prefilter_var, self.raster_settings, bg_image)
+
+
+class BatchRasterizationSettings(NamedTuple):
+    """What B views of one batch share, plus their per-view cameras: viewmatrix / projmatrix [B,4,4] and campos [B,3]
+    CUDA tensors, tanfovx / tanfovy / timestamp sequences of B floats."""
+    image_height: int
+    image_width: int
+    tanfovx: tuple
+    tanfovy: tuple
+    bg: torch.Tensor
+    scale_modifier: float
+    viewmatrix: torch.Tensor
+    projmatrix: torch.Tensor
+    sh_degree: int
+    sh_degree_t: int
+    campos: torch.Tensor
+    timestamp: tuple
+    time_duration: float
+    rot_4d: bool
+    gaussian_dim: int
+    force_sh_3d: bool
+    prefiltered: bool
+    debug: bool
+
+
+class _RasterizeGaussiansBatch(torch.autograd.Function):
+    """B views of the same Gaussians in one forward and one backward (include/fdgs.h: fdgs_forward_batch).  Inputs, in
+    order: means3D, means2D [B,P,3], sh, sh_rest, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
+    prefilter_var, settings (BatchRasterizationSettings), raw, bg_image ([B,3,H,W] or None).  raw and sh / sh_rest as in
+    _RasterizeGaussians.  Returns color [B,3,H,W], radii [B,P], depth [B,1,H,W], alpha [B,1,H,W], flow [B,2,H,W].
+    Every per-Gaussian gradient is the sum of the views' gradients in view order; means2D's gradient stays per view."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, sh, sh_rest, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
+                prefilter_var, settings, raw, bg_image):
+        s = settings
+        cams = (s.viewmatrix, s.projmatrix, s.campos) + tuple(
+            torch.tensor(list(v), dtype=torch.float32) for v in (s.timestamp, s.tanfovx, s.tanfovy))
+        args = (s.bg, means3D, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r, s.scale_modifier,
+                prefilter_var) + cams + (s.image_height, s.image_width, sh, sh_rest, s.sh_degree, s.sh_degree_t,
+                                         s.time_duration, s.rot_4d, s.gaussian_dim, s.force_sh_3d, s.prefiltered, s.debug,
+                                         raw, _NONE if bg_image is None else bg_image)
+        (num_rendered, color, flow, depth, T, radii, geom_buf, binning_buf, img_buf,
+         out_means3D) = _invoke(_C.rasterize_gaussians_batch, args, s.debug, "snapshot_fw.dump")
+        ctx.cams = cams
+        ctx.settings = s
+        ctx.raw = raw
+        ctx.bg_image = bg_image
+        ctx.num_rendered = num_rendered
+        ctx.prefilter_var = prefilter_var
+        ctx.save_for_backward(means3D, out_means3D, radii, sh, sh_rest, flow_2d, opacities, ts, scales, scales_t,
+                              rotations, rotations_r, geom_buf, binning_buf, img_buf)
+        ctx.mark_non_differentiable(radii)
+        ctx.set_materialize_grads(False)
+        ctx.image_shape = tuple(color.shape)
+        return color, radii, depth, 1 - T, flow
+
+    @staticmethod
+    def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha, grad_flow):
+        s = ctx.settings
+        (means3D, out_means3D, radii, sh, sh_rest, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
+         geom_buf, binning_buf, img_buf) = ctx.saved_tensors
+        if grad_color is None:
+            grad_color = torch.zeros(ctx.image_shape, dtype=torch.float32, device=means3D.device)
+        none = torch.empty(0, dtype=torch.float32, device=means3D.device)   # "no gradient": the colour-only blend backward
+        grad_depth = none if grad_depth is None else grad_depth
+        grad_alpha = none if grad_alpha is None else grad_alpha
+        grad_flow = none if grad_flow is None else grad_flow
+        want_bg = ctx.needs_input_grad[14]
+        args = (s.bg, means3D, out_means3D, radii, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
+                s.scale_modifier, ctx.prefilter_var) + ctx.cams + (
+            grad_color, grad_depth, grad_alpha, grad_flow, sh, sh_rest, s.sh_degree, s.sh_degree_t, s.time_duration,
+            s.rot_4d, s.gaussian_dim, s.force_sh_3d, geom_buf, ctx.num_rendered, binning_buf, img_buf, s.debug, ctx.raw,
+            _NONE if ctx.bg_image is None else ctx.bg_image, bool(want_bg))
+        (g_means2D, g_opacities, g_means3D, g_sh, g_sh_rest, g_ts, g_scales, g_scales_t, g_rot, g_rot_r,
+         g_bg) = _invoke(_C.rasterize_gaussians_backward_batch, args, s.debug, "snapshot_bw.dump")
+
+        def for_input(grad, inp):
+            return grad if inp.numel() > 0 else None
+
+        return (g_means3D, g_means2D, g_sh, for_input(g_sh_rest, sh_rest), None, g_opacities, for_input(g_ts, ts),
+                g_scales, for_input(g_scales_t, scales_t), g_rot, for_input(g_rot_r, rotations_r), None, None, None,
+                g_bg if want_bg else None)
+
+
+def rasterize_gaussians_batch(means3D, means2D, opacities, sh, scales, rotations, settings, sh_rest=None, flow_2d=None,
+                              ts=None, scales_t=None, rotations_r=None, prefilter_var=-1.0, raw=False, bg_image=None):
+    """Rasterize B views of the same Gaussians in one call (see _RasterizeGaussiansBatch).  raw: the inputs are the
+    optimiser's raw parameters (forward_raw's convention: sh = features_dc, sh_rest = features_rest).  bg_image: per-view
+    background images [B,3,H,W] behind the Gaussians, or None."""
+    B = int(settings.viewmatrix.shape[0])
+    P = int(means3D.shape[0])
+    if tuple(means2D.shape) != (B, P, 3):
+        raise ValueError("means2D must have shape (B, P, 3) = %s, got %s" % ((B, P, 3), tuple(means2D.shape)))
+    for name in ("tanfovx", "tanfovy", "timestamp"):
+        if len(getattr(settings, name)) != B:
+            raise ValueError("settings.%s must hold one value per view (%d), got %d" % (name, B, len(getattr(settings, name))))
+    if bg_image is not None:
+        shape = (B, 3, int(settings.image_height), int(settings.image_width))
+        if not isinstance(bg_image, torch.Tensor) or tuple(bg_image.shape) != shape:
+            raise ValueError("bg_image must be a tensor of shape %s (B, 3, image_height, image_width)" % (shape,))
+    if settings.rot_4d and (rotations_r is None or scales_t is None or ts is None):
+        raise Exception('Please provide exactly rotations_r and scales_t and ts if rot_4d and cov3D_precomp is None!')
+
+    def opt(t):
+        return _NONE if t is None else t
+
+    return _RasterizeGaussiansBatch.apply(means3D, means2D, sh, opt(sh_rest), opt(flow_2d), opacities, opt(ts), scales,
+                                          opt(scales_t), rotations, opt(rotations_r), prefilter_var, settings, raw,
+                                          bg_image)

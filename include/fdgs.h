@@ -225,6 +225,54 @@ int fdgs_forward_bg(const fdgs_forward_args* args, const float* bg_image,
                     fdgs_forward_result* result);
 int fdgs_backward_bg(const fdgs_backward_args* args, const float* bg_image, float* dL_dbg_image, void* stream);
 
+/* Batched views: B >= 1 cameras of the same Gaussians in one call per direction, one launch per stage and ONE host
+ * synchronisation for the whole batch.  Every view's outputs are bit-identical to fdgs_forward_bg on that camera.
+ * `view` holds what the views share, as in fdgs_forward_args, except:
+ *   viewmatrix / projmatrix / cam_pos   [B,16] / [B,16] / [B,3] device tables, one row per view
+ *   timestamp / tan_fovx / tan_fovy     ignored: the per-view host arrays below
+ *   out_means3D [B,P,3], radii [B,P], out_color [B,3,H,W], out_flow [B,2,H,W], out_depth / out_T [B,1,H,W]
+ *   colors_precomp / cov3D_precomp      must be NULL (SH and scales / rotations only)
+ * bg_image: [B,3,H,W] per-view background images (fdgs_forward_bg), or NULL; bg_views must then equal B. */
+typedef struct fdgs_forward_batch_args {
+    fdgs_forward_args view;
+    int B;
+    const float* timestamps;   /* host [B] */
+    const float* tan_fovx;     /* host [B] */
+    const float* tan_fovy;     /* host [B] */
+    const float* bg_image;     /* [B,3,H,W] device, or NULL */
+    int bg_views;              /* leading dimension of bg_image */
+} fdgs_forward_batch_args;
+
+/* Backward of fdgs_forward_batch, fully asynchronous.  `view` as in fdgs_backward_args, except:
+ *   viewmatrix / projmatrix / campos, out_means3D, radii: the forward's per-view tables and outputs
+ *   timestamp / tan_fovx / tan_fovy   ignored (the forward keeps the per-view values in geom_buffer)
+ *   dL_dpix [B,3,H,W], dL_depths / dL_masks [B,1,H,W], dL_dpix_flow [B,2,H,W] (each optional but dL_dpix)
+ *   dL_dmean2D [B,P,3]                per view, accumulated (ZERO on entry)
+ *   dL_dopacity, dL_dmean3D, dL_dts, dL_dscale, dL_dscale_t, dL_drot, dL_drot_r: [P,...] sums over the views in
+ *                                     view order, ((g_0 + g_1) + g_2) + ... in fp32, overwritten
+ *   dL_dsh (+ dL_dsh_rest)            the SH rows summed over the views, overwritten
+ *   dL_dconic, dL_dcolor, dL_dflows, dL_dcov3D, sh_factors: ignored (per-view scratch lives in `scratch`)
+ * scratch: fdgs_backward_batch_scratch_bytes(P, B) bytes of device memory.  dL_dbg_image: [B,3,H,W] or NULL. */
+typedef struct fdgs_backward_batch_args {
+    fdgs_backward_args view;
+    int B;
+    const float* bg_image;     /* the forward's bg_image, or NULL */
+    int bg_views;
+    float* dL_dbg_image;       /* [B,3,H,W] overwritten, or NULL */
+    char* scratch;
+} fdgs_backward_batch_args;
+
+size_t fdgs_geom_batch_bytes(int P, int B);
+size_t fdgs_image_batch_bytes(int width, int height, int B);
+size_t fdgs_backward_batch_scratch_bytes(int P, int B);
+int fdgs_forward_batch(const fdgs_forward_batch_args* args,
+                       fdgs_alloc_fn geom_alloc, void* geom_ctx,
+                       fdgs_alloc_fn binning_alloc, void* binning_ctx,
+                       fdgs_alloc_fn image_alloc, void* image_ctx,
+                       void* stream,
+                       fdgs_forward_result* result);
+int fdgs_backward_batch(const fdgs_backward_batch_args* args, void* stream);
+
 /* Environment-map sky sphere (the reference's sky for scenes with an environment map: gaussian_renderer/__init__.py
  * and Camera.get_rays).  Each pixel's ray -- the pixel centre ((x + 0.5 - cx) / fl_x, (y + 0.5 - cy) / fl_y, 1, 1)
  * through c2w, minus campos, normalised -- is intersected with the sphere |X| = radius; the hit point gives
@@ -498,6 +546,10 @@ int fdgs_debug_export_binning(const char* binning_buffer, const char* image_buff
                               unsigned int* ranges /*[tiles,2]*/,
                               unsigned int* n_contrib /*[H*W]*/,
                               void* stream);
+/* One view of a batch (fdgs_forward_batch): its tile ranges [tiles,2] (offsets into the batch's point_list, which
+ * fdgs_debug_export_binning copies) and its n_contrib [H*W]. */
+int fdgs_debug_export_binning_view(const char* image_buffer, int width, int height, int B, int view,
+                                   unsigned int* ranges, unsigned int* n_contrib, void* stream);
 
 /* Test hook of the raw-parameter entry: applies the in-kernel activations to plain arrays of n elements (log_s, logit:
  * [n]; quat: [n,4]; mode = quaternion-norm summation order, 0 = the library's default). */
