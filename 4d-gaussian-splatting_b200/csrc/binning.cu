@@ -503,11 +503,11 @@ static cudaError_t launch_bin_pass(int P, int views, const uint4* binrec, int gr
     return cudaGetLastError();
 }
 
-cudaError_t launch_bin_count(int P, const uint4* binrec, int grid_x, int grid_y, uint32_t* matrix, cudaStream_t stream,
-                             int views, bool batch) {
+cudaError_t launch_bin_count(int P, const uint4* binrec, int grid_x, int grid_y, uint32_t* matrix, const ViewBatch& vb,
+                             cudaStream_t stream) {
     if (P <= 0)
-        return cudaMemsetAsync(matrix, 0, (size_t)bin_cta_count() * views * grid_x * grid_y * sizeof(uint32_t), stream);
-    if (batch) return launch_bin_pass<false, true>(P, views, binrec, grid_x, grid_y, matrix, nullptr, nullptr, stream);
+        return cudaMemsetAsync(matrix, 0, (size_t)bin_cta_count() * vb.B * grid_x * grid_y * sizeof(uint32_t), stream);
+    if (vb.scalars) return launch_bin_pass<false, true>(P, vb.B, binrec, grid_x, grid_y, matrix, nullptr, nullptr, stream);
     return launch_bin_pass<false, false>(P, 1, binrec, grid_x, grid_y, matrix, nullptr, nullptr, stream);
 }
 
@@ -519,8 +519,8 @@ cudaError_t launch_tile_scan(int num_tiles, uint32_t* matrix, uint32_t* tile_tot
 }
 
 cudaError_t launch_bin_scatter(int P, const uint4* binrec, int grid_x, int grid_y, uint32_t* matrix,
-                               const uint32_t* tile_offset, uint64_t* keys, cudaStream_t stream, int views, bool batch) {
-    if (batch) return launch_bin_pass<true, true>(P, views, binrec, grid_x, grid_y, matrix, tile_offset, keys, stream);
+                               const uint32_t* tile_offset, uint64_t* keys, const ViewBatch& vb, cudaStream_t stream) {
+    if (vb.scalars) return launch_bin_pass<true, true>(P, vb.B, binrec, grid_x, grid_y, matrix, tile_offset, keys, stream);
     return launch_bin_pass<true, false>(P, 1, binrec, grid_x, grid_y, matrix, tile_offset, keys, stream);
 }
 
@@ -544,11 +544,11 @@ static cudaError_t tile_sort_pack(int num_tiles, int max_count, const uint2* ran
 }
 
 cudaError_t launch_tile_sort_pack(int num_tiles, int max_count, int R, const uint2* ranges, uint64_t* keys,
-                                  const InstRec* grec, StageRec* recs, uint32_t* point_list, cudaStream_t stream,
-                                  int tiles_per_view, int P) {
+                                  const InstRec* grec, int P, StageRec* recs, uint32_t* point_list, const ViewBatch& vb,
+                                  cudaStream_t stream) {
     if (num_tiles <= 0 || R <= 0) return cudaSuccess;
-    if (tiles_per_view > 0)
-        return tile_sort_pack<true>(num_tiles, max_count, ranges, keys, grec, recs, point_list, tiles_per_view, P, stream);
+    if (vb.scalars)
+        return tile_sort_pack<true>(num_tiles, max_count, ranges, keys, grec, recs, point_list, num_tiles / vb.B, P, stream);
     return tile_sort_pack<false>(num_tiles, max_count, ranges, keys, grec, recs, point_list, 0, 0, stream);
 }
 

@@ -113,22 +113,29 @@ struct Carver {
     size_t total() const { return off + 128; }
 };
 
+// batch: the batched entry's layout, [B][P] stacks of every array, then the [B] per-view scalars
 struct GeomState {
     float* cov3D;            // [P,6]  (first: exposed as covs3D_com)
     fdgs::InstRec* grec;     // [P]    per-Gaussian 64-byte record
     uint8_t* clamped;        // [P]
     uint32_t* tiles_touched; // [P]
     uint4* binrec;           // [P] tile rectangle + depth bits of every Gaussian, for the binning passes
+    fdgs::ViewScalars* scalars;   // [B] (batch only, else NULL)
     size_t bytes;
-    static GeomState carve(char* base, long long P) {
+    static GeomState carve(char* base, int P, bool batch = false, int B = 0) {
         GeomState g;
         Carver c(base);
-        const size_t p = (size_t)(P > 0 ? P : 0);
+        const size_t p = (size_t)(P > 0 ? P : 0) * (batch ? (size_t)(B > 0 ? B : 0) : 1);
         g.cov3D = c.take<float>(6 * p);   // first: 128-byte aligned [P,6] view for covs3D_com
         g.grec = c.take<fdgs::InstRec>(p);
         g.clamped = c.take<uint8_t>(p);
         g.tiles_touched = c.take<uint32_t>(p);
         g.binrec = c.take<uint4>(p);
+        g.scalars = nullptr;
+        if (batch) {
+            c.off += 128;   // the view table starts one 128-byte block past the stacks (fdgs_geom_batch_bytes' layout)
+            g.scalars = c.take<fdgs::ViewScalars>((size_t)(B > 0 ? B : 0));
+        }
         g.bytes = c.total();
         return g;
     }
@@ -176,21 +183,6 @@ struct BinningState {
         b.keys = c.take<uint64_t>(r);
         b.bytes = c.total();
         return b;
-    }
-};
-
-// The batched entry's geometry buffer: the [B][P] stacks of GeomState, then the per-view scalars
-struct BatchGeomState {
-    GeomState g;
-    fdgs::ViewScalars* scalars;   // [B]
-    size_t bytes;
-    static BatchGeomState carve(char* base, int P, int B) {
-        BatchGeomState s;
-        s.g = GeomState::carve(base, (long long)(P > 0 ? P : 0) * (B > 0 ? B : 0));
-        const size_t off = (s.g.bytes + 127) & ~(size_t)127;
-        s.scalars = base ? reinterpret_cast<fdgs::ViewScalars*>(base + off) : nullptr;
-        s.bytes = off + (size_t)(B > 0 ? B : 0) * sizeof(fdgs::ViewScalars) + 128;
-        return s;
     }
 };
 
@@ -264,7 +256,7 @@ const char* fdgs_last_error(void) { return g_last_error.c_str(); }
 size_t fdgs_geom_bytes(int P) { return GeomState::carve(nullptr, P).bytes + 128; }
 size_t fdgs_image_bytes(int width, int height) { return ImageState::carve(nullptr, width, height).bytes + 128; }
 size_t fdgs_binning_bytes(int num_rendered, int, int) { return BinningState::carve(nullptr, num_rendered).bytes + 128; }
-size_t fdgs_geom_batch_bytes(int P, int B) { return BatchGeomState::carve(nullptr, P, B).bytes + 128; }
+size_t fdgs_geom_batch_bytes(int P, int B) { return GeomState::carve(nullptr, P, true, B).bytes + 128; }
 size_t fdgs_image_batch_bytes(int width, int height, int B) {
     return ImageState::carve(nullptr, width, height, B > 0 ? B : 0).bytes + 128;
 }
@@ -281,8 +273,8 @@ int check_forward_args(const fdgs_forward_args* a) {
     if (!a->out_color || !a->out_flow || !a->out_depth || !a->out_T || !a->background)
         return fail(FDGS_ERR_INVALID_ARG, "background and the output images must be set");
     if (P > 0) {
-        if (!a->means3D || !a->opacities || !a->viewmatrix || !a->projmatrix || !a->cam_pos || !a->background)
-            return fail(FDGS_ERR_INVALID_ARG, "means3D/opacities/viewmatrix/projmatrix/cam_pos/background must be set");
+        if (!a->means3D || !a->opacities || !a->viewmatrix || !a->projmatrix || !a->cam_pos)
+            return fail(FDGS_ERR_INVALID_ARG, "means3D/opacities/viewmatrix/projmatrix/cam_pos must be set");
         if (!a->out_means3D || !a->out_color || !a->out_flow || !a->out_depth || !a->out_T || !a->radii)
             return fail(FDGS_ERR_INVALID_ARG, "output pointers must be set");
         if (!a->cov3D_precomp) {
@@ -312,35 +304,15 @@ int check_forward_args(const fdgs_forward_args* a) {
     return FDGS_OK;
 }
 
-int forward_impl(const fdgs_forward_args* a, const float* bg_image, fdgs_alloc_fn geom_alloc, void* geom_ctx,
-                 fdgs_alloc_fn binning_alloc, void* binning_ctx, fdgs_alloc_fn image_alloc, void* image_ctx, void* stream_v,
-                 fdgs_forward_result* res) {
-    g_last_error.clear();
-    if (!a || !res || !geom_alloc || !binning_alloc || !image_alloc) return fail(FDGS_ERR_INVALID_ARG, "null argument");
-    memset(res, 0, sizeof(*res));
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
-    const bool debug = a->debug != 0;
+// The forward's stages on the carved geometry and image buffers, for one view (vb = {1, NULL}) or for the batched
+// entry's B views (vb = {B, the uploaded view table}: every per-view array is then a [B] stack, and the camera tables and
+// scalars are the views').  Allocates the binning buffer after the one host synchronisation.
+int forward_stages(const fdgs_forward_args* a, const float* bg_image, const fdgs::ViewBatch& vb, const GeomState& geom,
+                   const ImageState& img, fdgs_alloc_fn binning_alloc, void* binning_ctx, cudaStream_t stream,
+                   fdgs_forward_result* res) {
+    const bool debug = a->debug != 0, batch = vb.scalars != nullptr;
     const int P = a->P, W = a->width, H = a->height;
-    if (int rc = check_forward_args(a)) return rc;
     const int grid_x = (W + fdgs::TILE_X - 1) / fdgs::TILE_X, grid_y = (H + fdgs::TILE_Y - 1) / fdgs::TILE_Y;
-    const size_t N = (size_t)W * H;
-
-    // scratch: geometry + image
-    const size_t geom_bytes = fdgs_geom_bytes(P);
-    char* geom_raw = geom_alloc(geom_ctx, geom_bytes);
-    if (!geom_raw) return fail(FDGS_ERR_ALLOC, "geometry buffer allocation failed");
-    GeomState geom = GeomState::carve(align128(geom_raw), P);
-    const size_t img_bytes = fdgs_image_bytes(W, H);
-    char* img_raw = image_alloc(image_ctx, img_bytes);
-    if (!img_raw) return fail(FDGS_ERR_ALLOC, "image buffer allocation failed");
-    ImageState img = ImageState::carve(align128(img_raw), W, H);
-    res->geom_buffer = geom_raw;
-    res->geom_bytes = geom_bytes;
-    res->image_buffer = img_raw;
-    res->image_bytes = img_bytes;
-    res->cov3D = geom.cov3D;
-
-    int num_rendered = 0;
     if (P > 0) {
         fdgs::PreprocessFwdParams pp;
         memset(&pp, 0, sizeof(pp));
@@ -364,22 +336,24 @@ int forward_impl(const fdgs_forward_args* a, const float* bg_image, fdgs_alloc_f
         pp.out_means3D = a->out_means3D; pp.radii = a->radii; pp.cov3D = geom.cov3D; pp.grec = geom.grec;
         pp.clamped = geom.clamped; pp.tiles_touched = geom.tiles_touched; pp.binrec = geom.binrec;
         pp.tile_cull = g_tile_cull.load();
-        FDGS_STAGE(0, 1, fdgs::launch_preprocess_fwd(pp, stream), "preprocess_fwd");
+        pp.vb = vb;
+        FDGS_STAGE(0, 1, fdgs::launch_preprocess_fwd(pp, stream), batch ? "preprocess_fwd (batch)" : "preprocess_fwd");
     }
     // binning: per-tile counts, offsets, ranges and the total instance count R
     FDGS_STAGE(1, (P > 0 ? 1 : 0) + 2,
                [&]() {
-                   cudaError_t e = fdgs::launch_bin_count(P, geom.binrec, grid_x, grid_y, img.bin_matrix, stream);
+                   cudaError_t e = fdgs::launch_bin_count(P, geom.binrec, grid_x, grid_y, img.bin_matrix, vb, stream);
                    if (e != cudaSuccess) return e;
                    return fdgs::launch_tile_scan((int)img.tiles, img.bin_matrix, img.tile_total, img.tile_offset, img.ranges,
                                                  img.bin_info, stream);
                }(),
-               "bin_count + tile_scan");
-    // the one host synchronisation of the forward (reference: rasterizer_impl.cu:302)
+               batch ? "bin_count + tile_scan (batch)" : "bin_count + tile_scan");
+    // the one host synchronisation of the forward (reference: rasterizer_impl.cu:302): R over all views, the largest
+    // tile of any view, the overflow flag
     int bin_info[4] = {0, 0, 0, 0};
     FDGS_CUDA(cudaMemcpyAsync(bin_info, img.bin_info, sizeof(bin_info), cudaMemcpyDeviceToHost, stream), "num_rendered copy");
     FDGS_CUDA(cudaStreamSynchronize(stream), "num_rendered sync");
-    num_rendered = bin_info[0];
+    const int num_rendered = bin_info[0];
     // bin_info[2]: the 64-bit total computed on the device exceeded 2^31 - 1 (a wrapped 32-bit total would look valid)
     if (num_rendered < 0 || bin_info[2] != 0) return fail(FDGS_ERR_UNSUPPORTED, "more than 2^31 - 1 tile instances");
     res->num_rendered = num_rendered;
@@ -392,12 +366,14 @@ int forward_impl(const fdgs_forward_args* a, const float* bg_image, fdgs_alloc_f
     res->binning_bytes = bin_bytes;
 
     if (num_rendered > 0) {
-        FDGS_STAGE(2, 1, fdgs::launch_bin_scatter(P, geom.binrec, grid_x, grid_y, img.bin_matrix, img.tile_offset, bin.keys, stream),
-                   "bin_scatter");
+        FDGS_STAGE(2, 1,
+                   fdgs::launch_bin_scatter(P, geom.binrec, grid_x, grid_y, img.bin_matrix, img.tile_offset, bin.keys, vb,
+                                            stream),
+                   batch ? "bin_scatter (batch)" : "bin_scatter");
         FDGS_STAGE(3, fdgs::tile_sort_pack_kernel_count(bin_info[1]),
-                   fdgs::launch_tile_sort_pack((int)img.tiles, bin_info[1], num_rendered, img.ranges, bin.keys, geom.grec, bin.recs,
-                                               bin.point_list, stream),
-                   "tile_sort_pack");
+                   fdgs::launch_tile_sort_pack((int)img.tiles, bin_info[1], num_rendered, img.ranges, bin.keys, geom.grec, P,
+                                               bin.recs, bin.point_list, vb, stream),
+                   batch ? "tile_sort_pack (batch)" : "tile_sort_pack");
     }
     fdgs::BlendFwdParams bp;
     bp.W = W; bp.H = H; bp.grid_x = grid_x; bp.grid_y = grid_y;
@@ -405,64 +381,65 @@ int forward_impl(const fdgs_forward_args* a, const float* bg_image, fdgs_alloc_f
     bp.final_T = img.final_T; bp.n_contrib = img.n_contrib;
     bp.out_color = a->out_color; bp.out_flow = a->out_flow; bp.out_depth = a->out_depth; bp.out_T = a->out_T;
     bp.bg_image = bg_image;
-    bp.views = 0;
-    (void)N;
-    FDGS_STAGE(5, 1, fdgs::launch_blend_fwd(bp, stream), "blend_fwd");
+    bp.views = batch ? vb.B : 0;
+    FDGS_STAGE(5, 1, fdgs::launch_blend_fwd(bp, stream), batch ? "blend_fwd (batch)" : "blend_fwd");
     return FDGS_OK;
 }
 
-int backward_impl(const fdgs_backward_args* a, const float* bg_image, float* dL_dbg_image, void* stream_v) {
+int forward_impl(const fdgs_forward_args* a, const float* bg_image, fdgs_alloc_fn geom_alloc, void* geom_ctx,
+                 fdgs_alloc_fn binning_alloc, void* binning_ctx, fdgs_alloc_fn image_alloc, void* image_ctx, void* stream_v,
+                 fdgs_forward_result* res) {
     g_last_error.clear();
-    if (!a) return fail(FDGS_ERR_INVALID_ARG, "null argument");
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
-    const bool debug = a->debug != 0;
+    if (!a || !res || !geom_alloc || !binning_alloc || !image_alloc) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    memset(res, 0, sizeof(*res));
+    const int P = a->P, W = a->width, H = a->height;
+    if (int rc = check_forward_args(a)) return rc;
+
+    // scratch: geometry + image
+    const size_t geom_bytes = fdgs_geom_bytes(P);
+    char* geom_raw = geom_alloc(geom_ctx, geom_bytes);
+    if (!geom_raw) return fail(FDGS_ERR_ALLOC, "geometry buffer allocation failed");
+    GeomState geom = GeomState::carve(align128(geom_raw), P);
+    const size_t img_bytes = fdgs_image_bytes(W, H);
+    char* img_raw = image_alloc(image_ctx, img_bytes);
+    if (!img_raw) return fail(FDGS_ERR_ALLOC, "image buffer allocation failed");
+    ImageState img = ImageState::carve(align128(img_raw), W, H);
+    res->geom_buffer = geom_raw;
+    res->geom_bytes = geom_bytes;
+    res->image_buffer = img_raw;
+    res->image_bytes = img_bytes;
+    res->cov3D = geom.cov3D;
+    return forward_stages(a, bg_image, {1, nullptr}, geom, img, binning_alloc, binning_ctx,
+                          reinterpret_cast<cudaStream_t>(stream_v), res);
+}
+
+// The backward's stages on the forward's buffers: the blend backward (when there is an instance or dL_dbg_image to
+// write), then the per-Gaussian backward (when there is a Gaussian).  vb as in forward_stages; for a batch, a's
+// gradient outputs are the per-view stacks of BatchBwdScratch.  The arguments have been checked by the entry.
+int backward_stages(const fdgs_backward_args* a, const float* bg_image, float* dL_dbg_image, const fdgs::ViewBatch& vb,
+                    const GeomState& geom, const ImageState& img, cudaStream_t stream) {
+    const bool debug = a->debug != 0, batch = vb.scalars != nullptr;
     const int P = a->P, W = a->width, H = a->height, R = a->R;
-    if (P <= 0 && !dL_dbg_image) return FDGS_OK;
-    if (W <= 0 || H <= 0 || R < 0) return fail(FDGS_ERR_INVALID_ARG, "bad width / height / R");
-    if (P <= 0) {
-        // nothing was rendered: the background image takes the whole colour gradient (the blend kernel walks empty
-        // tile lists and writes dL_dbg_image only)
-        if (!a->image_buffer || !a->dL_dpix || !a->background)
-            return fail(FDGS_ERR_INVALID_ARG, "image buffer / colour image gradient / background required");
-        ImageState img = ImageState::carve(align128(const_cast<char*>(a->image_buffer)), W, H);
-        fdgs::BlendBwdParams bp;
-        memset(&bp, 0, sizeof(bp));
-        bp.W = W; bp.H = H; bp.grid_x = (W + fdgs::TILE_X - 1) / fdgs::TILE_X; bp.grid_y = (H + fdgs::TILE_Y - 1) / fdgs::TILE_Y;
-        bp.ranges = img.ranges; bp.background = a->background; bp.final_T = img.final_T; bp.n_contrib = img.n_contrib;
-        bp.dL_dpix = a->dL_dpix; bp.bg_image = bg_image; bp.dL_dbg_image = dL_dbg_image;
-        FDGS_STAGE(6, 1, fdgs::launch_blend_bwd(bp, stream), "blend_bwd");
-        return FDGS_OK;
-    }
-    if (!a->geom_buffer || !a->image_buffer || (R > 0 && !a->binning_buffer))
-        return fail(FDGS_ERR_INVALID_ARG, "scratch buffers of the forward pass required");
-    // dL_depths / dL_masks / dL_dpix_flow may be NULL: no upstream gradient for that image
-    if (!a->dL_dpix) return fail(FDGS_ERR_INVALID_ARG, "colour image gradient required");
-    if (!a->background || !a->radii || !a->out_means3D || !a->viewmatrix || !a->projmatrix || !a->campos)
-        return fail(FDGS_ERR_INVALID_ARG, "background / radii / out_means3D / viewmatrix / projmatrix / campos required");
-    if (a->sh_factors && a->dL_dsh) return fail(FDGS_ERR_INVALID_ARG, "sh_factors and dL_dsh are mutually exclusive");
-    if (!a->dL_dmean2D || !a->dL_dconic || !a->dL_dopacity || !a->dL_dcolor || !a->dL_dflows || !a->dL_dmean3D ||
-        !a->dL_dcov3D || !a->dL_dts || !a->dL_dscale || !a->dL_dscale_t || !a->dL_drot || !a->dL_drot_r)
-        return fail(FDGS_ERR_INVALID_ARG, "gradient outputs required");
-    const int grid_x = (W + fdgs::TILE_X - 1) / fdgs::TILE_X, grid_y = (H + fdgs::TILE_Y - 1) / fdgs::TILE_Y;
-    GeomState geom = GeomState::carve(align128(const_cast<char*>(a->geom_buffer)), P);
-    ImageState img = ImageState::carve(align128(const_cast<char*>(a->image_buffer)), W, H);
     BinningState bin = BinningState::carve(a->binning_buffer ? align128(const_cast<char*>(a->binning_buffer)) : nullptr, R);
 
+    // with no instance at all the blend only has dL_dbg_image to write (P == 0: the background image takes the whole
+    // colour gradient, from empty tile lists)
+    const bool instances = P > 0 && R > 0;
     bool blend_raw = false;
-    // with no instance at all the blend only has dL_dbg_image to write
-    if (R > 0 || dL_dbg_image) {
+    if (instances || dL_dbg_image) {
         fdgs::BlendBwdParams bp;
-        bp.W = W; bp.H = H; bp.grid_x = grid_x; bp.grid_y = grid_y;
+        bp.W = W; bp.H = H; bp.grid_x = (W + fdgs::TILE_X - 1) / fdgs::TILE_X; bp.grid_y = (H + fdgs::TILE_Y - 1) / fdgs::TILE_Y;
         bp.ranges = img.ranges; bp.recs = bin.recs; bp.background = a->background;
         bp.final_T = img.final_T; bp.n_contrib = img.n_contrib;
         bp.dL_dpix = a->dL_dpix; bp.dL_depths = a->dL_depths; bp.dL_masks = a->dL_masks; bp.dL_dpix_flow = a->dL_dpix_flow;
         bp.dL_dmean2D = a->dL_dmean2D; bp.dL_dconic = a->dL_dconic; bp.dL_dopacity = a->dL_dopacity;
         bp.dL_dcolor = a->dL_dcolor; bp.dL_dflows = a->dL_dflows;
         bp.bg_image = bg_image; bp.dL_dbg_image = dL_dbg_image;
-        bp.views = 0; bp.P = P;
-        blend_raw = R > 0 && fdgs::blend_bwd_is_raw(bp);
-        FDGS_STAGE(6, 1, fdgs::launch_blend_bwd(bp, stream), "blend_bwd");
+        bp.views = batch ? vb.B : 0; bp.P = P;
+        blend_raw = instances && fdgs::blend_bwd_is_raw(bp);
+        FDGS_STAGE(6, 1, fdgs::launch_blend_bwd(bp, stream), batch ? "blend_bwd (batch)" : "blend_bwd");
     }
+    if (P <= 0) return FDGS_OK;
     fdgs::PreprocessBwdParams pb;
     memset(&pb, 0, sizeof(pb));
     pb.P = P; pb.D = a->D; pb.D_t = a->D_t; pb.M = a->M;
@@ -483,16 +460,45 @@ int backward_impl(const fdgs_backward_args* a, const float* bg_image, float* dL_
     if (a->dL_dsh && (reinterpret_cast<uintptr_t>(a->dL_dsh) % 16) != 0) pb.sh_bulk_ok = 0;
     pb.raw_params = a->raw_params; pb.quat_norm_mode = g_quat_norm_mode;
     pb.shs_rest = a->shs ? a->shs_rest : nullptr; pb.dL_dsh_rest = a->dL_dsh_rest;
-    if (pb.shs_rest && a->dL_dsh && !a->dL_dsh_rest) return fail(FDGS_ERR_INVALID_ARG, "split SH rows need dL_dsh_rest");
-    if (!pb.shs_rest && a->dL_dsh_rest) return fail(FDGS_ERR_INVALID_ARG, "dL_dsh_rest without shs_rest");
     pb.dL_dmean2D = a->dL_dmean2D; pb.dL_dconic = a->dL_dconic; pb.dL_dopacity = a->dL_dopacity; pb.dL_dcolor = a->dL_dcolor;
     pb.dL_dmean3D = a->dL_dmean3D; pb.dL_dcov3D = a->dL_dcov3D; pb.dL_dsh = a->dL_dsh; pb.sh_factors = a->sh_factors;
     pb.dL_dts = a->dL_dts;
     pb.dL_dscale = a->dL_dscale; pb.dL_dscale_t = a->dL_dscale_t; pb.dL_drot = a->dL_drot; pb.dL_drot_r = a->dL_drot_r;
-    if (pb.has_scales && pb.rot_4d && (!a->rotations_r || !a->scales_t || !a->ts || !a->opacities))
-        return fail(FDGS_ERR_INVALID_ARG, "rot_4d backward needs rotations_r, scales_t, ts, opacities");
-    FDGS_STAGE(7, fdgs::preprocess_bwd_kernel_count(pb), fdgs::launch_preprocess_bwd(pb, stream), "preprocess_bwd");
+    pb.vb = vb; pb.factor_stride = BatchBwdScratch::factor_stride(P);
+    FDGS_STAGE(7, fdgs::preprocess_bwd_kernel_count(pb), fdgs::launch_preprocess_bwd(pb, stream),
+               batch ? "preprocess_bwd (batch)" : "preprocess_bwd");
     return FDGS_OK;
+}
+
+int backward_impl(const fdgs_backward_args* a, const float* bg_image, float* dL_dbg_image, void* stream_v) {
+    g_last_error.clear();
+    if (!a) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    const int P = a->P, W = a->width, H = a->height, R = a->R;
+    if (P <= 0 && !dL_dbg_image) return FDGS_OK;
+    if (W <= 0 || H <= 0 || R < 0) return fail(FDGS_ERR_INVALID_ARG, "bad width / height / R");
+    if (P <= 0) {
+        if (!a->image_buffer || !a->dL_dpix || !a->background)
+            return fail(FDGS_ERR_INVALID_ARG, "image buffer / colour image gradient / background required");
+    } else {
+        if (!a->geom_buffer || !a->image_buffer || (R > 0 && !a->binning_buffer))
+            return fail(FDGS_ERR_INVALID_ARG, "scratch buffers of the forward pass required");
+        // dL_depths / dL_masks / dL_dpix_flow may be NULL: no upstream gradient for that image
+        if (!a->dL_dpix) return fail(FDGS_ERR_INVALID_ARG, "colour image gradient required");
+        if (!a->background || !a->radii || !a->out_means3D || !a->viewmatrix || !a->projmatrix || !a->campos)
+            return fail(FDGS_ERR_INVALID_ARG, "background / radii / out_means3D / viewmatrix / projmatrix / campos required");
+        if (a->sh_factors && a->dL_dsh) return fail(FDGS_ERR_INVALID_ARG, "sh_factors and dL_dsh are mutually exclusive");
+        if (!a->dL_dmean2D || !a->dL_dconic || !a->dL_dopacity || !a->dL_dcolor || !a->dL_dflows || !a->dL_dmean3D ||
+            !a->dL_dcov3D || !a->dL_dts || !a->dL_dscale || !a->dL_dscale_t || !a->dL_drot || !a->dL_drot_r)
+            return fail(FDGS_ERR_INVALID_ARG, "gradient outputs required");
+        const bool split = a->shs && a->shs_rest;   // split SH rows are read only with shs
+        if (split && a->dL_dsh && !a->dL_dsh_rest) return fail(FDGS_ERR_INVALID_ARG, "split SH rows need dL_dsh_rest");
+        if (!split && a->dL_dsh_rest) return fail(FDGS_ERR_INVALID_ARG, "dL_dsh_rest without shs_rest");
+        if (a->scales && a->rot_4d && (!a->rotations_r || !a->scales_t || !a->ts || !a->opacities))
+            return fail(FDGS_ERR_INVALID_ARG, "rot_4d backward needs rotations_r, scales_t, ts, opacities");
+    }
+    GeomState geom = GeomState::carve(align128(const_cast<char*>(a->geom_buffer)), P);
+    ImageState img = ImageState::carve(align128(const_cast<char*>(a->image_buffer)), W, H);
+    return backward_stages(a, bg_image, dL_dbg_image, {1, nullptr}, geom, img, reinterpret_cast<cudaStream_t>(stream_v));
 }
 
 // ---- batched views: B cameras of the same Gaussians in one pass per stage (include/fdgs.h: fdgs_forward_batch) -------
@@ -519,17 +525,15 @@ int forward_batch_impl(const fdgs_forward_batch_args* b, fdgs_alloc_fn geom_allo
     if (a->P > 0 && (a->colors_precomp || a->cov3D_precomp))
         return fail(FDGS_ERR_INVALID_ARG, "the batched entry takes SH and scales / rotations, not precomputed colours or covariances");
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
-    const bool debug = a->debug != 0;
     const int P = a->P, W = a->width, H = a->height;
     const int grid_x = (W + fdgs::TILE_X - 1) / fdgs::TILE_X, grid_y = (H + fdgs::TILE_Y - 1) / fdgs::TILE_Y;
-    const int tiles = grid_x * grid_y;
-    if ((long long)tiles * B > 0x7fffffffLL || (long long)P * B > 0x7fffffffLL)
+    if ((long long)grid_x * grid_y * B > 0x7fffffffLL || (long long)P * B > 0x7fffffffLL)
         return fail(FDGS_ERR_UNSUPPORTED, "B * tiles or B * P exceeds 2^31 - 1");
 
     const size_t geom_bytes = fdgs_geom_batch_bytes(P, B);
     char* geom_raw = geom_alloc(geom_ctx, geom_bytes);
     if (!geom_raw) return fail(FDGS_ERR_ALLOC, "geometry buffer allocation failed");
-    BatchGeomState geom = BatchGeomState::carve(align128(geom_raw), P, B);
+    GeomState geom = GeomState::carve(align128(geom_raw), P, true, B);
     const size_t img_bytes = fdgs_image_batch_bytes(W, H, B);
     char* img_raw = image_alloc(image_ctx, img_bytes);
     if (!img_raw) return fail(FDGS_ERR_ALLOC, "image buffer allocation failed");
@@ -538,7 +542,7 @@ int forward_batch_impl(const fdgs_forward_batch_args* b, fdgs_alloc_fn geom_allo
     res->geom_bytes = geom_bytes;
     res->image_buffer = img_raw;
     res->image_bytes = img_bytes;
-    res->cov3D = geom.g.cov3D;
+    res->cov3D = geom.cov3D;
 
     // the per-view scalars, focal lengths computed as the single-view entry computes them (reference: rasterizer_impl.cu:235-236);
     // a pageable host-to-device copy is staged before the call returns and does not synchronise
@@ -552,69 +556,7 @@ int forward_batch_impl(const fdgs_forward_batch_args* b, fdgs_alloc_fn geom_allo
         vs[v].focal_x = W / (2.0f * b->tan_fovx[v]);
     }
     FDGS_CUDA(cudaMemcpyAsync(geom.scalars, vs.data(), vs.size() * sizeof(vs[0]), cudaMemcpyHostToDevice, stream), "view table copy");
-
-    if (P > 0) {
-        fdgs::PreprocessFwdParams pp;
-        memset(&pp, 0, sizeof(pp));
-        pp.P = P; pp.D = a->D; pp.D_t = a->D_t; pp.M = a->M;
-        pp.means3D = a->means3D; pp.ts = a->ts; pp.scales = a->scales; pp.scales_t = a->scales_t;
-        pp.scale_modifier = a->scale_modifier; pp.rotations = a->rotations; pp.rotations_r = a->rotations_r;
-        pp.opacities = a->opacities; pp.shs = a->shs; pp.prefilter_var = a->prefilter_var;
-        pp.viewmatrix = a->viewmatrix; pp.projmatrix = a->projmatrix; pp.cam_pos = a->cam_pos;
-        pp.time_duration = a->time_duration;
-        pp.rot_4d = a->rot_4d; pp.gaussian_dim = a->gaussian_dim; pp.force_sh_3d = a->force_sh_3d;
-        pp.W = W; pp.H = H; pp.grid_x = grid_x; pp.grid_y = grid_y; pp.prefiltered = a->prefiltered;
-        sh_staging(a->shs, a->M, true, &pp.sh_bulk_ok, &pp.sh_row_stride_floats);
-        pp.raw_params = a->raw_params; pp.quat_norm_mode = g_quat_norm_mode; pp.shs_rest = a->shs_rest;
-        pp.flows = a->flows_precomp;
-        pp.out_means3D = a->out_means3D; pp.radii = a->radii; pp.cov3D = geom.g.cov3D; pp.grec = geom.g.grec;
-        pp.clamped = geom.g.clamped; pp.tiles_touched = geom.g.tiles_touched; pp.binrec = geom.g.binrec;
-        pp.tile_cull = g_tile_cull.load();
-        pp.vb.B = B; pp.vb.scalars = geom.scalars;
-        FDGS_STAGE(0, 1, fdgs::launch_preprocess_fwd(pp, stream), "preprocess_fwd (batch)");
-    }
-    FDGS_STAGE(1, (P > 0 ? 1 : 0) + 2,
-               [&]() {
-                   cudaError_t e = fdgs::launch_bin_count(P, geom.g.binrec, grid_x, grid_y, img.bin_matrix, stream, B, true);
-                   if (e != cudaSuccess) return e;
-                   return fdgs::launch_tile_scan((int)img.tiles, img.bin_matrix, img.tile_total, img.tile_offset, img.ranges,
-                                                 img.bin_info, stream);
-               }(),
-               "bin_count + tile_scan (batch)");
-    // the one host synchronisation of the batch: R over all views, the largest tile of any view, the overflow flag
-    int bin_info[4] = {0, 0, 0, 0};
-    FDGS_CUDA(cudaMemcpyAsync(bin_info, img.bin_info, sizeof(bin_info), cudaMemcpyDeviceToHost, stream), "num_rendered copy");
-    FDGS_CUDA(cudaStreamSynchronize(stream), "num_rendered sync");
-    const int num_rendered = bin_info[0];
-    if (num_rendered < 0 || bin_info[2] != 0) return fail(FDGS_ERR_UNSUPPORTED, "more than 2^31 - 1 tile instances");
-    res->num_rendered = num_rendered;
-
-    const size_t bin_bytes = fdgs_binning_bytes(num_rendered, W, H);
-    char* bin_raw = binning_alloc(binning_ctx, bin_bytes);
-    if (!bin_raw) return fail(FDGS_ERR_ALLOC, "binning buffer allocation failed");
-    BinningState bin = BinningState::carve(align128(bin_raw), num_rendered);
-    res->binning_buffer = bin_raw;
-    res->binning_bytes = bin_bytes;
-
-    if (num_rendered > 0) {
-        FDGS_STAGE(2, 1,
-                   fdgs::launch_bin_scatter(P, geom.g.binrec, grid_x, grid_y, img.bin_matrix, img.tile_offset, bin.keys, stream,
-                                            B, true),
-                   "bin_scatter (batch)");
-        FDGS_STAGE(3, fdgs::tile_sort_pack_kernel_count(bin_info[1]),
-                   fdgs::launch_tile_sort_pack((int)img.tiles, bin_info[1], num_rendered, img.ranges, bin.keys, geom.g.grec,
-                                               bin.recs, bin.point_list, stream, tiles, P),
-                   "tile_sort_pack (batch)");
-    }
-    fdgs::BlendFwdParams bp;
-    bp.W = W; bp.H = H; bp.grid_x = grid_x; bp.grid_y = grid_y;
-    bp.ranges = img.ranges; bp.recs = bin.recs; bp.background = a->background;
-    bp.final_T = img.final_T; bp.n_contrib = img.n_contrib;
-    bp.out_color = a->out_color; bp.out_flow = a->out_flow; bp.out_depth = a->out_depth; bp.out_T = a->out_T;
-    bp.bg_image = b->bg_image;
-    bp.views = B;
-    FDGS_STAGE(5, 1, fdgs::launch_blend_fwd(bp, stream), "blend_fwd (batch)");
-    return FDGS_OK;
+    return forward_stages(a, b->bg_image, {B, geom.scalars}, geom, img, binning_alloc, binning_ctx, stream, res);
 }
 
 int backward_batch_impl(const fdgs_backward_batch_args* b, void* stream_v) {
@@ -632,19 +574,10 @@ int backward_batch_impl(const fdgs_backward_batch_args* b, void* stream_v) {
     const int grid_x = (W + fdgs::TILE_X - 1) / fdgs::TILE_X, grid_y = (H + fdgs::TILE_Y - 1) / fdgs::TILE_Y;
     if ((long long)grid_x * grid_y * B > 0x7fffffffLL || (long long)P * B > 0x7fffffffLL)
         return fail(FDGS_ERR_UNSUPPORTED, "B * tiles or B * P exceeds 2^31 - 1");
+    GeomState geom = GeomState::carve(align128(const_cast<char*>(a->geom_buffer)), P, true, B);
     ImageState img = ImageState::carve(align128(const_cast<char*>(a->image_buffer)), W, H, B);
-    fdgs::BlendBwdParams bp;
-    memset(&bp, 0, sizeof(bp));
-    bp.W = W; bp.H = H; bp.grid_x = grid_x; bp.grid_y = grid_y;
-    bp.ranges = img.ranges; bp.background = a->background; bp.final_T = img.final_T; bp.n_contrib = img.n_contrib;
-    bp.dL_dpix = a->dL_dpix; bp.dL_depths = a->dL_depths; bp.dL_masks = a->dL_masks; bp.dL_dpix_flow = a->dL_dpix_flow;
-    bp.bg_image = b->bg_image; bp.dL_dbg_image = b->dL_dbg_image;
-    bp.views = B; bp.P = P;
-    if (P == 0) {
-        // nothing was rendered: the background image takes the whole colour gradient
-        if (b->dL_dbg_image) FDGS_STAGE(6, 1, fdgs::launch_blend_bwd(bp, stream), "blend_bwd (batch)");
-        return FDGS_OK;
-    }
+    const fdgs::ViewBatch vb = {B, geom.scalars};
+    if (P == 0) return backward_stages(a, b->bg_image, b->dL_dbg_image, vb, geom, img, stream);
     if (R > 0 && !a->binning_buffer) return fail(FDGS_ERR_INVALID_ARG, "scratch buffers of the forward pass required");
     if (!a->radii || !a->out_means3D || !a->viewmatrix || !a->projmatrix || !a->campos)
         return fail(FDGS_ERR_INVALID_ARG, "radii / out_means3D / viewmatrix / projmatrix / campos required");
@@ -658,38 +591,17 @@ int backward_batch_impl(const fdgs_backward_batch_args* b, void* stream_v) {
     if (a->shs_rest && !a->dL_dsh_rest) return fail(FDGS_ERR_INVALID_ARG, "split SH rows need dL_dsh_rest");
     if (!a->shs_rest && a->dL_dsh_rest) return fail(FDGS_ERR_INVALID_ARG, "dL_dsh_rest without shs_rest");
 
-    BatchGeomState geom = BatchGeomState::carve(align128(const_cast<char*>(a->geom_buffer)), P, B);
-    BinningState bin = BinningState::carve(a->binning_buffer ? align128(const_cast<char*>(a->binning_buffer)) : nullptr, R);
     BatchBwdScratch sc = BatchBwdScratch::carve(align128(b->scratch), P, B);
     FDGS_CUDA(cudaMemsetAsync(sc.dL_dconic, 0, sc.zero_bytes, stream), "zero the accumulated gradients");
-
-    bool blend_raw = false;
-    if (R > 0 || b->dL_dbg_image) {
-        bp.recs = bin.recs;
-        bp.dL_dmean2D = a->dL_dmean2D; bp.dL_dconic = sc.dL_dconic; bp.dL_dopacity = sc.dL_dopacity;
-        bp.dL_dcolor = sc.dL_dcolor; bp.dL_dflows = sc.dL_dflows;
-        blend_raw = R > 0 && fdgs::blend_bwd_is_raw(bp);
-        FDGS_STAGE(6, 1, fdgs::launch_blend_bwd(bp, stream), "blend_bwd (batch)");
-    }
-    fdgs::PreprocessBwdParams pb;
-    memset(&pb, 0, sizeof(pb));
-    pb.P = P; pb.D = a->D; pb.D_t = a->D_t; pb.M = a->M;
-    pb.means3D = a->out_means3D; pb.radii = a->radii; pb.shs = a->shs; pb.ts = a->ts; pb.opacities = a->opacities;
-    pb.clamped = geom.g.clamped; pb.tiles_touched = geom.g.tiles_touched;
-    pb.scales = a->scales; pb.scales_t = a->scales_t; pb.rotations = a->rotations; pb.rotations_r = a->rotations_r;
-    pb.scale_modifier = a->scale_modifier; pb.cov3D = geom.g.cov3D;
-    pb.prefilter_var = a->prefilter_var; pb.viewmatrix = a->viewmatrix; pb.projmatrix = a->projmatrix; pb.campos = a->campos;
-    pb.time_duration = a->time_duration;
-    pb.rot_4d = a->rot_4d; pb.gaussian_dim = a->gaussian_dim; pb.force_sh_3d = a->force_sh_3d;
-    pb.has_scales = 1;
-    pb.grec = geom.g.grec; pb.blend_raw = blend_raw ? 1 : 0; pb.W = W; pb.H = H;
-    sh_staging(a->shs, a->M, false, &pb.sh_bulk_ok, &pb.sh_row_stride_floats);
-    pb.raw_params = a->raw_params; pb.quat_norm_mode = g_quat_norm_mode; pb.shs_rest = a->shs_rest;
-    pb.dL_dmean2D = a->dL_dmean2D; pb.dL_dconic = sc.dL_dconic; pb.dL_dopacity = sc.dL_dopacity; pb.dL_dcolor = sc.dL_dcolor;
-    pb.dL_dmean3D = sc.dL_dmean3D; pb.dL_dcov3D = sc.dL_dcov3D; pb.sh_factors = sc.table; pb.dL_dts = sc.dL_dts;
-    pb.dL_dscale = sc.dL_dscale; pb.dL_dscale_t = sc.dL_dscale_t; pb.dL_drot = sc.dL_drot; pb.dL_drot_r = sc.dL_drot_r;
-    pb.vb.B = B; pb.vb.scalars = geom.scalars; pb.factor_stride = BatchBwdScratch::factor_stride(P);
-    FDGS_STAGE(7, fdgs::preprocess_bwd_kernel_count(pb), fdgs::launch_preprocess_bwd(pb, stream), "preprocess_bwd (batch)");
+    // the stages write every view's gradients into the scratch stacks and its colour factors into the sh_outer_sum table;
+    // dL_dmean2D stays the caller's [B,P,3]
+    fdgs_backward_args views = *a;
+    views.dL_dconic = sc.dL_dconic; views.dL_dopacity = sc.dL_dopacity; views.dL_dcolor = sc.dL_dcolor;
+    views.dL_dflows = sc.dL_dflows; views.dL_dmean3D = sc.dL_dmean3D; views.dL_dcov3D = sc.dL_dcov3D;
+    views.dL_dsh = nullptr; views.sh_factors = sc.table; views.dL_dsh_rest = nullptr; views.dL_dts = sc.dL_dts;
+    views.dL_dscale = sc.dL_dscale; views.dL_dscale_t = sc.dL_dscale_t; views.dL_drot = sc.dL_drot;
+    views.dL_drot_r = sc.dL_drot_r;
+    if (int rc = backward_stages(&views, b->bg_image, b->dL_dbg_image, vb, geom, img, stream)) return rc;
 
     // every per-Gaussian gradient but the SH rows: summed over the views in view order
     fdgs::ViewSumParams vsum;

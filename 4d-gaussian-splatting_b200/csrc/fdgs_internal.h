@@ -37,7 +37,8 @@ struct ViewScalars {
     float timestamp, tan_fovx, tan_fovy, focal_x, focal_y, pad[3];
 };
 // Batched kernels run one view per blockIdx.y (per-Gaussian kernels) or blockIdx.z (tile kernels); every per-view
-// array is a [B][...] stack with the stride of one view's array.  The single-view instantiations never read these.
+// array is a [B][...] stack with the stride of one view's array.  One view is {1, NULL}: the single-view instantiations
+// never read these.
 struct ViewBatch {
     int B;                      // views
     const ViewScalars* scalars; // [B] device
@@ -95,22 +96,21 @@ cudaError_t launch_debug_activate(int n, const float* log_s, const float* logit,
 int bin_ctas();                                 // rows of the [bin_ctas()][num_tiles] count matrix
 // binrec[i] = { x0 | y0 << 16, x1 | y1 << 16, depth bits, tile mask }: tile rectangle (empty = not listed anywhere) of
 // Gaussian i; for rectangles of up to 32 tiles bit j of the mask = tile j (row-major) takes an instance
-// views > 1 (the batched entry, any views >= 1 with batch = true): binrec is a [views][P] stack, the matrix has
-// views * grid_x * grid_y columns and view v's tiles are the columns v * tiles .. v * tiles + tiles - 1
-cudaError_t launch_bin_count(int P, const uint4* binrec, int grid_x, int grid_y, uint32_t* matrix, cudaStream_t stream,
-                             int views = 1, bool batch = false);
+// a batch (vb.scalars != NULL): binrec is a [vb.B][P] stack, the matrix has vb.B * grid_x * grid_y columns and view v's
+// tiles are the columns v * tiles .. v * tiles + tiles - 1
+cudaError_t launch_bin_count(int P, const uint4* binrec, int grid_x, int grid_y, uint32_t* matrix, const ViewBatch& vb,
+                             cudaStream_t stream);
 // matrix -> per-CTA column prefixes; tile_offset / ranges; info[0] = total instances R, info[1] = largest tile
 cudaError_t launch_tile_scan(int num_tiles, uint32_t* matrix, uint32_t* tile_total, uint32_t* tile_offset, uint2* ranges,
                              uint32_t* info, cudaStream_t stream);
 cudaError_t launch_bin_scatter(int P, const uint4* binrec, int grid_x, int grid_y, uint32_t* matrix,
-                               const uint32_t* tile_offset, uint64_t* keys, cudaStream_t stream, int views = 1,
-                               bool batch = false);
-// sorts every tile's keys and writes the 64-byte instance records + the sorted index list.  tiles_per_view > 0 (the
-// batched entry): num_tiles = views * tiles_per_view and tile t gathers from grec's view slice t / tiles_per_view
+                               const uint32_t* tile_offset, uint64_t* keys, const ViewBatch& vb, cudaStream_t stream);
+// sorts every tile's keys and writes the 64-byte instance records + the sorted index list.  A batch: num_tiles =
+// vb.B * tiles per view, and every tile gathers from the slice of its view in grec, a [vb.B][P] stack
 int tile_sort_pack_kernel_count(int max_count);
 cudaError_t launch_tile_sort_pack(int num_tiles, int max_count, int R, const uint2* ranges, uint64_t* keys,
-                                  const InstRec* grec, StageRec* recs, uint32_t* point_list, cudaStream_t stream,
-                                  int tiles_per_view = 0, int P = 0);
+                                  const InstRec* grec, int P, StageRec* recs, uint32_t* point_list, const ViewBatch& vb,
+                                  cudaStream_t stream);
 cudaError_t launch_unpack_grec(int P, const InstRec* grec, const int* radii, float* depths, float* means2D,
                                float* conic_opacity, float* rgb, cudaStream_t stream);
 

@@ -66,6 +66,72 @@ const float* fptr(const torch::Tensor& t) {
 
 torch::Tensor contig(const torch::Tensor& t) { return (t.defined() && t.numel() > 0) ? t.contiguous() : t; }
 
+bool provided(const torch::Tensor& t) { return t.defined() && t.numel() != 0; }
+
+// The contiguous copies of a call's input tensors, kept alive until the call returns
+struct Inputs {
+    std::vector<torch::Tensor> held;
+    const float* operator()(const torch::Tensor& t) {
+        held.push_back(contig(t));
+        return fptr(held.back());
+    }
+    const char* bytes(const torch::Tensor& t) {
+        held.push_back(contig(t));
+        return provided(held.back()) ? reinterpret_cast<const char*>(held.back().data_ptr()) : nullptr;
+    }
+};
+
+// SH coefficients per Gaussian: sh [P,M,3], or the raw-parameter entry's split rows sh [P,1,3] + sh_rest [P,M-1,3]
+int sh_coefficients(const torch::Tensor& sh, const torch::Tensor& sh_rest) {
+    return (provided(sh) ? (int)sh.size(1) : 0) + (provided(sh_rest) ? (int)sh_rest.size(1) : 0);
+}
+
+// The fields of fdgs_forward_args that the single-view and the batched binding fill alike: the Gaussians, the
+// background colour, the image size and the flags.  The camera, the outputs and the precomputed colours / covariances
+// are the caller's.
+void forward_gaussians(fdgs_forward_args& a, Inputs& in, const torch::Tensor& background, const torch::Tensor& means3D,
+                       const torch::Tensor& flows, const torch::Tensor& opacity, const torch::Tensor& ts,
+                       const torch::Tensor& scales, const torch::Tensor& scales_t, const torch::Tensor& rotations,
+                       const torch::Tensor& rotations_r, float scale_modifier, float prefilter_var, const torch::Tensor& sh,
+                       const torch::Tensor& sh_rest, int degree, int degree_t, float time_duration, bool rot_4d,
+                       int gaussian_dim, bool force_sh_3d, bool prefiltered, bool debug, bool raw_params, int H, int W) {
+    a.P = means3D.size(0); a.D = degree; a.D_t = degree_t; a.M = sh_coefficients(sh, sh_rest);
+    if (provided(sh_rest))
+        TORCH_CHECK(provided(sh) && sh.size(1) == 1 && sh_rest.dim() == 3 && sh_rest.size(0) == a.P,
+                    "fdgs: split SH rows are [P,1,3] + [P,M-1,3]");
+    a.shs_rest = in(sh_rest); a.raw_params = raw_params;
+    a.background = in(background); a.width = W; a.height = H;
+    a.means3D = in(means3D); a.shs = in(sh); a.flows_precomp = in(flows);
+    a.opacities = in(opacity); a.ts = in(ts); a.scales = in(scales); a.scales_t = in(scales_t);
+    a.scale_modifier = scale_modifier; a.rotations = in(rotations); a.rotations_r = in(rotations_r);
+    a.prefilter_var = prefilter_var; a.time_duration = time_duration; a.rot_4d = rot_4d; a.gaussian_dim = gaussian_dim;
+    a.force_sh_3d = force_sh_3d; a.prefiltered = prefiltered; a.debug = debug;
+}
+
+// The same for fdgs_backward_args, with the forward's scratch buffers and the image gradients
+void backward_gaussians(fdgs_backward_args& a, Inputs& in, const torch::Tensor& background, const torch::Tensor& means3D,
+                        const torch::Tensor& flows, const torch::Tensor& opacities, const torch::Tensor& ts,
+                        const torch::Tensor& scales, const torch::Tensor& scales_t, const torch::Tensor& rotations,
+                        const torch::Tensor& rotations_r, float scale_modifier, float prefilter_var, const torch::Tensor& sh,
+                        const torch::Tensor& sh_rest, int degree, int degree_t, float time_duration, bool rot_4d,
+                        int gaussian_dim, bool force_sh_3d, bool debug, bool raw_params, int H, int W,
+                        const torch::Tensor& dL_dout_color, const torch::Tensor& dL_dout_depth,
+                        const torch::Tensor& dL_dout_mask, const torch::Tensor& dL_dout_flow,
+                        const torch::Tensor& geomBuffer, int R, const torch::Tensor& binningBuffer,
+                        const torch::Tensor& imageBuffer) {
+    a.P = means3D.size(0); a.D = degree; a.D_t = degree_t; a.M = sh_coefficients(sh, sh_rest); a.R = R;
+    a.shs_rest = in(sh_rest); a.raw_params = raw_params;
+    a.background = in(background); a.width = W; a.height = H;
+    a.shs = in(sh); a.flows_2d = in(flows);
+    a.opacities = in(opacities); a.ts = in(ts); a.scales = in(scales); a.scales_t = in(scales_t);
+    a.scale_modifier = scale_modifier; a.rotations = in(rotations); a.rotations_r = in(rotations_r);
+    a.prefilter_var = prefilter_var; a.time_duration = time_duration; a.rot_4d = rot_4d; a.gaussian_dim = gaussian_dim;
+    a.force_sh_3d = force_sh_3d; a.debug = debug;
+    a.geom_buffer = in.bytes(geomBuffer); a.binning_buffer = in.bytes(binningBuffer); a.image_buffer = in.bytes(imageBuffer);
+    a.dL_dpix = in(dL_dout_color); a.dL_depths = in(dL_dout_depth); a.dL_masks = in(dL_dout_mask);
+    a.dL_dpix_flow = in(dL_dout_flow);
+}
+
 // the per-pixel background image of a call, checked against the image size (undefined / empty = none)
 torch::Tensor background_image(const torch::Tensor& bg_image, const torch::Tensor& like, int H, int W) {
     if (!bg_image.defined() || bg_image.numel() == 0) return torch::Tensor();
@@ -155,32 +221,15 @@ ForwardOut RasterizeGaussiansExt(const torch::Tensor& background, const torch::T
     torch::Tensor binningBuffer = torch::empty({0}, bopts);
     torch::Tensor imgBuffer = torch::empty({0}, bopts);
 
-    // keep contiguous copies alive for the duration of the call
-    const auto bg_c = contig(background), means_c = contig(means3D), col_c = contig(colors), flow_c = contig(flows),
-               op_c = contig(opacity), ts_c = contig(ts), sc_c = contig(scales), sct_c = contig(scales_t),
-               rot_c = contig(rotations), rotr_c = contig(rotations_r), cov_c = contig(cov3D_precomp),
-               view_c = contig(viewmatrix), proj_c = contig(projmatrix), sh_c = contig(sh), cam_c = contig(campos);
-
     fdgs_forward_args a;
     memset(&a, 0, sizeof(a));
-    a.P = P; a.D = degree; a.D_t = degree_t;
-    const auto shr_c = contig(sh_rest);
-    a.M = (sh.defined() && sh.numel() != 0) ? (int)sh.size(1) : 0;
-    if (shr_c.defined() && shr_c.numel() != 0) {
-        TORCH_CHECK(a.M == 1 && shr_c.dim() == 3 && shr_c.size(0) == P, "fdgs: split SH rows are [P,1,3] + [P,M-1,3]");
-        a.M += (int)shr_c.size(1);
-        a.shs_rest = fptr(shr_c);
-    }
-    a.raw_params = raw_params;
-    a.background = fptr(bg_c); a.width = W; a.height = H;
-    a.means3D = fptr(means_c); a.shs = fptr(sh_c); a.colors_precomp = fptr(col_c); a.flows_precomp = fptr(flow_c);
-    a.opacities = fptr(op_c); a.ts = fptr(ts_c); a.scales = fptr(sc_c); a.scales_t = fptr(sct_c);
-    a.scale_modifier = scale_modifier; a.rotations = fptr(rot_c); a.rotations_r = fptr(rotr_c);
-    a.cov3D_precomp = fptr(cov_c); a.prefilter_var = prefilter_var;
-    a.viewmatrix = fptr(view_c); a.projmatrix = fptr(proj_c); a.cam_pos = fptr(cam_c);
-    a.timestamp = timestamp; a.time_duration = time_duration; a.rot_4d = rot_4d; a.gaussian_dim = gaussian_dim;
-    a.force_sh_3d = force_sh_3d; a.tan_fovx = tan_fovx; a.tan_fovy = tan_fovy; a.prefiltered = prefiltered;
-    a.debug = debug;
+    Inputs in;
+    forward_gaussians(a, in, background, means3D, flows, opacity, ts, scales, scales_t, rotations, rotations_r, scale_modifier,
+                      prefilter_var, sh, sh_rest, degree, degree_t, time_duration, rot_4d, gaussian_dim, force_sh_3d,
+                      prefiltered, debug, raw_params, H, W);
+    a.colors_precomp = in(colors); a.cov3D_precomp = in(cov3D_precomp);
+    a.viewmatrix = in(viewmatrix); a.projmatrix = in(projmatrix); a.cam_pos = in(campos);
+    a.timestamp = timestamp; a.tan_fovx = tan_fovx; a.tan_fovy = tan_fovy;
     a.out_means3D = out_means3D.data_ptr<float>(); a.out_color = out_color.data_ptr<float>();
     a.out_flow = out_flow.data_ptr<float>(); a.out_depth = out_depth.data_ptr<float>();
     a.out_T = out_T.data_ptr<float>(); a.radii = radii.data_ptr<int>();
@@ -244,8 +293,8 @@ RasterizeGaussiansBackwardExt(const torch::Tensor& background, const torch::Tens
     const DeviceStream on(means3D);
     const int P = means3D.size(0);
     const int H = dL_dout_color.size(1), W = dL_dout_color.size(2);
-    const bool split = sh_rest.defined() && sh_rest.numel() != 0;
-    const int M = ((sh.defined() && sh.numel() != 0) ? (int)sh.size(1) : 0) + (split ? (int)sh_rest.size(1) : 0);
+    const bool split = provided(sh_rest);
+    const int M = sh_coefficients(sh, sh_rest);
     auto opts = means3D.options().dtype(torch::kFloat32);
 
     // accumulated by the blend kernel -> one zero-filled slab, sliced into the five API tensors
@@ -272,39 +321,24 @@ RasterizeGaussiansBackwardExt(const torch::Tensor& background, const torch::Tens
     const auto bgi_c = background_image(bg_image, means3D, H, W);
 
     if (P != 0 || want_dbg) {
-        const auto bg_c = contig(background), om_c = contig(out_means3D), rad_c = contig(radii), col_c = contig(colors),
-                   flow_c = contig(flows_2d), op_c = contig(opacities), ts_c = contig(ts), sc_c = contig(scales),
-                   sct_c = contig(scales_t), rot_c = contig(rotations), rotr_c = contig(rotations_r),
-                   cov_c = contig(cov3D_precomp), view_c = contig(viewmatrix), proj_c = contig(projmatrix),
-                   gc_c = contig(dL_dout_color), gd_c = contig(dL_dout_depth), gm_c = contig(dL_dout_mask),
-                   gf_c = contig(dL_dout_flow), sh_c = contig(sh), cam_c = contig(campos), geo_c = contig(geomBuffer),
-                   bin_c = contig(binningBuffer), img_c = contig(imageBuffer);
         fdgs_backward_args a;
         memset(&a, 0, sizeof(a));
-        a.P = P; a.D = degree; a.D_t = degree_t; a.M = M; a.R = R;
-        a.background = fptr(bg_c); a.width = W; a.height = H;
-        a.out_means3D = fptr(om_c); a.shs = fptr(sh_c); a.colors_precomp = fptr(col_c); a.flows_2d = fptr(flow_c);
-        a.opacities = fptr(op_c); a.ts = fptr(ts_c); a.scales = fptr(sc_c); a.scales_t = fptr(sct_c);
-        a.scale_modifier = scale_modifier; a.rotations = fptr(rot_c); a.rotations_r = fptr(rotr_c);
-        a.cov3D_precomp = fptr(cov_c); a.prefilter_var = prefilter_var;
-        a.viewmatrix = fptr(view_c); a.projmatrix = fptr(proj_c); a.campos = fptr(cam_c);
-        a.timestamp = timestamp; a.time_duration = time_duration; a.rot_4d = rot_4d; a.gaussian_dim = gaussian_dim;
-        a.force_sh_3d = force_sh_3d; a.tan_fovx = tan_fovx; a.tan_fovy = tan_fovy;
+        Inputs in;
+        backward_gaussians(a, in, background, means3D, flows_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
+                           scale_modifier, prefilter_var, sh, sh_rest, degree, degree_t, time_duration, rot_4d, gaussian_dim,
+                           force_sh_3d, debug, raw_params, H, W, dL_dout_color, dL_dout_depth, dL_dout_mask, dL_dout_flow,
+                           geomBuffer, R, binningBuffer, imageBuffer);
+        a.out_means3D = in(out_means3D); a.colors_precomp = in(colors); a.cov3D_precomp = in(cov3D_precomp);
+        a.viewmatrix = in(viewmatrix); a.projmatrix = in(projmatrix); a.campos = in(campos);
+        a.timestamp = timestamp; a.tan_fovx = tan_fovx; a.tan_fovy = tan_fovy;
+        const auto rad_c = contig(radii);
         a.radii = rad_c.numel() ? rad_c.data_ptr<int>() : nullptr;
-        a.geom_buffer = geo_c.numel() ? reinterpret_cast<const char*>(geo_c.data_ptr()) : nullptr;
-        a.binning_buffer = bin_c.numel() ? reinterpret_cast<const char*>(bin_c.data_ptr()) : nullptr;
-        a.image_buffer = reinterpret_cast<const char*>(img_c.data_ptr());
-        a.dL_dpix = fptr(gc_c); a.dL_depths = fptr(gd_c); a.dL_masks = fptr(gm_c); a.dL_dpix_flow = fptr(gf_c);
-        a.debug = debug;
         a.dL_dmean2D = dL_dmeans2D.data_ptr<float>(); a.dL_dconic = dL_dconic.data_ptr<float>();
         a.dL_dopacity = dL_dopacity.data_ptr<float>(); a.dL_dcolor = dL_dcolors.data_ptr<float>();
         a.dL_dflows = dL_dflows.data_ptr<float>(); a.dL_dmean3D = dL_dmeans3D.data_ptr<float>();
         a.dL_dcov3D = dL_dcov3D.data_ptr<float>(); a.dL_dsh = (M > 0 && !factors) ? dL_dsh.data_ptr<float>() : nullptr;
         a.sh_factors = factors ? sh_factors.data_ptr<float>() : nullptr;
-        const auto shr_c = contig(sh_rest);
-        a.shs_rest = split ? fptr(shr_c) : nullptr;
         a.dL_dsh_rest = (split && !factors) ? dL_dsh_rest.data_ptr<float>() : nullptr;
-        a.raw_params = raw_params;
         a.dL_dts = dL_dts.data_ptr<float>(); a.dL_dscale = dL_dscales.data_ptr<float>();
         a.dL_dscale_t = dL_dscales_t.data_ptr<float>(); a.dL_drot = dL_drotations.data_ptr<float>();
         a.dL_drot_r = dL_drotations_r.data_ptr<float>();
@@ -413,28 +447,14 @@ RasterizeGaussiansBatch(const torch::Tensor& background, const torch::Tensor& me
     torch::Tensor out_means3D = torch::empty({B, P, 3}, fopts);
     torch::Tensor geomBuffer = torch::empty({0}, bopts), binningBuffer = torch::empty({0}, bopts),
                   imgBuffer = torch::empty({0}, bopts);
-    const auto bg_c = contig(background), means_c = contig(means3D), flow_c = contig(flows), op_c = contig(opacity),
-               ts_c = contig(ts), sc_c = contig(scales), sct_c = contig(scales_t), rot_c = contig(rotations),
-               rotr_c = contig(rotations_r), sh_c = contig(sh), shr_c = contig(sh_rest);
     fdgs_forward_batch_args b;
     memset(&b, 0, sizeof(b));
     fdgs_forward_args& a = b.view;
-    a.P = P; a.D = degree; a.D_t = degree_t;
-    a.M = (sh.defined() && sh.numel() != 0) ? (int)sh.size(1) : 0;
-    if (shr_c.defined() && shr_c.numel() != 0) {
-        TORCH_CHECK(a.M == 1 && shr_c.dim() == 3 && shr_c.size(0) == P, "fdgs: split SH rows are [P,1,3] + [P,M-1,3]");
-        a.M += (int)shr_c.size(1);
-        a.shs_rest = fptr(shr_c);
-    }
-    a.raw_params = raw_params;
-    a.background = fptr(bg_c); a.width = W; a.height = H;
-    a.means3D = fptr(means_c); a.shs = fptr(sh_c); a.flows_precomp = fptr(flow_c);
-    a.opacities = fptr(op_c); a.ts = fptr(ts_c); a.scales = fptr(sc_c); a.scales_t = fptr(sct_c);
-    a.scale_modifier = scale_modifier; a.rotations = fptr(rot_c); a.rotations_r = fptr(rotr_c);
-    a.prefilter_var = prefilter_var;
+    Inputs in;
+    forward_gaussians(a, in, background, means3D, flows, opacity, ts, scales, scales_t, rotations, rotations_r, scale_modifier,
+                      prefilter_var, sh, sh_rest, degree, degree_t, time_duration, rot_4d, gaussian_dim, force_sh_3d,
+                      prefiltered, debug, raw_params, H, W);
     a.viewmatrix = cams.view; a.projmatrix = cams.proj; a.cam_pos = cams.campos;
-    a.time_duration = time_duration; a.rot_4d = rot_4d; a.gaussian_dim = gaussian_dim;
-    a.force_sh_3d = force_sh_3d; a.prefiltered = prefiltered; a.debug = debug;
     a.out_means3D = out_means3D.data_ptr<float>(); a.out_color = out_color.data_ptr<float>();
     a.out_flow = out_flow.data_ptr<float>(); a.out_depth = out_depth.data_ptr<float>();
     a.out_T = out_T.data_ptr<float>(); a.radii = radii.data_ptr<int>();
@@ -474,14 +494,14 @@ RasterizeGaussiansBackwardBatch(const torch::Tensor& background, const torch::Te
     const float* bgi = batch_bg_image(bg_image, means3D, B, H, W);
     const float* om = arg<float>(out_means3D, "out_means3D", B, 3ll * B * P, REQUIRED);
     const int* rad = arg<int>(radii, "radii", B, (int64_t)B * P, REQUIRED);
-    const auto gc_c = contig(dL_dout_color), gd_c = contig(dL_dout_depth), gm_c = contig(dL_dout_mask),
-               gf_c = contig(dL_dout_flow);
-    TORCH_CHECK(gd_c.numel() == 0 || gd_c.numel() == (int64_t)B * H * W, "fdgs: the depth gradient must be [B,1,H,W]");
-    TORCH_CHECK(gm_c.numel() == 0 || gm_c.numel() == (int64_t)B * H * W, "fdgs: the alpha gradient must be [B,1,H,W]");
-    TORCH_CHECK(gf_c.numel() == 0 || gf_c.numel() == 2ll * B * H * W, "fdgs: the flow gradient must be [B,2,H,W]");
+    TORCH_CHECK(!provided(dL_dout_depth) || dL_dout_depth.numel() == (int64_t)B * H * W,
+                "fdgs: the depth gradient must be [B,1,H,W]");
+    TORCH_CHECK(!provided(dL_dout_mask) || dL_dout_mask.numel() == (int64_t)B * H * W,
+                "fdgs: the alpha gradient must be [B,1,H,W]");
+    TORCH_CHECK(!provided(dL_dout_flow) || dL_dout_flow.numel() == 2ll * B * H * W, "fdgs: the flow gradient must be [B,2,H,W]");
     const DeviceStream on(means3D);
-    const bool split = sh_rest.defined() && sh_rest.numel() != 0;
-    const int M = ((sh.defined() && sh.numel() != 0) ? (int)sh.size(1) : 0) + (split ? (int)sh_rest.size(1) : 0);
+    const bool split = provided(sh_rest);
+    const int M = sh_coefficients(sh, sh_rest);
     auto opts = means3D.options().dtype(torch::kFloat32);
     torch::Tensor dL_dmeans2D = torch::zeros({B, P, 3}, opts);
     torch::Tensor dL_dopacity = torch::empty({P, 1}, opts), dL_dmeans3D = torch::empty({P, 3}, opts);
@@ -492,30 +512,19 @@ RasterizeGaussiansBackwardBatch(const torch::Tensor& background, const torch::Te
                   dL_drot_r = torch::empty({P, 4}, opts);
     torch::Tensor dL_dbg_image = want_dbg ? torch::empty({B, 3, H, W}, opts) : torch::empty({0}, opts);
     torch::Tensor scratch = torch::empty({(int64_t)fdgs_backward_batch_scratch_bytes(P, B)}, means3D.options().dtype(torch::kByte));
-    const auto bg_c = contig(background), flow_c = contig(flows), op_c = contig(opacities), ts_c = contig(ts),
-               sc_c = contig(scales), sct_c = contig(scales_t), rot_c = contig(rotations), rotr_c = contig(rotations_r),
-               sh_c = contig(sh), shr_c = contig(sh_rest), geo_c = contig(geomBuffer), bin_c = contig(binningBuffer),
-               img_c = contig(imageBuffer);
     fdgs_backward_batch_args b;
     memset(&b, 0, sizeof(b));
     fdgs_backward_args& a = b.view;
-    a.P = P; a.D = degree; a.D_t = degree_t; a.M = M; a.R = R;
-    a.background = fptr(bg_c); a.width = W; a.height = H;
-    a.out_means3D = om; a.shs = fptr(sh_c); a.flows_2d = fptr(flow_c);
-    a.opacities = fptr(op_c); a.ts = fptr(ts_c); a.scales = fptr(sc_c); a.scales_t = fptr(sct_c);
-    a.scale_modifier = scale_modifier; a.rotations = fptr(rot_c); a.rotations_r = fptr(rotr_c);
-    a.prefilter_var = prefilter_var;
+    Inputs in;
+    backward_gaussians(a, in, background, means3D, flows, opacities, ts, scales, scales_t, rotations, rotations_r,
+                       scale_modifier, prefilter_var, sh, sh_rest, degree, degree_t, time_duration, rot_4d, gaussian_dim,
+                       force_sh_3d, debug, raw_params, H, W, dL_dout_color, dL_dout_depth, dL_dout_mask, dL_dout_flow,
+                       geomBuffer, R, binningBuffer, imageBuffer);
+    a.out_means3D = om; a.radii = rad;
     a.viewmatrix = cams.view; a.projmatrix = cams.proj; a.campos = cams.campos;
-    a.time_duration = time_duration; a.rot_4d = rot_4d; a.gaussian_dim = gaussian_dim; a.force_sh_3d = force_sh_3d;
-    a.radii = rad;
-    a.geom_buffer = geo_c.numel() ? reinterpret_cast<const char*>(geo_c.data_ptr()) : nullptr;
-    a.binning_buffer = bin_c.numel() ? reinterpret_cast<const char*>(bin_c.data_ptr()) : nullptr;
-    a.image_buffer = img_c.numel() ? reinterpret_cast<const char*>(img_c.data_ptr()) : nullptr;
-    a.dL_dpix = fptr(gc_c); a.dL_depths = fptr(gd_c); a.dL_masks = fptr(gm_c); a.dL_dpix_flow = fptr(gf_c);
-    a.debug = debug; a.raw_params = raw_params;
     a.dL_dmean2D = dL_dmeans2D.data_ptr<float>(); a.dL_dopacity = dL_dopacity.data_ptr<float>();
     a.dL_dmean3D = dL_dmeans3D.data_ptr<float>(); a.dL_dsh = dL_dsh.data_ptr<float>();
-    a.shs_rest = split ? fptr(shr_c) : nullptr; a.dL_dsh_rest = split ? dL_dsh_rest.data_ptr<float>() : nullptr;
+    a.dL_dsh_rest = split ? dL_dsh_rest.data_ptr<float>() : nullptr;
     a.dL_dts = dL_dts.data_ptr<float>(); a.dL_dscale = dL_dscales.data_ptr<float>();
     a.dL_dscale_t = dL_dscales_t.data_ptr<float>(); a.dL_drot = dL_drot.data_ptr<float>(); a.dL_drot_r = dL_drot_r.data_ptr<float>();
     b.B = B; b.bg_image = bgi; b.bg_views = bgi ? B : 0;
