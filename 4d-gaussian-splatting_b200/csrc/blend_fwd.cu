@@ -15,6 +15,11 @@
 //     instances.  The cull box is the exact alpha >= 1/255 extent of the Gaussian, so skipped
 //     (pixel, Gaussian) pairs are pairs the reference would have rejected anyway;
 //   * pairs whose power is below log(1/(255*opacity)) skip expf() (same argument).
+//
+// In training (single view) the kernel also writes the zero rows of the dense SH gradient -- the rows of the Gaussians
+// the view does not render, about 2/3 of the 1.15 GB tensor at 2M Gaussians.  The blend is bound by instruction issue
+// and leaves DRAM nearly idle, so these rows go out as bulk (TMA) stores from a zeroed shared block, each CTA a stripe
+// of rows, issued before the CTA blends and drained when it retires; the SH backward then streams only rendered rows.
 #include "fdgs_internal.h"
 
 namespace fdgs {
@@ -24,13 +29,42 @@ constexpr int BF_THREADS = 256;
 constexpr int BF_WARPS = BF_THREADS / 32;
 constexpr int BF_BATCH = 128;
 constexpr int BF_STAGES = 3;
+constexpr int BF_ZERO_BYTES = 576;   // zero source of the bulk stores: one dL_dsh row of 48 coefficients
 
 struct __align__(128) BlendFwdSmem {
     StageRec recs[BF_STAGES][BF_BATCH];
+    float4 zero[BF_ZERO_BYTES / 16];
     uint64_t full[BF_STAGES];
     uint64_t empty[BF_STAGES];
     int done_warps;
 };
+
+// floats [0, n) at dst set to zero: the 16-byte-aligned interior as bulk stores from the zeroed shared block (row
+// sizes and offsets of split rows are not multiples of 16 bytes), the few floats around it as plain stores
+__device__ __forceinline__ void zero_row(float* dst, int n, const float4* zsrc) {
+    float* end = dst + n;
+    float* a = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(dst) + 15) & ~uintptr_t(15));
+    float* b = reinterpret_cast<float*>(reinterpret_cast<uintptr_t>(end) & ~uintptr_t(15));
+    if (a >= b) a = b = end;
+    for (float* q = dst; q < a; ++q) *q = 0.f;
+    for (float* q = b; q < end; ++q) *q = 0.f;
+    for (char* q = reinterpret_cast<char*>(a); q < reinterpret_cast<char*>(b); q += BF_ZERO_BYTES)
+        bulk_s2g(q, zsrc, (uint32_t)min(BF_ZERO_BYTES, (int)(reinterpret_cast<char*>(b) - q)));
+}
+
+// this CTA's stripe of SH gradient rows: every row of a Gaussian the view does not render (sh_bwd_kernel's test)
+__device__ __forceinline__ void zero_unrendered_rows(const BlendFwdParams& p, int tile, const float4* zsrc) {
+    const long long r0 = (long long)tile * p.zero_stripe;
+    const long long r1 = min((long long)p.P, r0 + p.zero_stripe);
+    bool issued = false;
+    for (long long g = r0 + threadIdx.x; g < r1; g += BF_THREADS) {
+        if (p.radii[g] > 0 && p.tiles_touched[g] != 0u) continue;
+        zero_row(p.zero_rows[0] + g * p.zero_row_floats[0], p.zero_row_floats[0], zsrc);
+        if (p.zero_rows[1]) zero_row(p.zero_rows[1] + g * p.zero_row_floats[1], p.zero_row_floats[1], zsrc);
+        issued = true;
+    }
+    if (issued) bulk_commit();
+}
 
 // view v of a batch (blockIdx.z): the same kernel on the view's slices of ranges and of every image
 __device__ __forceinline__ BlendFwdParams blend_fwd_view(BlendFwdParams p, int v) {
@@ -67,6 +101,7 @@ __device__ __forceinline__ void blend_fwd_body(const BlendFwdParams& p_) {
     const int n = (int)(range.y - range.x);
     const int nb = (n + BF_BATCH - 1) / BF_BATCH;
     const StageRec* src = p.recs + range.x;
+    const bool zero_rows = !BATCH && p.zero_rows[0] != nullptr;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < BF_STAGES; ++s) {
@@ -75,6 +110,10 @@ __device__ __forceinline__ void blend_fwd_body(const BlendFwdParams& p_) {
         }
         sm.done_warps = 0;
         mbar_fence_init();
+    }
+    if (zero_rows && threadIdx.x < BF_ZERO_BYTES / 16) {
+        sm.zero[threadIdx.x] = make_float4(0.f, 0.f, 0.f, 0.f);
+        fence_async_smem();
     }
     __syncthreads();
 
@@ -86,6 +125,7 @@ __device__ __forceinline__ void blend_fwd_body(const BlendFwdParams& p_) {
             bulk_g2s(&sm.recs[issued][0], src + (size_t)issued * BF_BATCH, (uint32_t)cnt * kStageRecBytes, &sm.full[issued]);
         }
     }
+    if (zero_rows) zero_unrendered_rows(p, tile, sm.zero);
 
     float T = 1.0f;
     float C0 = 0.f, C1 = 0.f, C2 = 0.f, F0 = 0.f, F1 = 0.f, Dp = 0.f;
@@ -203,6 +243,8 @@ __device__ __forceinline__ void blend_fwd_body(const BlendFwdParams& p_) {
         p.out_flow[1 * HW + pix_id] = F1;
         p.out_depth[pix_id] = Dp;
     }
+    // the zero block must outlive the bulk stores that read it
+    if (zero_rows) bulk_wait_all();
 }
 
 __global__ void __launch_bounds__(BF_THREADS) blend_fwd_kernel(const BlendFwdParams p_) {
@@ -217,6 +259,8 @@ __global__ void __launch_bounds__(BF_THREADS) blend_fwd_batch_kernel(const Blend
 }  // namespace
 
 cudaError_t launch_blend_fwd(const BlendFwdParams& p, cudaStream_t stream) {
+    if (p.zero_rows[0] != nullptr && (p.views > 0 || p.zero_stripe <= 0 || !p.radii || !p.tiles_touched))
+        return cudaErrorInvalidValue;
     if (p.views > 0) blend_fwd_batch_kernel<<<dim3(p.grid_x, p.grid_y, p.views), BF_THREADS, 0, stream>>>(p);
     else blend_fwd_kernel<<<dim3(p.grid_x, p.grid_y, 1), BF_THREADS, 0, stream>>>(p);
     return cudaGetLastError();

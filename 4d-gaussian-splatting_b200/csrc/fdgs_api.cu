@@ -307,9 +307,10 @@ int check_forward_args(const fdgs_forward_args* a) {
 // The forward's stages on the carved geometry and image buffers, for one view (vb = {1, NULL}) or for the batched
 // entry's B views (vb = {B, the uploaded view table}: every per-view array is then a [B] stack, and the camera tables and
 // scalars are the views').  Allocates the binning buffer after the one host synchronisation.
-int forward_stages(const fdgs_forward_args* a, const float* bg_image, const fdgs::ViewBatch& vb, const GeomState& geom,
-                   const ImageState& img, fdgs_alloc_fn binning_alloc, void* binning_ctx, cudaStream_t stream,
-                   fdgs_forward_result* res) {
+// zero_sh / zero_sh_rest (single view): the SH gradient rows the blend zeroes (fdgs_forward_zero_sh), or NULL.
+int forward_stages(const fdgs_forward_args* a, const float* bg_image, float* zero_sh, float* zero_sh_rest,
+                   const fdgs::ViewBatch& vb, const GeomState& geom, const ImageState& img, fdgs_alloc_fn binning_alloc,
+                   void* binning_ctx, cudaStream_t stream, fdgs_forward_result* res) {
     const bool debug = a->debug != 0, batch = vb.scalars != nullptr;
     const int P = a->P, W = a->width, H = a->height;
     const int grid_x = (W + fdgs::TILE_X - 1) / fdgs::TILE_X, grid_y = (H + fdgs::TILE_Y - 1) / fdgs::TILE_Y;
@@ -382,18 +383,34 @@ int forward_stages(const fdgs_forward_args* a, const float* bg_image, const fdgs
     bp.out_color = a->out_color; bp.out_flow = a->out_flow; bp.out_depth = a->out_depth; bp.out_T = a->out_T;
     bp.bg_image = bg_image;
     bp.views = batch ? vb.B : 0;
+    bp.zero_rows[0] = bp.zero_rows[1] = nullptr;
+    bp.zero_row_floats[0] = bp.zero_row_floats[1] = 0;
+    bp.zero_stripe = 0; bp.P = P; bp.radii = a->radii; bp.tiles_touched = geom.tiles_touched;
+    if (zero_sh && P > 0) {
+        const bool split = zero_sh_rest != nullptr;
+        bp.zero_rows[0] = zero_sh; bp.zero_row_floats[0] = split ? 3 : 3 * a->M;
+        bp.zero_rows[1] = zero_sh_rest; bp.zero_row_floats[1] = split ? 3 * (a->M - 1) : 0;
+        const long long tiles = (long long)grid_x * grid_y;
+        bp.zero_stripe = (int)((P + tiles - 1) / tiles);
+    }
     FDGS_STAGE(5, 1, fdgs::launch_blend_fwd(bp, stream), batch ? "blend_fwd (batch)" : "blend_fwd");
     return FDGS_OK;
 }
 
-int forward_impl(const fdgs_forward_args* a, const float* bg_image, fdgs_alloc_fn geom_alloc, void* geom_ctx,
-                 fdgs_alloc_fn binning_alloc, void* binning_ctx, fdgs_alloc_fn image_alloc, void* image_ctx, void* stream_v,
-                 fdgs_forward_result* res) {
+int forward_impl(const fdgs_forward_args* a, const float* bg_image, float* zero_sh, float* zero_sh_rest,
+                 fdgs_alloc_fn geom_alloc, void* geom_ctx, fdgs_alloc_fn binning_alloc, void* binning_ctx,
+                 fdgs_alloc_fn image_alloc, void* image_ctx, void* stream_v, fdgs_forward_result* res) {
     g_last_error.clear();
     if (!a || !res || !geom_alloc || !binning_alloc || !image_alloc) return fail(FDGS_ERR_INVALID_ARG, "null argument");
     memset(res, 0, sizeof(*res));
     const int P = a->P, W = a->width, H = a->height;
     if (int rc = check_forward_args(a)) return rc;
+    if (zero_sh_rest && !zero_sh) return fail(FDGS_ERR_INVALID_ARG, "dL_dsh_rest without dL_dsh");
+    if (zero_sh && P > 0) {
+        if (!a->shs || a->colors_precomp || a->M <= 0) return fail(FDGS_ERR_INVALID_ARG, "dL_dsh rows need shs, not colors_precomp");
+        if (a->shs_rest && !zero_sh_rest) return fail(FDGS_ERR_INVALID_ARG, "split SH rows need dL_dsh_rest");
+        if (!a->shs_rest && zero_sh_rest) return fail(FDGS_ERR_INVALID_ARG, "dL_dsh_rest without shs_rest");
+    }
 
     // scratch: geometry + image
     const size_t geom_bytes = fdgs_geom_bytes(P);
@@ -409,15 +426,16 @@ int forward_impl(const fdgs_forward_args* a, const float* bg_image, fdgs_alloc_f
     res->image_buffer = img_raw;
     res->image_bytes = img_bytes;
     res->cov3D = geom.cov3D;
-    return forward_stages(a, bg_image, {1, nullptr}, geom, img, binning_alloc, binning_ctx,
+    return forward_stages(a, bg_image, zero_sh, zero_sh_rest, {1, nullptr}, geom, img, binning_alloc, binning_ctx,
                           reinterpret_cast<cudaStream_t>(stream_v), res);
 }
 
 // The backward's stages on the forward's buffers: the blend backward (when there is an instance or dL_dbg_image to
 // write), then the per-Gaussian backward (when there is a Gaussian).  vb as in forward_stages; for a batch, a's
-// gradient outputs are the per-view stacks of BatchBwdScratch.  The arguments have been checked by the entry.
-int backward_stages(const fdgs_backward_args* a, const float* bg_image, float* dL_dbg_image, const fdgs::ViewBatch& vb,
-                    const GeomState& geom, const ImageState& img, cudaStream_t stream) {
+// gradient outputs are the per-view stacks of BatchBwdScratch.  sh_rows_zeroed: the forward zeroed the non-rendered
+// dL_dsh rows (fdgs_backward_zero_sh).  The arguments have been checked by the entry.
+int backward_stages(const fdgs_backward_args* a, const float* bg_image, float* dL_dbg_image, int sh_rows_zeroed,
+                    const fdgs::ViewBatch& vb, const GeomState& geom, const ImageState& img, cudaStream_t stream) {
     const bool debug = a->debug != 0, batch = vb.scalars != nullptr;
     const int P = a->P, W = a->width, H = a->height, R = a->R;
     BinningState bin = BinningState::carve(a->binning_buffer ? align128(const_cast<char*>(a->binning_buffer)) : nullptr, R);
@@ -462,6 +480,7 @@ int backward_stages(const fdgs_backward_args* a, const float* bg_image, float* d
     pb.shs_rest = a->shs ? a->shs_rest : nullptr; pb.dL_dsh_rest = a->dL_dsh_rest;
     pb.dL_dmean2D = a->dL_dmean2D; pb.dL_dconic = a->dL_dconic; pb.dL_dopacity = a->dL_dopacity; pb.dL_dcolor = a->dL_dcolor;
     pb.dL_dmean3D = a->dL_dmean3D; pb.dL_dcov3D = a->dL_dcov3D; pb.dL_dsh = a->dL_dsh; pb.sh_factors = a->sh_factors;
+    pb.sh_rows_zeroed = (sh_rows_zeroed && a->dL_dsh && !batch) ? 1 : 0;
     pb.dL_dts = a->dL_dts;
     pb.dL_dscale = a->dL_dscale; pb.dL_dscale_t = a->dL_dscale_t; pb.dL_drot = a->dL_drot; pb.dL_drot_r = a->dL_drot_r;
     pb.vb = vb; pb.factor_stride = BatchBwdScratch::factor_stride(P);
@@ -470,7 +489,8 @@ int backward_stages(const fdgs_backward_args* a, const float* bg_image, float* d
     return FDGS_OK;
 }
 
-int backward_impl(const fdgs_backward_args* a, const float* bg_image, float* dL_dbg_image, void* stream_v) {
+int backward_impl(const fdgs_backward_args* a, const float* bg_image, float* dL_dbg_image, int sh_rows_zeroed,
+                  void* stream_v) {
     g_last_error.clear();
     if (!a) return fail(FDGS_ERR_INVALID_ARG, "null argument");
     const int P = a->P, W = a->width, H = a->height, R = a->R;
@@ -498,7 +518,8 @@ int backward_impl(const fdgs_backward_args* a, const float* bg_image, float* dL_
     }
     GeomState geom = GeomState::carve(align128(const_cast<char*>(a->geom_buffer)), P);
     ImageState img = ImageState::carve(align128(const_cast<char*>(a->image_buffer)), W, H);
-    return backward_stages(a, bg_image, dL_dbg_image, {1, nullptr}, geom, img, reinterpret_cast<cudaStream_t>(stream_v));
+    return backward_stages(a, bg_image, dL_dbg_image, sh_rows_zeroed, {1, nullptr}, geom, img,
+                           reinterpret_cast<cudaStream_t>(stream_v));
 }
 
 // ---- batched views: B cameras of the same Gaussians in one pass per stage (include/fdgs.h: fdgs_forward_batch) -------
@@ -556,7 +577,8 @@ int forward_batch_impl(const fdgs_forward_batch_args* b, fdgs_alloc_fn geom_allo
         vs[v].focal_x = W / (2.0f * b->tan_fovx[v]);
     }
     FDGS_CUDA(cudaMemcpyAsync(geom.scalars, vs.data(), vs.size() * sizeof(vs[0]), cudaMemcpyHostToDevice, stream), "view table copy");
-    return forward_stages(a, b->bg_image, {B, geom.scalars}, geom, img, binning_alloc, binning_ctx, stream, res);
+    return forward_stages(a, b->bg_image, nullptr, nullptr, {B, geom.scalars}, geom, img, binning_alloc, binning_ctx, stream,
+                          res);
 }
 
 int backward_batch_impl(const fdgs_backward_batch_args* b, void* stream_v) {
@@ -577,7 +599,7 @@ int backward_batch_impl(const fdgs_backward_batch_args* b, void* stream_v) {
     GeomState geom = GeomState::carve(align128(const_cast<char*>(a->geom_buffer)), P, true, B);
     ImageState img = ImageState::carve(align128(const_cast<char*>(a->image_buffer)), W, H, B);
     const fdgs::ViewBatch vb = {B, geom.scalars};
-    if (P == 0) return backward_stages(a, b->bg_image, b->dL_dbg_image, vb, geom, img, stream);
+    if (P == 0) return backward_stages(a, b->bg_image, b->dL_dbg_image, 0, vb, geom, img, stream);
     if (R > 0 && !a->binning_buffer) return fail(FDGS_ERR_INVALID_ARG, "scratch buffers of the forward pass required");
     if (!a->radii || !a->out_means3D || !a->viewmatrix || !a->projmatrix || !a->campos)
         return fail(FDGS_ERR_INVALID_ARG, "radii / out_means3D / viewmatrix / projmatrix / campos required");
@@ -601,7 +623,7 @@ int backward_batch_impl(const fdgs_backward_batch_args* b, void* stream_v) {
     views.dL_dsh = nullptr; views.sh_factors = sc.table; views.dL_dsh_rest = nullptr; views.dL_dts = sc.dL_dts;
     views.dL_dscale = sc.dL_dscale; views.dL_dscale_t = sc.dL_dscale_t; views.dL_drot = sc.dL_drot;
     views.dL_drot_r = sc.dL_drot_r;
-    if (int rc = backward_stages(&views, b->bg_image, b->dL_dbg_image, vb, geom, img, stream)) return rc;
+    if (int rc = backward_stages(&views, b->bg_image, b->dL_dbg_image, 0, vb, geom, img, stream)) return rc;
 
     // every per-Gaussian gradient but the SH rows: summed over the views in view order
     fdgs::ViewSumParams vsum;
@@ -657,19 +679,33 @@ extern "C" {
 
 int fdgs_forward(const fdgs_forward_args* a, fdgs_alloc_fn geom_alloc, void* geom_ctx, fdgs_alloc_fn binning_alloc,
                  void* binning_ctx, fdgs_alloc_fn image_alloc, void* image_ctx, void* stream, fdgs_forward_result* res) {
-    return forward_impl(a, nullptr, geom_alloc, geom_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, stream, res);
+    return forward_impl(a, nullptr, nullptr, nullptr, geom_alloc, geom_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx,
+                        stream, res);
 }
 
 int fdgs_forward_bg(const fdgs_forward_args* a, const float* bg_image, fdgs_alloc_fn geom_alloc, void* geom_ctx,
                     fdgs_alloc_fn binning_alloc, void* binning_ctx, fdgs_alloc_fn image_alloc, void* image_ctx, void* stream,
                     fdgs_forward_result* res) {
-    return forward_impl(a, bg_image, geom_alloc, geom_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, stream, res);
+    return forward_impl(a, bg_image, nullptr, nullptr, geom_alloc, geom_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx,
+                        stream, res);
 }
 
-int fdgs_backward(const fdgs_backward_args* a, void* stream) { return backward_impl(a, nullptr, nullptr, stream); }
+int fdgs_forward_zero_sh(const fdgs_forward_args* a, const float* bg_image, float* dL_dsh, float* dL_dsh_rest,
+                         fdgs_alloc_fn geom_alloc, void* geom_ctx, fdgs_alloc_fn binning_alloc, void* binning_ctx,
+                         fdgs_alloc_fn image_alloc, void* image_ctx, void* stream, fdgs_forward_result* res) {
+    return forward_impl(a, bg_image, dL_dsh, dL_dsh_rest, geom_alloc, geom_ctx, binning_alloc, binning_ctx, image_alloc,
+                        image_ctx, stream, res);
+}
+
+int fdgs_backward(const fdgs_backward_args* a, void* stream) { return backward_impl(a, nullptr, nullptr, 0, stream); }
 
 int fdgs_backward_bg(const fdgs_backward_args* a, const float* bg_image, float* dL_dbg_image, void* stream) {
-    return backward_impl(a, bg_image, dL_dbg_image, stream);
+    return backward_impl(a, bg_image, dL_dbg_image, 0, stream);
+}
+
+int fdgs_backward_zero_sh(const fdgs_backward_args* a, const float* bg_image, float* dL_dbg_image, int sh_rows_zeroed,
+                          void* stream) {
+    return backward_impl(a, bg_image, dL_dbg_image, sh_rows_zeroed, stream);
 }
 
 int fdgs_forward_batch(const fdgs_forward_batch_args* args, fdgs_alloc_fn geom_alloc, void* geom_ctx,

@@ -128,6 +128,16 @@ struct BlendFwdParams {
     float* out_T;          // [H,W]
     const float* bg_image; // [3,H,W] per-pixel background behind the Gaussians, or NULL
     int views;             // > 0: batched entry, blockIdx.z = view; ranges and every image are [views] stacks
+    // single view only: the SH gradient's rows of the Gaussians the view does not render (radii == 0 or no tile, the
+    // test of sh_bwd_kernel), zeroed here so that the backward writes only the rendered rows.  zero_rows[0] is
+    // [P, zero_row_floats[0]] (dL_dsh, or dL_dsh [P,1,3] of split rows), zero_rows[1] NULL or [P, zero_row_floats[1]]
+    // (dL_dsh_rest).  Each CTA owns a stripe of zero_stripe consecutive rows.
+    float* zero_rows[2];
+    int zero_row_floats[2];
+    int zero_stripe;
+    int P;
+    const int* radii;
+    const uint32_t* tiles_touched;
 };
 cudaError_t launch_blend_fwd(const BlendFwdParams& p, cudaStream_t stream);
 
@@ -199,6 +209,7 @@ struct PreprocessBwdParams {
     float* dL_dcov3D;
     float* dL_dsh;          // [P,M,3], or NULL when sh_factors is set
     float* sh_factors;      // [P,3] clamp-masked colour gradient (view-parallel mode) instead of the dL_dsh rows
+    int sh_rows_zeroed;     // the forward's blend zeroed the non-rendered dL_dsh (| dL_dsh_rest) rows: write rendered rows only
     float* dL_dts;
     float* dL_dscale;
     float* dL_dscale_t;

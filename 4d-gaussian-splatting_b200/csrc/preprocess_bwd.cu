@@ -7,7 +7,9 @@
 //
 //   sh_bwd_kernel    HBM-bound.  Reads the 12*M-byte SH row of every rendered Gaussian and writes
 //                    the 12*M-byte dL_dsh row of EVERY Gaussian (zeros where not rendered, so the
-//                    host never memsets the 1.15 GB tensor; reference: rasterize_points.cu:209).
+//                    host never memsets the 1.15 GB tensor; reference: rasterize_points.cu:209) --
+//                    or, when the forward's blend already zeroed the non-rendered rows
+//                    (sh_rows_zeroed, blend_fwd.cu), the rendered rows only.
 //                    Rows move with cp.async.bulk in both directions (global->shared on an
 //                    mbarrier, shared->global as a bulk group); in shared memory a row is read and
 //                    overwritten in place with conflict-free 128-bit accesses; only rendered rows
@@ -292,13 +294,15 @@ __device__ __forceinline__ void sh_bwd_body(const PreprocessBwdParams& a_) {
         meta[2] = a.campos[1];
         meta[3] = a.campos[2];
     }
-    // zero rows: every float4 of every non-rendered row of this CTA, coalesced
+    // zero rows: every float4 of every non-rendered row of this CTA, coalesced (unless the forward's blend wrote them)
     if (FACTORS) {
         if (in_range && !vis) {
             a.sh_factors[3 * idx + 0] = 0.f;
             a.sh_factors[3 * idx + 1] = 0.f;
             a.sh_factors[3 * idx + 2] = 0.f;
         }
+    } else if (a.sh_rows_zeroed) {
+        // the non-rendered rows are already zero (blend_fwd.cu)
     } else if (a.dL_dsh_rest != nullptr) {
         // split gradient tensors: [P,1,3] and [P,M-1,3]; a warp per non-rendered row
         const int rows_here = min(SB_THREADS, a.P - blockIdx.x * SB_THREADS);

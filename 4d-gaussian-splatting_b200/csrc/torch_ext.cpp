@@ -12,9 +12,9 @@
 //
 // and one extended entry per direction, which the autograd Function of this package calls:
 //
-//   rasterize_gaussians_ext(30 args, sh_rest, raw_params, bg_image)  -> the same 11-tuple
-//   rasterize_gaussians_backward_ext(37 args, sh_rest, raw_params, bg_image, sh_factor_mode, want_dbg)
-//                                         -> [12 gradients, sh_factors, dL_dsh_rest, dL_dbg_image]
+//   rasterize_gaussians_ext(30 args, sh_rest, raw_params, bg_image[, dL_dsh, dL_dsh_rest])  -> the same 11-tuple
+//   rasterize_gaussians_backward_ext(37 args, sh_rest, raw_params, bg_image, sh_factor_mode, want_dbg[, dL_dsh,
+//                                    dL_dsh_rest])  -> [12 gradients, sh_factors, dL_dsh_rest, dL_dbg_image]
 //
 // and a batched pair over B cameras of the same Gaussians (include/fdgs.h: fdgs_forward_batch):
 //
@@ -142,6 +142,16 @@ torch::Tensor background_image(const torch::Tensor& bg_image, const torch::Tenso
     return bg_image.contiguous();
 }
 
+// an SH gradient tensor handed in by the caller to be written in place: float32, contiguous, [P,m,3], on the device of
+// means3D (undefined / empty = none)
+float* sh_grad_rows(const torch::Tensor& t, const char* name, const torch::Tensor& like, int64_t P, int64_t m) {
+    if (!provided(t)) return nullptr;
+    TORCH_CHECK(t.is_cuda() && t.device() == like.device(), "fdgs: ", name, " must be on the device of means3D");
+    TORCH_CHECK(t.scalar_type() == torch::kFloat32 && t.is_contiguous(), "fdgs: ", name, " must be contiguous float32");
+    TORCH_CHECK(t.dim() == 3 && t.size(0) == P && t.size(1) == m && t.size(2) == 3, "fdgs: ", name, " has the wrong shape");
+    return t.data_ptr<float>();
+}
+
 // ---- the training-step bindings' strict contract: no copies, so a tensor of the wrong dtype, layout or shape is an
 // error.  dtype, layout and shape of every argument are checked first (arg), then the device (same_cuda_device), and
 // only then is anything allocated or launched: a malformed call fails before any GPU work. ---------------------------
@@ -188,7 +198,9 @@ using ForwardOut = std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, 
 // unused: sh_rest and raw_params, the raw-parameter entry (fdgs_forward_args.raw_params: scales = log-scales, rotations
 // un-normalised, opacity = logits; sh = features_dc [P,1,3], sh_rest = features_rest [P,M-1,3]), and bg_image, a
 // per-pixel background [3,H,W] (fdgs_forward_bg).  Returns the reference's 11-tuple.
-ForwardOut RasterizeGaussiansExt(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors,
+// dL_dsh / dL_dsh_rest: the SH gradient tensors the backward will return (shaped as it returns them); the forward then
+// zeroes the rows of the Gaussians it does not render (fdgs_forward_zero_sh).  Empty: not provided.
+ForwardOut RasterizeGaussiansExtZeroSh(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors,
                                  const torch::Tensor& flows, const torch::Tensor& opacity, const torch::Tensor& ts,
                                  const torch::Tensor& scales, const torch::Tensor& scales_t, const torch::Tensor& rotations,
                                  const torch::Tensor& rotations_r, const float scale_modifier,
@@ -198,7 +210,8 @@ ForwardOut RasterizeGaussiansExt(const torch::Tensor& background, const torch::T
                                  const torch::Tensor& sh, const int degree, const int degree_t, const torch::Tensor& campos,
                                  const float timestamp, const float time_duration, const bool rot_4d,
                                  const int gaussian_dim, const bool force_sh_3d, const bool prefiltered, const bool debug,
-                                 const torch::Tensor& sh_rest, const bool raw_params, const torch::Tensor& bg_image) {
+                                 const torch::Tensor& sh_rest, const bool raw_params, const torch::Tensor& bg_image,
+                                 const torch::Tensor& dL_dsh, const torch::Tensor& dL_dsh_rest) {
     if (means3D.ndimension() != 2 || means3D.size(1) != 3) {
         AT_ERROR("means3D must have dimensions (num_points, 3)");   // reference: rasterize_points.cu:69-71
     }
@@ -235,9 +248,11 @@ ForwardOut RasterizeGaussiansExt(const torch::Tensor& background, const torch::T
     a.out_T = out_T.data_ptr<float>(); a.radii = radii.data_ptr<int>();
 
     const auto bgi_c = background_image(bg_image, means3D, H, W);
+    float* zero_sh = sh_grad_rows(dL_dsh, "dL_dsh", means3D, P, provided(sh_rest) ? 1 : a.M);
+    float* zero_sh_rest = sh_grad_rows(dL_dsh_rest, "dL_dsh_rest", means3D, P, a.M - 1);
     fdgs_forward_result r;
-    check(fdgs_forward_bg(&a, fptr(bgi_c), resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer,
-                          (void*)on.stream, &r),
+    check(fdgs_forward_zero_sh(&a, fptr(bgi_c), zero_sh, zero_sh_rest, resize_cb, &geomBuffer, resize_cb, &binningBuffer,
+                               resize_cb, &imgBuffer, (void*)on.stream, &r),
           "forward");
 
     torch::Tensor covs3D_com;
@@ -249,6 +264,24 @@ ForwardOut RasterizeGaussiansExt(const torch::Tensor& background, const torch::T
     }
     return std::make_tuple(r.num_rendered, out_color, out_flow, out_depth, out_T, radii, geomBuffer, binningBuffer,
                            imgBuffer, covs3D_com, out_means3D);
+}
+
+ForwardOut RasterizeGaussiansExt(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& colors,
+                                 const torch::Tensor& flows, const torch::Tensor& opacity, const torch::Tensor& ts,
+                                 const torch::Tensor& scales, const torch::Tensor& scales_t, const torch::Tensor& rotations,
+                                 const torch::Tensor& rotations_r, const float scale_modifier,
+                                 const torch::Tensor& cov3D_precomp, const float prefilter_var,
+                                 const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx,
+                                 const float tan_fovy, const int image_height, const int image_width,
+                                 const torch::Tensor& sh, const int degree, const int degree_t, const torch::Tensor& campos,
+                                 const float timestamp, const float time_duration, const bool rot_4d,
+                                 const int gaussian_dim, const bool force_sh_3d, const bool prefiltered, const bool debug,
+                                 const torch::Tensor& sh_rest, const bool raw_params, const torch::Tensor& bg_image) {
+    return RasterizeGaussiansExtZeroSh(background, means3D, colors, flows, opacity, ts, scales, scales_t, rotations,
+                                       rotations_r, scale_modifier, cov3D_precomp, prefilter_var, viewmatrix, projmatrix,
+                                       tan_fovx, tan_fovy, image_height, image_width, sh, degree, degree_t, campos, timestamp,
+                                       time_duration, rot_4d, gaussian_dim, force_sh_3d, prefiltered, debug, sh_rest,
+                                       raw_params, bg_image, torch::Tensor(), torch::Tensor());
 }
 
 // the reference's entry point: 30 positional arguments, 11-tuple (rasterize_points.h:18-49)
@@ -271,10 +304,12 @@ ForwardOut RasterizeGaussiansCUDA(const torch::Tensor& background, const torch::
 // The reference's 37 arguments (rasterize_points.h:51-89) + the forward's sh_rest, raw_params and bg_image, and:
 //   sh_factor_mode: the view-parallel mode -- no dL_dsh rows, the [P,3] colour factors instead (include/fdgs.h: sh_factors)
 //   want_dbg:       whether dL/dbg_image is wanted (fdgs_backward_bg)
+//   sh_grad / sh_rest_grad: the tensors the forward zeroed (rasterize_gaussians_ext's dL_dsh / dL_dsh_rest), returned
+//                   as the SH gradient with their rendered rows written (fdgs_backward_zero_sh); empty: allocated here
 // Returns 15 tensors: the 12 gradients (w.r.t. the raw parameters under raw_params; dL_dsh is [P,1,3] when sh_rest is
 // given), sh_factors [P,3], dL_dsh_rest [P,M-1,3] and dL_dbg_image [3,H,W]; a tensor not asked for comes back empty.
 std::vector<torch::Tensor>
-RasterizeGaussiansBackwardExt(const torch::Tensor& background, const torch::Tensor& means3D,
+RasterizeGaussiansBackwardExtZeroSh(const torch::Tensor& background, const torch::Tensor& means3D,
                               const torch::Tensor& out_means3D, const torch::Tensor& radii, const torch::Tensor& colors,
                               const torch::Tensor& flows_2d, const torch::Tensor& opacities, const torch::Tensor& ts,
                               const torch::Tensor& scales, const torch::Tensor& scales_t, const torch::Tensor& rotations,
@@ -288,7 +323,8 @@ RasterizeGaussiansBackwardExt(const torch::Tensor& background, const torch::Tens
                               const bool force_sh_3d, const torch::Tensor& geomBuffer, const int R,
                               const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer, const bool debug,
                               const torch::Tensor& sh_rest, const bool raw_params, const torch::Tensor& bg_image,
-                              const bool sh_factor_mode, const bool want_dbg) {
+                              const bool sh_factor_mode, const bool want_dbg, const torch::Tensor& sh_grad,
+                              const torch::Tensor& sh_rest_grad) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor");
     const DeviceStream on(means3D);
     const int P = means3D.size(0);
@@ -309,8 +345,15 @@ RasterizeGaussiansBackwardExt(const torch::Tensor& background, const torch::Tens
     torch::Tensor dL_dts = torch::empty({P, 1}, opts);
     torch::Tensor dL_dcov3D = torch::empty({P, 6}, opts);
     const bool factors = sh_factor_mode && M > 0;
-    torch::Tensor dL_dsh = factors ? torch::empty({0}, opts) : torch::empty({P, split ? 1 : M, 3}, opts);
-    torch::Tensor dL_dsh_rest = (split && !factors) ? torch::empty({P, M - 1, 3}, opts) : torch::empty({0}, opts);
+    const bool zeroed = !factors && provided(sh_grad);
+    if (zeroed) {
+        sh_grad_rows(sh_grad, "dL_dsh", means3D, P, split ? 1 : M);
+        TORCH_CHECK(split == provided(sh_rest_grad), "fdgs: split SH rows need both zeroed gradient tensors");
+        if (split) sh_grad_rows(sh_rest_grad, "dL_dsh_rest", means3D, P, M - 1);
+    }
+    torch::Tensor dL_dsh = factors ? torch::empty({0}, opts) : zeroed ? sh_grad : torch::empty({P, split ? 1 : M, 3}, opts);
+    torch::Tensor dL_dsh_rest = (split && !factors) ? (zeroed ? sh_rest_grad : torch::empty({P, M - 1, 3}, opts))
+                                                    : torch::empty({0}, opts);
     torch::Tensor sh_factors = factors ? torch::empty({P, 3}, opts) : torch::empty({0}, opts);
     torch::Tensor dL_dscales = torch::empty({P, 3}, opts);
     torch::Tensor dL_dscales_t = torch::empty({P, 1}, opts);
@@ -342,11 +385,36 @@ RasterizeGaussiansBackwardExt(const torch::Tensor& background, const torch::Tens
         a.dL_dts = dL_dts.data_ptr<float>(); a.dL_dscale = dL_dscales.data_ptr<float>();
         a.dL_dscale_t = dL_dscales_t.data_ptr<float>(); a.dL_drot = dL_drotations.data_ptr<float>();
         a.dL_drot_r = dL_drotations_r.data_ptr<float>();
-        check(fdgs_backward_bg(&a, fptr(bgi_c), want_dbg ? dL_dbg_image.data_ptr<float>() : nullptr, (void*)on.stream),
+        check(fdgs_backward_zero_sh(&a, fptr(bgi_c), want_dbg ? dL_dbg_image.data_ptr<float>() : nullptr, zeroed ? 1 : 0,
+                                    (void*)on.stream),
               "backward");
     }
     return {dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dflows, dL_dts, dL_dscales,
             dL_dscales_t, dL_drotations, dL_drotations_r, sh_factors, dL_dsh_rest, dL_dbg_image};
+}
+
+std::vector<torch::Tensor>
+RasterizeGaussiansBackwardExt(const torch::Tensor& background, const torch::Tensor& means3D,
+                              const torch::Tensor& out_means3D, const torch::Tensor& radii, const torch::Tensor& colors,
+                              const torch::Tensor& flows_2d, const torch::Tensor& opacities, const torch::Tensor& ts,
+                              const torch::Tensor& scales, const torch::Tensor& scales_t, const torch::Tensor& rotations,
+                              const torch::Tensor& rotations_r, const float scale_modifier,
+                              const torch::Tensor& cov3D_precomp, const float prefilter_var,
+                              const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx,
+                              const float tan_fovy, const torch::Tensor& dL_dout_color, const torch::Tensor& dL_dout_depth,
+                              const torch::Tensor& dL_dout_mask, const torch::Tensor& dL_dout_flow, const torch::Tensor& sh,
+                              const int degree, const int degree_t, const torch::Tensor& campos, const float timestamp,
+                              const float time_duration, const bool rot_4d, const int gaussian_dim,
+                              const bool force_sh_3d, const torch::Tensor& geomBuffer, const int R,
+                              const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer, const bool debug,
+                              const torch::Tensor& sh_rest, const bool raw_params, const torch::Tensor& bg_image,
+                              const bool sh_factor_mode, const bool want_dbg) {
+    return RasterizeGaussiansBackwardExtZeroSh(
+        background, means3D, out_means3D, radii, colors, flows_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
+        scale_modifier, cov3D_precomp, prefilter_var, viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color,
+        dL_dout_depth, dL_dout_mask, dL_dout_flow, sh, degree, degree_t, campos, timestamp, time_duration, rot_4d,
+        gaussian_dim, force_sh_3d, geomBuffer, R, binningBuffer, imageBuffer, debug, sh_rest, raw_params, bg_image,
+        sh_factor_mode, want_dbg, torch::Tensor(), torch::Tensor());
 }
 
 // the reference's entry point: 37 positional arguments, 12 gradients (rasterize_points.h:51-89)
@@ -1128,7 +1196,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("rasterize_gaussians", &RasterizeGaussiansCUDA);
     m.def("rasterize_gaussians_backward", &RasterizeGaussiansBackwardCUDA);
     m.def("rasterize_gaussians_ext", &RasterizeGaussiansExt);
+    m.def("rasterize_gaussians_ext", &RasterizeGaussiansExtZeroSh);
     m.def("rasterize_gaussians_backward_ext", &RasterizeGaussiansBackwardExt);
+    m.def("rasterize_gaussians_backward_ext", &RasterizeGaussiansBackwardExtZeroSh);
     m.def("rasterize_gaussians_batch", &RasterizeGaussiansBatch);
     m.def("rasterize_gaussians_backward_batch", &RasterizeGaussiansBackwardBatch);
     m.def("debug_export_binning_view", &DebugExportBinningView);

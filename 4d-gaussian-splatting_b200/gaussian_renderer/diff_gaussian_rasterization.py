@@ -77,6 +77,18 @@ def _notify_forward(radii):
         step.on_forward(radii)
 
 
+def _wants_factors(sh, cov3Ds_precomp):
+    """The view-parallel step (fdgs/dist.py) takes this view's SH gradient as colour factors, not dense rows."""
+    from fdgs.dist import ViewParallelStep
+    step = ViewParallelStep.current()
+    return step is not None and step.wants_factors(sh, cov3Ds_precomp)
+
+
+def _grad_sh(*sh):
+    """Whether autograd will ask for the SH gradient of a call made now (inside Function.forward grad mode is off)."""
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in sh)
+
+
 class GaussianRasterizationSettings(NamedTuple):
     """Per-view constants (reference: :227-245; names and order are the contract)."""
     image_height: int
@@ -108,18 +120,26 @@ class _RasterizeGaussians(torch.autograd.Function):
     sh = features_dc [P,1,3] / sh_rest = features_rest [P,M-1,3] -- and the gradients come back w.r.t. exactly those, so
     the exp / F.normalize x2 / sigmoid kernels and the 1.15 GB torch.cat of the reference's getters
     (scene/gaussian_model.py:179-219), with their autograd mirror images, disappear from the frame.  Otherwise sh_rest is
-    empty.  bg_image: a per-pixel background [3,H,W] behind the Gaussians, or None."""
+    empty.  bg_image: a per-pixel background [3,H,W] behind the Gaussians, or None.  grad_sh: the caller runs under grad
+    mode and the SH input requires a gradient -- the forward then allocates the dense SH gradient and its blend writes
+    the zero rows of the Gaussians this view does not render, so that the backward writes only the rendered rows."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, sh_rest, colors_precomp, flow_2d, opacities, ts, scales, scales_t,
-                rotations, rotations_r, cov3Ds_precomp, prefilter_var, raster_settings, raw, bg_image):
+                rotations, rotations_r, cov3Ds_precomp, prefilter_var, raster_settings, raw, bg_image, grad_sh):
         s = raster_settings
+        g_sh = g_sh_rest = _NONE
+        if grad_sh and sh.numel() > 0 and colors_precomp.numel() == 0 and not _wants_factors(sh, cov3Ds_precomp):
+            P = means3D.shape[0]
+            g_sh = torch.empty((P, sh.shape[1], 3), dtype=torch.float32, device=means3D.device)
+            if sh_rest.numel() > 0:
+                g_sh_rest = torch.empty((P, sh_rest.shape[1], 3), dtype=torch.float32, device=means3D.device)
         # _C.rasterize_gaussians' positional layout (reference: :88-119, rasterize_points.h:18-49) + the extensions
         args = (s.bg, means3D, colors_precomp, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
                 s.scale_modifier, cov3Ds_precomp, prefilter_var, s.viewmatrix, s.projmatrix, s.tanfovx, s.tanfovy,
                 s.image_height, s.image_width, sh, s.sh_degree, s.sh_degree_t, s.campos, s.timestamp,
                 s.time_duration, s.rot_4d, s.gaussian_dim, s.force_sh_3d, s.prefiltered, s.debug,
-                sh_rest, raw, _NONE if bg_image is None else bg_image)
+                sh_rest, raw, _NONE if bg_image is None else bg_image, g_sh, g_sh_rest)
         (num_rendered, color, flow, depth, T, radii, geom_buf, binning_buf, img_buf, covs_com,
          out_means3D) = _invoke(_C.rasterize_gaussians_ext, args, s.debug, "snapshot_fw.dump")
 
@@ -131,6 +151,8 @@ class _RasterizeGaussians(torch.autograd.Function):
         ctx.prefilter_var = prefilter_var
         ctx.save_for_backward(colors_precomp, means3D, out_means3D, scales, rotations, cov3Ds_precomp, radii, sh, sh_rest,
                               flow_2d, opacities, ts, scales_t, rotations_r, geom_buf, binning_buf, img_buf)
+        # outputs of this call, written once more by the backward: kept out of save_for_backward's version checks
+        ctx.g_sh = (g_sh, g_sh_rest)
         ctx.mark_non_differentiable(radii)
         # outputs the loss does not touch arrive as None in backward() instead of zero images; the
         # library then skips their recurrences (the reference always blends all seven channels back)
@@ -157,6 +179,9 @@ class _RasterizeGaussians(torch.autograd.Function):
         step = ViewParallelStep.current()
         factors = (step is not None and step.wants_factors(sh, cov3Ds_precomp)
                    and (ctx.needs_input_grad[2] or ctx.needs_input_grad[3]))
+        zeroed_sh, zeroed_sh_rest = (_NONE, _NONE) if factors else ctx.g_sh
+        # once returned, the tensors belong to autograd: a second backward (retain_graph) allocates its own
+        ctx.g_sh = (_NONE, _NONE)
         want_bg = ctx.needs_input_grad[16]
         # _C.rasterize_gaussians_backward's positional layout (reference: :154-190, rasterize_points.h:51-89) + the
         # extensions
@@ -165,7 +190,8 @@ class _RasterizeGaussians(torch.autograd.Function):
                 s.projmatrix, s.tanfovx, s.tanfovy, grad_out_color, grad_depth, grad_alpha, grad_flow, sh,
                 s.sh_degree, s.sh_degree_t, s.campos, s.timestamp, s.time_duration, s.rot_4d, s.gaussian_dim,
                 s.force_sh_3d, geom_buf, ctx.num_rendered, binning_buf, img_buf, s.debug,
-                sh_rest, ctx.raw, _NONE if ctx.bg_image is None else ctx.bg_image, bool(factors), bool(want_bg))
+                sh_rest, ctx.raw, _NONE if ctx.bg_image is None else ctx.bg_image, bool(factors), bool(want_bg),
+                zeroed_sh, zeroed_sh_rest)
         (g_means2D, g_colors, g_opacities, g_means3D, g_cov3D, g_sh, g_flows, g_ts, g_scales, g_scales_t, g_rot, g_rot_r,
          sh_factors, g_sh_rest, g_bg) = _invoke(_C.rasterize_gaussians_backward_ext, args, s.debug, "snapshot_bw.dump")
         if factors:
@@ -180,11 +206,11 @@ class _RasterizeGaussians(torch.autograd.Function):
             # inputs passed as the empty "not provided" placeholder take no gradient
             return grad if (inp.numel() > 0 and grad is not None) else None
 
-        # one entry per forward input (reference: :208-223); prefilter_var / settings / raw get None
+        # one entry per forward input (reference: :208-223); prefilter_var / settings / raw / grad_sh get None
         return (g_means3D, g_means2D, for_input(g_sh, sh), for_input(g_sh_rest, sh_rest), for_input(g_colors, colors_precomp),
                 for_input(g_flows, flow_2d), g_opacities, for_input(g_ts, ts), for_input(g_scales, scales),
                 for_input(g_scales_t, scales_t), for_input(g_rot, rotations), for_input(g_rot_r, rotations_r),
-                for_input(g_cov3D, cov3Ds_precomp), None, None, None, g_bg if want_bg else None)
+                for_input(g_cov3D, cov3Ds_precomp), None, None, None, g_bg if want_bg else None, None)
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, flow_2d, opacities, ts, scales, scales_t,
@@ -195,7 +221,7 @@ def rasterize_gaussians(means3D, means2D, sh, colors_precomp, flow_2d, opacities
     _check_bg_image(bg_image, raster_settings, means3D)
     return _RasterizeGaussians.apply(means3D, means2D, sh, _NONE, colors_precomp, flow_2d, opacities, ts, scales,
                                      scales_t, rotations, rotations_r, cov3Ds_precomp, prefilter_var,
-                                     raster_settings, False, bg_image)
+                                     raster_settings, False, bg_image, _grad_sh(sh))
 
 
 class GaussianRasterizer(nn.Module):
@@ -225,7 +251,8 @@ class GaussianRasterizer(nn.Module):
         _check_bg_image(bg_image, self.raster_settings, means3D)
         return _RasterizeGaussians.apply(means3D, means2D, features_dc, opt(features_rest), _NONE, opt(flow_2d),
                                          opacity_logits, opt(ts), log_scales, opt(log_scales_t), rotations_raw,
-                                         opt(rotations_r_raw), _NONE, prefilter_var, self.raster_settings, True, bg_image)
+                                         opt(rotations_r_raw), _NONE, prefilter_var, self.raster_settings, True, bg_image,
+                                         _grad_sh(features_dc, features_rest))
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, flow_2d=None, ts=None,
                 scales=None, scales_t=None, rotations=None, rotations_r=None, cov3D_precomp=None,

@@ -225,6 +225,23 @@ int fdgs_forward_bg(const fdgs_forward_args* args, const float* bg_image,
                     fdgs_forward_result* result);
 int fdgs_backward_bg(const fdgs_backward_args* args, const float* bg_image, float* dL_dbg_image, void* stream);
 
+/* The SH gradient's zero rows written by the forward.  In training most Gaussians are not rendered by a view, and their
+ * dL_dsh rows are zero: about 800 MB of a 2M-Gaussian model's 1.15 GB [P,48,3] gradient.  fdgs_forward_zero_sh is
+ * fdgs_forward_bg that, with dL_dsh non-NULL, also writes those rows -- every row of a Gaussian with radii == 0 or no
+ * tile touched -- from the blend kernel, whose DRAM is otherwise nearly idle.  dL_dsh is [P,M,3], or with shs_rest the
+ * split pair dL_dsh [P,1,3] + dL_dsh_rest [P,M-1,3]; the other rows are left as they are.  Both NULL: fdgs_forward_bg.
+ * fdgs_backward_zero_sh is fdgs_backward_bg; with sh_rows_zeroed != 0 it takes the SAME dL_dsh (| dL_dsh_rest) that its
+ * forward zeroed and writes only the rendered rows (the view-parallel sh_factors mode ignores the flag), computed as
+ * fdgs_backward_bg computes them: together the two calls leave the dense gradient fdgs_backward_bg writes. */
+int fdgs_forward_zero_sh(const fdgs_forward_args* args, const float* bg_image, float* dL_dsh, float* dL_dsh_rest,
+                         fdgs_alloc_fn geom_alloc, void* geom_ctx,
+                         fdgs_alloc_fn binning_alloc, void* binning_ctx,
+                         fdgs_alloc_fn image_alloc, void* image_ctx,
+                         void* stream,
+                         fdgs_forward_result* result);
+int fdgs_backward_zero_sh(const fdgs_backward_args* args, const float* bg_image, float* dL_dbg_image, int sh_rows_zeroed,
+                          void* stream);
+
 /* Batched views: B >= 1 cameras of the same Gaussians in one call per direction, one launch per stage and ONE host
  * synchronisation for the whole batch.  Every view's outputs are bit-identical to fdgs_forward_bg on that camera.
  * `view` holds what the views share, as in fdgs_forward_args, except:
