@@ -5,34 +5,21 @@
 // the per-pixel n_contrib cut), but
 //
 //   * the 12 fp32 atomicAdd per contributing (pixel, Gaussian) PAIR of the reference
-//     (backward.cu:1076,1091,1124-1134) become one warp reduce-scatter (13 shuffles for 12
-//     values) per (warp, Gaussian) followed by a single RED instruction with 12 active lanes --
-//     a 32x..(32/cull) reduction in atomic traffic, and none at all for Gaussians whose
+//     (backward.cu:1076,1091,1124-1134) become one tensor-core reduction over the warp's 32 pixels
+//     per 8 Gaussians followed by one RED per per-Gaussian sum, and none at all for Gaussians whose
 //     alpha >= 1/255 footprint misses the warp's 8x4 pixel rectangle (culled before any math);
 //   * the work list is streamed with cp.async.bulk through the same mbarrier ring as the
 //     forward, walking the tile's contiguous record range from the back, starting at the deepest
 //     position any pixel of the tile actually reached (max n_contrib) instead of the list end;
 //   * when the caller has no gradient for the flow / depth / alpha images (the reference's default
 //     training loss only touches the colour image) the AUX = false instantiation drops their
-//     recurrences and reduces 9 values with 12 shuffles.  The constant factors of the
-//     mean / conic gradients (-0.5, -W/2, -H/2) are applied once per Gaussian after the reduction.
-#include <stdlib.h>
+//     recurrences;
+//   * the mean / conic / opacity gradients leave as raw moment sums of w = G dL/dalpha about each
+//     Gaussian's mean; geom_bwd_kernel (preprocess_bwd.cu) applies their linear map once per Gaussian.
 #include "fdgs_internal.h"
 
 namespace fdgs {
 namespace {
-
-constexpr int BB_THREADS = 256;
-constexpr int BB_WARPS = BB_THREADS / 32;
-constexpr int BB_BATCH = 128;
-constexpr int BB_STAGES = 3;
-
-struct __align__(128) BlendBwdSmem {
-    StageRec recs[BB_STAGES][BB_BATCH];
-    uint64_t full[BB_STAGES];
-    uint64_t empty[BB_STAGES];
-    unsigned int nmax;
-};
 
 __device__ __forceinline__ float ex2_approx(float x) {
     float y;
@@ -80,283 +67,14 @@ __device__ __forceinline__ BlendBwdParams blend_bwd_view(BlendBwdParams p, int v
     return p;
 }
 
-template <bool AUX, bool BATCH>
-__device__ __forceinline__ void blend_bwd_body(const BlendBwdParams& p_) {
-    __shared__ BlendBwdSmem sm;
-    // an lvalue on both sides: the single-view instantiation reads its parameters in place, no copy
-    BlendBwdParams view_;
-    if (BATCH) view_ = blend_bwd_view(p_, blockIdx.z);
-    const BlendBwdParams& p = BATCH ? view_ : p_;
-    const int tile = blockIdx.y * p.grid_x + blockIdx.x;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int wx0 = blockIdx.x * TILE_X + (warp & 1) * 8;
-    const int wy0 = blockIdx.y * TILE_Y + (warp >> 1) * 4;
-    const int pix_x = wx0 + (lane & 7), pix_y = wy0 + (lane >> 3);
-    const bool inside = pix_x < p.W && pix_y < p.H;
-    const float pxf = (float)pix_x, pyf = (float)pix_y;
-    const float bx0 = (float)wx0, bx1 = (float)(wx0 + 7), by0 = (float)wy0, by1 = (float)(wy0 + 3);
-    const int HW = p.H * p.W;
-    const int pix_id = pix_y * p.W + pix_x;
-
-    const uint2 range = p.ranges[tile];
-    const int n_list = (int)(range.y - range.x);
-    const unsigned int my_last = inside ? p.n_contrib[pix_id] : 0u;   // backward.cu:982
-    const unsigned int wmax = __reduce_max_sync(0xffffffffu, my_last);
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < BB_STAGES; ++s) {
-            mbar_init(&sm.full[s], 1);
-            mbar_init(&sm.empty[s], BB_WARPS);
-        }
-        sm.nmax = 0;
-        mbar_fence_init();
-    }
-    __syncthreads();
-    if (lane == 0 && wmax) atomicMax(&sm.nmax, wmax);
-    __syncthreads();
-    // entries at list positions >= max n_contrib are skipped by every pixel (backward.cu:1040)
-    const int n = min(n_list, (int)sm.nmax);
-    const int nb = (n + BB_BATCH - 1) / BB_BATCH;
-    const StageRec* src = p.recs + range.x;
-
-    int issued = 0;
-    if (threadIdx.x == 0) {
-        for (; issued < nb && issued < BB_STAGES; ++issued) {
-            const int hi = n - issued * BB_BATCH, lo = max(0, hi - BB_BATCH);
-            mbar_expect_tx(&sm.full[issued], (uint32_t)(hi - lo) * kStageRecBytes);
-            bulk_g2s(&sm.recs[issued][0], src + lo, (uint32_t)(hi - lo) * kStageRecBytes, &sm.full[issued]);
-        }
-    }
-
-    // per-pixel state, backward.cu:976-1011
-    const float T_final = inside ? p.final_T[pix_id] : 0.f;
-    float T = T_final;
-    float acc_c0 = 0.f, acc_c1 = 0.f, acc_c2 = 0.f, acc_f0 = 0.f, acc_f1 = 0.f, acc_d = 0.f, acc_m = 0.f;
-    float gp0 = 0.f, gp1 = 0.f, gp2 = 0.f, gf0 = 0.f, gf1 = 0.f, gd = 0.f, gm = 0.f;
-    if (inside) {
-        gp0 = p.dL_dpix[0 * HW + pix_id];
-        gp1 = p.dL_dpix[1 * HW + pix_id];
-        gp2 = p.dL_dpix[2 * HW + pix_id];
-        if (AUX) {
-            if (p.dL_dpix_flow) { gf0 = p.dL_dpix_flow[0 * HW + pix_id]; gf1 = p.dL_dpix_flow[1 * HW + pix_id]; }
-            if (p.dL_depths) gd = p.dL_depths[pix_id];
-            if (p.dL_masks) gm = p.dL_masks[pix_id];
-        }
-    }
-    float bg0 = p.background[0], bg1 = p.background[1], bg2 = p.background[2];
-    if (inside) background_image_terms(p, pix_id, HW, T_final, gp0, gp1, gp2, bg0, bg1, bg2);
-    // background term of dL_dalpha, backward.cu:1110-1113:  (-T_final / (1 - alpha)) * (bg . dL_dpixel)
-    const float tb = -T_final * (bg0 * gp0 + bg1 * gp1 + bg2 * gp2);
-
-    // Reduce-scatter targets.  AUX: 12 values { dcolor r,g,b | dmean2D x,y,depth | dconic x,y,w |
-    // dflow x,y, dopacity }, value 6*b4 + 3*b3 + (b1 ? 2 : b2) ends on the even lanes (b_k = bit k of
-    // the lane id).  !AUX: 8 values { dcolor r,g,b, dmean2D x,y, dconic x,y,w } on lanes 0,4,..,28
-    // plus dopacity on lane 2.  red_scale = the constant factor of that gradient component:
-    // ddelx_dx = W/2, ddely_dy = H/2 (backward.cu:1008-1009) and the -0.5 of the conic terms.
-    const bool hi16 = (lane & 16) != 0, hi8 = (lane & 8) != 0, hi4 = (lane & 4) != 0, hi2 = (lane & 2) != 0;
-    float* red_ptr = nullptr;
-    unsigned int red_mul = 0;
-    float red_scale = 1.f;
-    bool red_lane;
-    {
-        int idx;   // position in the 12-value list above
-        if (AUX) {
-            red_lane = ((lane & 1) == 0) && !(hi2 && hi4);
-            idx = 6 * (int)hi16 + 3 * (int)hi8 + (hi2 ? 2 : (int)hi4);
-        } else {
-            red_lane = ((lane & 3) == 0) || lane == 2;
-            const int i8 = (lane >> 2) & 7;   // r g b mx my cx cy cw
-            idx = (lane == 2) ? 11 : (i8 < 5 ? i8 : i8 + 1);
-        }
-        if (idx < 3) { red_ptr = p.dL_dcolor + idx; red_mul = 3; }
-        else if (idx < 6) {
-            red_ptr = p.dL_dmean2D + (idx - 3); red_mul = 3;
-            red_scale = (idx == 3) ? -0.5f * (float)p.W : (idx == 4) ? -0.5f * (float)p.H : 1.f;
-        } else if (idx < 9) { red_ptr = p.dL_dconic + ((idx == 8) ? 3 : idx - 6); red_mul = 4; red_scale = -0.5f; }
-        else if (idx < 11) { red_ptr = p.dL_dflows + (idx - 9); red_mul = 2; }
-        else { red_ptr = p.dL_dopacity; red_mul = 1; }
-    }
-
-    for (int b = 0; b < nb; ++b) {
-        const int s = b % BB_STAGES;
-        const uint32_t ph = (uint32_t)(b / BB_STAGES) & 1u;
-        const int hi = n - b * BB_BATCH, lo = max(0, hi - BB_BATCH), cnt = hi - lo;
-        mbar_wait(&sm.full[s], ph);
-        if ((unsigned)lo < wmax) {
-            const StageRec* st = sm.recs[s];
-            for (int r0 = ((cnt - 1) >> 5) << 5; r0 >= 0; r0 -= 32) {
-                const int j = r0 + lane;
-                bool rel = false;
-                if (j < cnt && (unsigned)(lo + j) < wmax) {
-                    const float4 a = st[j].q0;
-                    const float4 c = st[j].q1;
-                    const float4 e = st[j].q3;
-                    rel = rect_may_contribute(a.x, a.y, c.x, c.y, c.z, a.z, e.z, e.w, bx0, bx1, by0, by1);
-                }
-                uint32_t m = __ballot_sync(0xffffffffu, rel);
-                while (m) {
-                    const int k = 31 - __clz(m);
-                    m &= ~(1u << k);
-                    const StageRec* g = st + (r0 + k);
-                    const unsigned int pos = (unsigned)(lo + r0 + k);   // "contributor" index
-                    const float4 q0 = g->q0;
-                    const float4 q1 = g->q1;
-                    const float dx = fsub(q0.x, pxf);
-                    const float dy = fsub(q0.y, pyf);
-                    const float power =
-                        ffma(ffma(dx, fmul(dx, q1.x), fmul(dy, fmul(dy, q1.z))), -0.5f, -fmul(dy, fmul(dx, q1.y)));
-                    bool contrib = (pos < my_last) && !(power > 0.0f) && !(power < q0.z);
-                    float G = 0.f, alpha = 0.f;
-                    if (contrib) {
-                        // exp(power): the fast exponential is accurate to ~6e-7 here (power in [-6, 0]);
-                        // next to the 1/255 threshold the decision is redone with the forward's expf
-                        // so that both passes agree on the set of contributors (forward.cu:590).
-                        G = ex2_approx(power * 1.4426950408889634f);
-                        float og = q1.w * G;
-                        if (fabsf(og - 0.00392156886f) < 2.0e-8f) {
-                            G = expf(power);
-                            og = fmul(q1.w, G);
-                        }
-                        alpha = fminf(og, 0.99f);
-                        contrib = !(alpha < 1.0f / 255.0f);
-                    }
-                    if (!__any_sync(0xffffffffu, contrib)) continue;
-
-                    constexpr int NV = AUX ? 12 : 8;
-                    float v[NV];
-                    float z = 0.f;   // !AUX: dopacity
-#pragma unroll
-                    for (int i = 0; i < NV; ++i) v[i] = 0.f;
-                    if (contrib) {
-                        const float4 q2 = g->q2;
-                        // 1/(1-alpha): alpha <= 0.99, so the approximate reciprocal (1 ulp) is safe; the
-                        // reference divides twice here (backward.cu:1056,1113)
-                        const float om = 1.f - alpha;
-                        float rom;
-                        asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rom) : "f"(om));
-                        T = T * rom;
-                        const float dchannel_dcolor = alpha * T;
-                        // colour / flow / depth / mask recurrences, backward.cu:1062-1102.  acc_* are the
-                        // blended values behind this Gaussian; acc + alpha * (c - acc) = the value as
-                        // seen by the next (nearer) one.
-                        const float d0 = q2.x - acc_c0, d1 = q2.y - acc_c1, d2 = q2.z - acc_c2;
-                        float dL_dalpha = d0 * gp0;
-                        dL_dalpha = fmaf(d1, gp1, dL_dalpha);
-                        dL_dalpha = fmaf(d2, gp2, dL_dalpha);
-                        acc_c0 = fmaf(alpha, d0, acc_c0);
-                        acc_c1 = fmaf(alpha, d1, acc_c1);
-                        acc_c2 = fmaf(alpha, d2, acc_c2);
-                        if (AUX) {
-                            const float2 fl = *reinterpret_cast<const float2*>(&g->q3);
-                            const float e0 = fl.x - acc_f0, e1 = fl.y - acc_f1, dd = q2.w - acc_d, dm = 1.0f - acc_m;
-                            dL_dalpha = fmaf(e0, gf0, dL_dalpha);
-                            dL_dalpha = fmaf(e1, gf1, dL_dalpha);
-                            dL_dalpha = fmaf(dd, gd, dL_dalpha);
-                            dL_dalpha = fmaf(dm, gm, dL_dalpha);
-                            acc_f0 = fmaf(alpha, e0, acc_f0);
-                            acc_f1 = fmaf(alpha, e1, acc_f1);
-                            acc_d = fmaf(alpha, dd, acc_d);
-                            acc_m = fmaf(alpha, dm, acc_m);
-                        }
-                        dL_dalpha = fmaf(tb, rom, dL_dalpha * T);
-
-                        // w = G dL_dalpha = dL_dopacity term; ko = G dL_dG; the mean / conic gradients are
-                        // ko * {dx, dy} moments (their -0.5 / -W/2 / -H/2 factors follow the reduction)
-                        const float w = G * dL_dalpha;
-                        const float ko = q1.w * w;
-                        const float hx = ko * dx, hy = ko * dy;
-                        v[0] = dchannel_dcolor * gp0;
-                        v[1] = dchannel_dcolor * gp1;
-                        v[2] = dchannel_dcolor * gp2;
-                        v[3] = fmaf(hx, q1.x, hy * q1.y);
-                        v[4] = fmaf(hy, q1.z, hx * q1.y);
-                        if (AUX) {
-                            v[5] = gd * dchannel_dcolor;
-                            v[6] = hx * dx;
-                            v[7] = hx * dy;
-                            v[8] = hy * dy;
-                            v[9] = dchannel_dcolor * gf0;
-                            v[10] = dchannel_dcolor * gf1;
-                            v[11] = w;
-                        } else {
-                            v[5] = hx * dx;
-                            v[6] = hx * dy;
-                            v[7] = hy * dy;
-                            z = w;
-                        }
-                    }
-                    // warp reduce-scatter: every level halves the values a lane carries; an odd value
-                    // rides along as a plain butterfly until it can pair up
-                    constexpr int H1 = NV / 2, H2 = NV / 4;
-                    float a[H1];
-#pragma unroll
-                    for (int i = 0; i < H1; ++i) {
-                        const float send = hi16 ? v[i] : v[i + H1];
-                        const float keep = hi16 ? v[i + H1] : v[i];
-                        a[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-                    }
-                    float bb[H2];
-#pragma unroll
-                    for (int i = 0; i < H2; ++i) {
-                        const float send = hi8 ? a[i] : a[i + H2];
-                        const float keep = hi8 ? a[i + H2] : a[i];
-                        bb[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-                    }
-                    float c4;
-                    if (AUX) {
-                        // 3 values per lane: two pair up, the third becomes the butterfly rider
-                        c4 = (hi4 ? bb[1] : bb[0]) + __shfl_xor_sync(0xffffffffu, hi4 ? bb[0] : bb[1], 4);
-                        z = bb[2] + __shfl_xor_sync(0xffffffffu, bb[2], 4);
-                    } else {
-                        z += __shfl_xor_sync(0xffffffffu, z, 16);
-                        z += __shfl_xor_sync(0xffffffffu, z, 8);
-                        c4 = (hi4 ? bb[1] : bb[0]) + __shfl_xor_sync(0xffffffffu, hi4 ? bb[0] : bb[1], 4);
-                        z += __shfl_xor_sync(0xffffffffu, z, 4);
-                    }
-                    float d = (hi2 ? z : c4) + __shfl_xor_sync(0xffffffffu, hi2 ? c4 : z, 2);
-                    d += __shfl_xor_sync(0xffffffffu, d, 1);
-                    if (red_lane) {
-                        const unsigned int gid = __float_as_uint(q0.w);
-                        atomicAdd(red_ptr + (size_t)gid * red_mul, d * red_scale);
-                    }
-                }
-            }
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&sm.empty[s]);
-        if (threadIdx.x == 0 && issued < nb) {
-            mbar_wait(&sm.empty[s], ph);
-            const int nhi = n - issued * BB_BATCH, nlo = max(0, nhi - BB_BATCH);
-            mbar_expect_tx(&sm.full[s], (uint32_t)(nhi - nlo) * kStageRecBytes);
-            bulk_g2s(&sm.recs[s][0], src + nlo, (uint32_t)(nhi - nlo) * kStageRecBytes, &sm.full[s]);
-            ++issued;
-        }
-    }
-}
-
-template <bool AUX>
-__global__ void __launch_bounds__(BB_THREADS, AUX ? 3 : 4) blend_bwd_kernel(const BlendBwdParams p_) {
-    blend_bwd_body<AUX, false>(p_);
-}
-
-// the batched entry (fdgs_forward_batch / fdgs_backward_batch): one view per blockIdx.z
-template <bool AUX>
-__global__ void __launch_bounds__(BB_THREADS, AUX ? 3 : 4) blend_bwd_batch_kernel(const BlendBwdParams p_) {
-    blend_bwd_body<AUX, true>(p_);
-}
-
-
 // =====================================================================================================
-// v2: colour-only backward (no upstream gradient for flow / depth / alpha), the training default.
-//
-// Same per-pixel recurrences as above; what changes is how a (warp, Gaussian) step is evaluated and
-// how the 32 per-pixel partial sums of a Gaussian are reduced -- the two things the ncu capture of
-// v1 showed the issue slots going to:
+// The kernel.  The blend is bound by instruction issue, so two things set its speed: how a (warp, Gaussian)
+// step is evaluated and how the 32 per-pixel partial sums of a Gaussian are reduced.
 //
 //   * power(pixel) is a quadratic in the pixel offset, so the lane that culls an instance against the
 //     warp's 8x4 rectangle also expands it about the rectangle centre (6 coefficients, pre-scaled by
 //     log2 e) and parks them in a per-warp shared-memory slot; a step is then 2 LDS.128 + 5 FFMA +
-//     1 MUFU.EX2 instead of bit-scan + 2 LDS.128 + 2 FADD + 7 FMUL/FFMA + FMUL + MUFU.  The polynomial
+//     1 MUFU.EX2 instead of the forward's per-pixel expression.  The polynomial
 //     differs from the forward's exact power by a few 1e-6 (absolute); pairs whose alpha lands within
 //     6e-7 of the 1/255 cut, or whose power is within 1e-4 of 0, and every pair of an instance whose
 //     quadratic has large cancelling terms (thin rotated Gaussians far from their centre), are re-decided
@@ -367,11 +85,11 @@ __global__ void __launch_bounds__(BB_THREADS, AUX ? 3 : 4) blend_bwd_batch_kerne
 //     product  [weights 16 x 32] x [values 32 x 8 Gaussians]  and runs on the tensor cores
 //     (mma.sync m16n8k8 tf32, fp32 accumulate; values split hi+lo so the result is fp32-accurate; the
 //     monomials are exact in tf32, the colour gradients are split as well): 2 STS per step and one
-//     flush per 8 Gaussians (16 LDS + 16 splits + 16 HMMA + moment re-centring) replace
-//     12 SHFL + 17 FSEL + 13 FADD + a 9-lane RED per step.  The raw moments are re-centred on the
+//     flush per 8 Gaussians (16 LDS + 16 splits + 16 HMMA + moment re-centring).  AUX adds the depth and
+//     flow gradients as rows of the a1-weighted tile.  The raw moments are re-centred on the
 //     Gaussian's own mean per (warp, Gaussian) -- small numbers, no cancellation -- and accumulated with
 //     RED; their constant linear map to dL/dmean2D, dL/dconic (conic and opacity factors) is applied
-//     once per Gaussian by geom_bwd_kernel (PreprocessBwdParams::blend_raw).
+//     once per Gaussian by geom_bwd_kernel.
 constexpr int B2_THREADS = 256;
 constexpr int B2_WARPS = B2_THREADS / 32;
 constexpr int B2_BATCH = 64;
@@ -405,7 +123,7 @@ struct __align__(128) B2Smem {
 };
 
 // The forward's exact evaluation of one (pixel, Gaussian) pair (forward.cu:578-590 as compiled; see
-// blend_fwd.cu): decides the pairs the polynomial of the v2 kernel cannot (rare, kept out of line).
+// blend_fwd.cu): decides the pairs the polynomial cannot (rare, kept out of line).
 __device__ __noinline__ float2 exact_pair(const StageRec* g, float pxf, float pyf) {
     const float4 q0 = g->q0, q1 = g->q1;
     const float dx = fsub(q0.x, pxf), dy = fsub(q0.y, pyf);
@@ -748,38 +466,25 @@ __global__ void __launch_bounds__(B2_THREADS, (ACOL_SMEM && !AUX) ? 4 : 3) blend
 
 }  // namespace
 
-bool blend_bwd_is_raw(const BlendBwdParams&) {
-    // the v2 kernels leave RAW moment sums in dL_dmean2D.xy / dL_dconic / dL_dopacity for geom_bwd_kernel to finish
-    // (PreprocessBwdParams::blend_raw); FDGS_BLEND_BWD_V1 selects the shuffle-reduction kernels (kept for comparison)
-    static const bool force_v1 = getenv("FDGS_BLEND_BWD_V1") != nullptr;
-    return !force_v1;
-}
-
 template <bool BATCH>
 static cudaError_t blend_bwd(const BlendBwdParams& p, cudaStream_t stream) {
     const dim3 grid(p.grid_x, p.grid_y, BATCH ? p.views : 1);
     const bool aux = p.dL_depths || p.dL_masks || p.dL_dpix_flow;
-    if (blend_bwd_is_raw(p)) {
-        if (!aux) {
-            // colour fragments in shared memory + 3 stages: 64 registers, 53 KB -> 4 CTAs / SM.  (Keeping them in
-            // registers costs 80 registers -> 3 CTAs / SM and measured 8 % slower.)
-            const auto k = BATCH ? blend_bwd2_batch_kernel<3, true, false> : blend_bwd2_kernel<3, true, false>;
-            static PerDeviceOnce once;
-            cudaError_t e = ensure_dynamic_smem(k, (int)sizeof(B2Smem<3, true, false>), once);
-            if (e != cudaSuccess) return e;
-            k<<<grid, B2_THREADS, sizeof(B2Smem<3, true, false>), stream>>>(p);
-        } else {
-            // upstream gradients for the depth / alpha / flow images too: 6 a1-weighted rows (16-row A tile), 3 CTAs / SM
-            const auto k = BATCH ? blend_bwd2_batch_kernel<3, true, true> : blend_bwd2_kernel<3, true, true>;
-            static PerDeviceOnce once_aux;
-            cudaError_t e = ensure_dynamic_smem(k, (int)sizeof(B2Smem<3, true, true>), once_aux);
-            if (e != cudaSuccess) return e;
-            k<<<grid, B2_THREADS, sizeof(B2Smem<3, true, true>), stream>>>(p);
-        }
+    if (!aux) {
+        // colour fragments in shared memory + 3 stages: 64 registers, 53 KB -> 4 CTAs / SM.  (Keeping them in
+        // registers costs 80 registers -> 3 CTAs / SM and measured 8 % slower.)
+        const auto k = BATCH ? blend_bwd2_batch_kernel<3, true, false> : blend_bwd2_kernel<3, true, false>;
+        static PerDeviceOnce once;
+        cudaError_t e = ensure_dynamic_smem(k, (int)sizeof(B2Smem<3, true, false>), once);
+        if (e != cudaSuccess) return e;
+        k<<<grid, B2_THREADS, sizeof(B2Smem<3, true, false>), stream>>>(p);
     } else {
-        const auto k = aux ? (BATCH ? blend_bwd_batch_kernel<true> : blend_bwd_kernel<true>)
-                           : (BATCH ? blend_bwd_batch_kernel<false> : blend_bwd_kernel<false>);
-        k<<<grid, BB_THREADS, 0, stream>>>(p);
+        // upstream gradients for the depth / alpha / flow images too: 6 a1-weighted rows (16-row A tile), 3 CTAs / SM
+        const auto k = BATCH ? blend_bwd2_batch_kernel<3, true, true> : blend_bwd2_kernel<3, true, true>;
+        static PerDeviceOnce once_aux;
+        cudaError_t e = ensure_dynamic_smem(k, (int)sizeof(B2Smem<3, true, true>), once_aux);
+        if (e != cudaSuccess) return e;
+        k<<<grid, B2_THREADS, sizeof(B2Smem<3, true, true>), stream>>>(p);
     }
     return cudaGetLastError();
 }

@@ -43,8 +43,6 @@ constexpr size_t kMaxProfEvents = 4096;
 std::atomic<long long> g_kernel_launches{0};
 // FDGS_TRACE=1 + debug=true: print every stage to stderr before and after its synchronisation
 const bool g_trace = getenv("FDGS_TRACE") != nullptr;
-// summation order of the quaternion norm in the raw-parameter entry (fdgs_common.cuh: quat_norm); 0 = ATen's order
-const int g_quat_norm_mode = getenv("FDGS_NORMALIZE_MODE") ? atoi(getenv("FDGS_NORMALIZE_MODE")) : 0;
 
 // tile lists: 1 = only the tiles a Gaussian's alpha >= 1/255 footprint reaches, 0 = the reference's 3-sigma square
 // (include/fdgs.h: fdgs_set_tile_cull)
@@ -331,7 +329,7 @@ int forward_stages(const fdgs_forward_args* a, const float* bg_image, float* zer
         pp.focal_x = W / (2.0f * a->tan_fovx);
         pp.grid_x = grid_x; pp.grid_y = grid_y; pp.prefiltered = a->prefiltered;
         sh_staging(a->colors_precomp ? nullptr : a->shs, a->M, true, &pp.sh_bulk_ok, &pp.sh_row_stride_floats);
-        pp.raw_params = a->raw_params; pp.quat_norm_mode = g_quat_norm_mode;
+        pp.raw_params = a->raw_params;
         pp.shs_rest = a->colors_precomp ? nullptr : a->shs_rest;
         pp.flows = a->flows_precomp;
         pp.out_means3D = a->out_means3D; pp.radii = a->radii; pp.cov3D = geom.cov3D; pp.grec = geom.grec;
@@ -442,9 +440,7 @@ int backward_stages(const fdgs_backward_args* a, const float* bg_image, float* d
 
     // with no instance at all the blend only has dL_dbg_image to write (P == 0: the background image takes the whole
     // colour gradient, from empty tile lists)
-    const bool instances = P > 0 && R > 0;
-    bool blend_raw = false;
-    if (instances || dL_dbg_image) {
+    if ((P > 0 && R > 0) || dL_dbg_image) {
         fdgs::BlendBwdParams bp;
         bp.W = W; bp.H = H; bp.grid_x = (W + fdgs::TILE_X - 1) / fdgs::TILE_X; bp.grid_y = (H + fdgs::TILE_Y - 1) / fdgs::TILE_Y;
         bp.ranges = img.ranges; bp.recs = bin.recs; bp.background = a->background;
@@ -454,7 +450,6 @@ int backward_stages(const fdgs_backward_args* a, const float* bg_image, float* d
         bp.dL_dcolor = a->dL_dcolor; bp.dL_dflows = a->dL_dflows;
         bp.bg_image = bg_image; bp.dL_dbg_image = dL_dbg_image;
         bp.views = batch ? vb.B : 0; bp.P = P;
-        blend_raw = instances && fdgs::blend_bwd_is_raw(bp);
         FDGS_STAGE(6, 1, fdgs::launch_blend_bwd(bp, stream), batch ? "blend_bwd (batch)" : "blend_bwd");
     }
     if (P <= 0) return FDGS_OK;
@@ -473,10 +468,10 @@ int backward_stages(const fdgs_backward_args* a, const float* bg_image, float* d
     pb.timestamp = a->timestamp; pb.time_duration = a->time_duration;
     pb.rot_4d = a->rot_4d; pb.gaussian_dim = a->gaussian_dim; pb.force_sh_3d = a->force_sh_3d;
     pb.has_scales = (a->scales != nullptr) ? 1 : 0;
-    pb.grec = geom.grec; pb.blend_raw = blend_raw ? 1 : 0; pb.W = W; pb.H = H;
+    pb.grec = geom.grec; pb.W = W; pb.H = H;
     sh_staging(a->shs, a->M, false, &pb.sh_bulk_ok, &pb.sh_row_stride_floats);
     if (a->dL_dsh && (reinterpret_cast<uintptr_t>(a->dL_dsh) % 16) != 0) pb.sh_bulk_ok = 0;
-    pb.raw_params = a->raw_params; pb.quat_norm_mode = g_quat_norm_mode;
+    pb.raw_params = a->raw_params;
     pb.shs_rest = a->shs ? a->shs_rest : nullptr; pb.dL_dsh_rest = a->dL_dsh_rest;
     pb.dL_dmean2D = a->dL_dmean2D; pb.dL_dconic = a->dL_dconic; pb.dL_dopacity = a->dL_dopacity; pb.dL_dcolor = a->dL_dcolor;
     pb.dL_dmean3D = a->dL_dmean3D; pb.dL_dcov3D = a->dL_dcov3D; pb.dL_dsh = a->dL_dsh; pb.sh_factors = a->sh_factors;
@@ -1075,7 +1070,8 @@ int fdgs_debug_activate(int n, const float* log_s, const float* logit, const flo
                         float* q_out, void* stream_v) {
     g_last_error.clear();
     if (n < 0 || (n > 0 && (!log_s || !logit || !quat || !s_out || !o_out || !q_out))) return fail(FDGS_ERR_INVALID_ARG, "null argument");
-    FDGS_CUDA(fdgs::launch_debug_activate(n, log_s, logit, quat, mode, s_out, o_out, q_out, reinterpret_cast<cudaStream_t>(stream_v)),
+    if (mode != 0) return fail(FDGS_ERR_INVALID_ARG, "mode must be 0 (ATen's summation order of the quaternion norm)");
+    FDGS_CUDA(fdgs::launch_debug_activate(n, log_s, logit, quat, s_out, o_out, q_out, reinterpret_cast<cudaStream_t>(stream_v)),
               "debug_activate");
     return FDGS_OK;
 }

@@ -60,25 +60,21 @@ struct Camera {
 //   exp      : expf (full-precision libdevice, what std::exp resolves to in ATen's exp kernel)
 //   sigmoid  : 1 / (1 + expf(-x))                                  (ATen sigmoid kernel, opmath = float)
 //   normalize: q / max(||q||_2, 1e-12); ATen's norm reduction of a 4-element row adds the rounded squares as
-//              (x^2 + z^2) + (y^2 + w^2) -- found by tools/probe_normalize.py on the GPU (all 24 x 2 plain-fp32
-//              orders tried against torch.linalg.vector_norm over 1M rows: only this pairing gives 0 differing words)
+//              (x^2 + z^2) + (y^2 + w^2).  Other plain-fp32 orders differ from F.normalize in the last bit of some
+//              rows; tests/test_gpu_raw_entry.py (test_activations_bit_identical_to_torch) checks all three
+//              activations word for word against torch over 1M rows.
 __device__ __forceinline__ float act_exp(float x) { return expf(x); }
 __device__ __forceinline__ float act_sigmoid(float x) { return fdiv(1.0f, fadd(1.0f, expf(-x))); }
-__device__ __forceinline__ float quat_norm(const float4 q, int mode) {
-    float s;
-    if (mode == 1) s = fadd(fadd(fadd(fmul(q.x, q.x), fmul(q.y, q.y)), fmul(q.z, q.z)), fmul(q.w, q.w));   // sequential
-    else if (mode == 2) s = ffma(q.w, q.w, ffma(q.z, q.z, ffma(q.y, q.y, fmul(q.x, q.x))));                 // fma chain
-    else if (mode == 3) s = fadd(fadd(fmul(q.x, q.x), fmul(q.y, q.y)), fadd(fmul(q.z, q.z), fmul(q.w, q.w)));   // (x,y)+(z,w)
-    else s = fadd(fadd(fmul(q.x, q.x), fmul(q.z, q.z)), fadd(fmul(q.y, q.y), fmul(q.w, q.w)));              // ATen: (x,z)+(y,w)
-    return fsqrt(s);
+__device__ __forceinline__ float quat_norm(const float4 q) {
+    return fsqrt(fadd(fadd(fmul(q.x, q.x), fmul(q.z, q.z)), fadd(fmul(q.y, q.y), fmul(q.w, q.w))));
 }
-__device__ __forceinline__ float4 act_normalize(const float4 q, int mode) {
-    const float d = fmaxf(quat_norm(q, mode), 1e-12f);
+__device__ __forceinline__ float4 act_normalize(const float4 q) {
+    const float d = fmaxf(quat_norm(q), 1e-12f);
     return make_float4(fdiv(q.x, d), fdiv(q.y, d), fdiv(q.z, d), fdiv(q.w, d));
 }
 // gradient w.r.t. the raw quaternion given the gradient g w.r.t. the normalised one (autograd of q / clamp_min(||q||, eps))
-__device__ __forceinline__ float4 act_normalize_bwd(const float4 q, const float4 g, int mode) {
-    const float n = quat_norm(q, mode);
+__device__ __forceinline__ float4 act_normalize_bwd(const float4 q, const float4 g) {
+    const float n = quat_norm(q);
     const float d = fmaxf(n, 1e-12f);
     const float inv = 1.0f / d;
     const float dot = g.x * q.x + g.y * q.y + g.z * q.z + g.w * q.w;

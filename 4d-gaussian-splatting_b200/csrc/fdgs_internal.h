@@ -71,7 +71,6 @@ struct PreprocessFwdParams {
     int sh_bulk_ok;             // SH rows can be streamed with cp.async.bulk (16-byte aligned rows)
     int sh_row_stride_floats;   // padded shared-memory row stride (multiple of 4 floats)
     int raw_params;             // scales / scales_t are log-scales, rotations un-normalised, opacities logits
-    int quat_norm_mode;         // summation order of the quaternion norm (fdgs_common.cuh: quat_norm)
     const float* shs_rest;      // non-NULL: SH row split as shs = [P,1,3] (dc) | shs_rest = [P,M-1,3]
     // outputs
     const float* flows;     // [P,2] or NULL
@@ -88,8 +87,8 @@ struct PreprocessFwdParams {
     ViewBatch vb;
 };
 cudaError_t launch_preprocess_fwd(const PreprocessFwdParams& p, cudaStream_t stream);
-cudaError_t launch_debug_activate(int n, const float* log_s, const float* logit, const float* quat, int mode, float* s_out,
-                                  float* o_out, float* q_out, cudaStream_t stream);
+cudaError_t launch_debug_activate(int n, const float* log_s, const float* logit, const float* quat, float* s_out, float* o_out,
+                                  float* q_out, cudaStream_t stream);
 
 // ---- binning -----------------------------------------------------------------------------------
 // counting sort of the (Gaussian, tile) instances by tile, BIN_CTAS persistent CTAs (binning.cu)
@@ -162,11 +161,9 @@ struct BlendBwdParams {
     int views;               // > 0: batched entry, blockIdx.z = view; images and the five gradients are [views] stacks
     int P;                   // Gaussians per view (the batched entry's gradient stride)
 };
+// leaves RAW moment sums (W10, W01 | W20, W11, W02 | W00 of w = G dL/dalpha about each Gaussian's mean) in
+// dL_dmean2D.xy / dL_dconic / dL_dopacity instead of the final gradients; launch_preprocess_bwd finishes them
 cudaError_t launch_blend_bwd(const BlendBwdParams& p, cudaStream_t stream);
-// true when launch_blend_bwd(p) leaves RAW moment sums (W10, W01 | W20, W11, W02 | W00 of w = G dL/dalpha
-// about each Gaussian's mean) in dL_dmean2D.xy / dL_dconic / dL_dopacity instead of the final
-// gradients; launch_preprocess_bwd finishes them (PreprocessBwdParams::blend_raw)
-bool blend_bwd_is_raw(const BlendBwdParams& p);
 
 // ---- backward preprocess ------------------------------------------------------------------------
 struct PreprocessBwdParams {
@@ -195,15 +192,13 @@ struct PreprocessBwdParams {
     int sh_bulk_ok;         // SH rows are 16-byte aligned and 16-byte multiples: stream with cp.async.bulk
     int sh_row_stride_floats;
     int raw_params;         // as in the forward: gradients then come out w.r.t. the RAW parameters
-    int quat_norm_mode;
     const float* shs_rest;  // split SH input (see PreprocessFwdParams)
     float* dL_dsh_rest;     // [P,M-1,3] when shs_rest is given (dL_dsh is then [P,1,3])
-    float* dL_dmean2D;      // in/out when blend_raw
-    float* dL_dconic;       // in/out when blend_raw
+    float* dL_dmean2D;      // in/out: .xy raw moment sums of the blend backward in, final gradients out
+    float* dL_dconic;       // in/out: raw moment sums in, final gradients out
     float* dL_dopacity;     // in/out
     const float* dL_dcolor;
     const InstRec* grec;    // per-Gaussian records of the forward (conic, blended opacity)
-    int blend_raw;          // dL_dmean2D.xy / dL_dconic hold raw moment sums (blend_bwd v2)
     int W, H;
     float* dL_dmean3D;
     float* dL_dcov3D;

@@ -655,25 +655,23 @@ __device__ __forceinline__ void geom_bwd_body(const PreprocessBwdParams& a_, con
 #pragma unroll
         for (int i = 0; i < 6; ++i) c3[i] = a.cov3D[6 * idx + i];
 
-        // blend_bwd v2 leaves moment sums of w = G dL/dalpha about the mean: W10, W01 in dL_dmean2D.xy,
+        // The blend backward leaves moment sums of w = G dL/dalpha about the mean: W10, W01 in dL_dmean2D.xy,
         // W20, W11, W02 in dL_dconic.  Their per-Gaussian linear map to the reference's gradients
         // (backward.cu:1119-1134: dG/ddel = -G (A dx + B dy), ddelx/dx = W/2, dL/dconic = -0.5 G d d^T dL/dG,
         // dL/dG = opacity dL/dalpha) is applied here, once, instead of per (pixel, Gaussian) pair.
         float d2x = a.dL_dmean2D[3 * idx + 0], d2y = a.dL_dmean2D[3 * idx + 1];
         float dcx = a.dL_dconic[4 * idx + 0], dcy = a.dL_dconic[4 * idx + 1], dcz = a.dL_dconic[4 * idx + 3];
-        if (a.blend_raw) {
-            const float4 con = a.grec[idx].q1;   // A, B, C, blended opacity
-            const float W10 = d2x, W01 = d2y;
-            d2x = -0.5f * (float)a.W * con.w * (con.x * W10 + con.y * W01);
-            d2y = -0.5f * (float)a.H * con.w * (con.z * W01 + con.y * W10);
-            const float hs = -0.5f * con.w;
-            dcx *= hs; dcy *= hs; dcz *= hs;
-            a.dL_dmean2D[3 * idx + 0] = d2x;
-            a.dL_dmean2D[3 * idx + 1] = d2y;
-            a.dL_dconic[4 * idx + 0] = dcx;
-            a.dL_dconic[4 * idx + 1] = dcy;
-            a.dL_dconic[4 * idx + 3] = dcz;
-        }
+        const float4 con = a.grec[idx].q1;   // A, B, C, blended opacity
+        const float W10 = d2x, W01 = d2y;
+        d2x = -0.5f * (float)a.W * con.w * (con.x * W10 + con.y * W01);
+        d2y = -0.5f * (float)a.H * con.w * (con.z * W01 + con.y * W10);
+        const float hs = -0.5f * con.w;
+        dcx *= hs; dcy *= hs; dcz *= hs;
+        a.dL_dmean2D[3 * idx + 0] = d2x;
+        a.dL_dmean2D[3 * idx + 1] = d2y;
+        a.dL_dconic[4 * idx + 0] = dcx;
+        a.dL_dconic[4 * idx + 1] = dcy;
+        a.dL_dconic[4 * idx + 3] = dcz;
 
         // ---------------- computeCov2DCUDA, backward.cu:486-617 ----------------
         {
@@ -758,7 +756,7 @@ __device__ __forceinline__ void geom_bwd_body(const PreprocessBwdParams& a_, con
             auto scale_in = [&](const float* sp, int i) { const float v = sp[i]; return raw ? act_exp(v) : v; };
             auto quat_in = [&](const float* qp) {
                 const float4 q = reinterpret_cast<const float4*>(qp)[idx];
-                return raw ? act_normalize(q, a.quat_norm_mode) : q;
+                return raw ? act_normalize(q) : q;
             };
             if (a.rot_4d) {
                 // backward.cu:689-834
@@ -851,11 +849,11 @@ __device__ __forceinline__ void geom_bwd_body(const PreprocessBwdParams& a_, con
                 for (int i = 0; i < 3; ++i) g_scale[i] *= act_exp(a.scales[3 * idx + i]);
                 if (a.scales_t) g_scale_t *= act_exp(a.scales_t[idx]);
                 const float4 gq = act_normalize_bwd(reinterpret_cast<const float4*>(a.rotations)[idx],
-                                                    make_float4(g_rot[0], g_rot[1], g_rot[2], g_rot[3]), a.quat_norm_mode);
+                                                    make_float4(g_rot[0], g_rot[1], g_rot[2], g_rot[3]));
                 g_rot[0] = gq.x; g_rot[1] = gq.y; g_rot[2] = gq.z; g_rot[3] = gq.w;
                 if (a.rot_4d) {
                     const float4 gr = act_normalize_bwd(reinterpret_cast<const float4*>(a.rotations_r)[idx],
-                                                        make_float4(g_rotr[0], g_rotr[1], g_rotr[2], g_rotr[3]), a.quat_norm_mode);
+                                                        make_float4(g_rotr[0], g_rotr[1], g_rotr[2], g_rotr[3]));
                     g_rotr[0] = gr.x; g_rotr[1] = gr.y; g_rotr[2] = gr.z; g_rotr[3] = gr.w;
                 }
             }

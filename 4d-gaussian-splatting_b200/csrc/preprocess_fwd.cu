@@ -255,7 +255,7 @@ __device__ __forceinline__ void preprocess_fwd_body(const PreprocessFwdParams& a
         auto scale_in = [&](const float* sp, int i) { const float v = sp[i]; return raw ? act_exp(v) : v; };
         auto quat_in = [&](const float* qp) {
             const float4 q = reinterpret_cast<const float4*>(qp)[idx];
-            return raw ? act_normalize(q, a.quat_norm_mode) : q;
+            return raw ? act_normalize(q) : q;
         };
         bool alive = true;
         float c3[6];
@@ -559,19 +559,19 @@ __global__ void __launch_bounds__(PRE_THREADS, 5) preprocess_fwd_batch_kernel(co
 // test hook: the in-kernel activations of the raw-parameter entry, applied to plain arrays (tests compare them with
 // torch.exp / torch.sigmoid / F.normalize bit for bit)
 __global__ void debug_activate_kernel(int n, const float* __restrict__ log_s, const float* __restrict__ logit,
-                                      const float* __restrict__ quat, int mode, float* __restrict__ s_out,
+                                      const float* __restrict__ quat, float* __restrict__ s_out,
                                       float* __restrict__ o_out, float* __restrict__ q_out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     s_out[i] = act_exp(log_s[i]);
     o_out[i] = act_sigmoid(logit[i]);
-    reinterpret_cast<float4*>(q_out)[i] = act_normalize(reinterpret_cast<const float4*>(quat)[i], mode);
+    reinterpret_cast<float4*>(q_out)[i] = act_normalize(reinterpret_cast<const float4*>(quat)[i]);
 }
 
-cudaError_t launch_debug_activate(int n, const float* log_s, const float* logit, const float* quat, int mode, float* s_out,
-                                  float* o_out, float* q_out, cudaStream_t stream) {
+cudaError_t launch_debug_activate(int n, const float* log_s, const float* logit, const float* quat, float* s_out, float* o_out,
+                                  float* q_out, cudaStream_t stream) {
     if (n <= 0) return cudaSuccess;
-    debug_activate_kernel<<<(n + 255) / 256, 256, 0, stream>>>(n, log_s, logit, quat, mode, s_out, o_out, q_out);
+    debug_activate_kernel<<<(n + 255) / 256, 256, 0, stream>>>(n, log_s, logit, quat, s_out, o_out, q_out);
     return cudaGetLastError();
 }
 

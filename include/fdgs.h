@@ -569,7 +569,8 @@ int fdgs_debug_export_binning_view(const char* image_buffer, int width, int heig
                                    unsigned int* ranges, unsigned int* n_contrib, void* stream);
 
 /* Test hook of the raw-parameter entry: applies the in-kernel activations to plain arrays of n elements (log_s, logit:
- * [n]; quat: [n,4]; mode = quaternion-norm summation order, 0 = the library's default). */
+ * [n]; quat: [n,4]).  mode must be 0, ATen's summation order of the quaternion norm, the only one the library has;
+ * any other value returns FDGS_ERR_INVALID_ARG. */
 int fdgs_debug_activate(int n, const float* log_s, const float* logit, const float* quat, int mode, float* s_out,
                         float* o_out, float* q_out, void* stream);
 

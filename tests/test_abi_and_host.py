@@ -45,6 +45,16 @@ def test_c_abi_rejects_null_arguments_without_touching_the_gpu():
     assert lib.fdgs_backward(None, None) == 1
 
 
+def test_debug_activate_rejects_other_norm_orders_without_touching_the_gpu():
+    # the library has one summation order of the quaternion norm (ATen's, mode 0); the exported signature keeps the argument
+    import fdgs
+    lib = fdgs.lib()
+    lib.fdgs_debug_activate.restype = ctypes.c_int
+    buf = [(ctypes.c_float * 4)() for _ in range(6)]
+    assert lib.fdgs_debug_activate(1, *buf[:3], 1, *buf[3:], None) == 1   # FDGS_ERR_INVALID_ARG
+    assert b"mode" in lib.fdgs_last_error()
+
+
 def test_extension_module_mirrors_reference_entry_points():
     import fdgs
     C = fdgs.ext()

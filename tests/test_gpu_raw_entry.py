@@ -22,6 +22,24 @@ def _render_and_backward(model, cam, pipe, G, aux=None):
     return pkg
 
 
+
+def test_activations_bit_identical_to_torch():
+    """The kernels' exp / sigmoid / quaternion normalisation (fdgs_common.cuh: act_exp, act_sigmoid, act_normalize) give
+    torch.exp / torch.sigmoid / F.normalize word for word, so the raw entry activates exactly what the getters would."""
+    import fdgs
+    g = torch.Generator().manual_seed(1)
+    n = 1 << 20
+    log_s = (torch.randn(n, generator=g) * 1.5 - 4.0).to(DEV)
+    logit = (torch.randn(n, generator=g) * 3.0).to(DEV)
+    quat = torch.randn(n, 4, generator=g) * (0.2 + 2 * torch.rand(n, 1, generator=g))
+    quat[0] = 0.0   # a zero quaternion: F.normalize divides by the 1e-12 floor
+    quat = quat.to(DEV)
+    s, o, q = fdgs.ext().debug_activate(log_s, logit, quat, 0)
+    for name, got, want in (("exp", s, torch.exp(log_s)), ("sigmoid", o, torch.sigmoid(logit)),
+                            ("normalize", q, torch.nn.functional.normalize(quat))):
+        differing = int((got.view(torch.int32) != want.view(torch.int32)).sum())
+        assert differing == 0, (name, differing)
+
 @pytest.mark.parametrize("name,aux", [("small", False), ("rotcam", True), ("dur10", False), ("smod2", False), ("dim3", False),
                                       ("norot4d", False), ("deg1m4", False), ("mid", False)])
 def test_fused_prologue_matches_getter_path(name, aux):

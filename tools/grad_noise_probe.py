@@ -1,5 +1,5 @@
 """Error of our gradients against the mean of K reference reruns, in units of the reference's own run-to-run spread.
-usage: python tools/grad_noise_probe.py <config> [aux|colour]   (env: FDGS_TILE_CULL, FDGS_BLEND_BWD_V1)"""
+usage: python tools/grad_noise_probe.py <config> [aux|colour]   (env: FDGS_TILE_CULL)"""
 import os
 import sys
 
@@ -23,8 +23,8 @@ fw = C.rasterize_gaussians(*helpers.fwd_args(st, sc, cfg))
 rf = ref.rasterize_gaussians(*helpers.fwd_args(st, sc, cfg))
 ours = [C.rasterize_gaussians_backward(*helpers.bwd_args(st, sc, cfg, fw, up if aux else (gc, e, e, e))) for _ in range(3)]
 runs = [ref.rasterize_gaussians_backward(*helpers.bwd_args(st, sc, cfg, rf, up)) for _ in range(K)]
-print("%s %s tile_cull=%s v1=%s R=%d (ref %d)" % (name, "aux" if aux else "colour", os.environ.get("FDGS_TILE_CULL", "1"),
-                                                   os.environ.get("FDGS_BLEND_BWD_V1"), fw[0], rf[0]))
+print("%s %s tile_cull=%s R=%d (ref %d)" % (name, "aux" if aux else "colour", os.environ.get("FDGS_TILE_CULL", "1"),
+                                            fw[0], rf[0]))
 for k, g in enumerate(helpers.GRAD_NAMES):
     if runs[0][k].numel() == 0:
         continue
