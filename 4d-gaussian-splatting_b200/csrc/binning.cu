@@ -149,6 +149,17 @@ __global__ void __launch_bounds__(BIN_THREADS) bin_pass_batch_kernel(int P, int 
     bin_pass_body<SCATTER, SMEM, true>(P, chunk, binrec, grid_x, num_tiles, matrix, tile_offset, keys);
 }
 
+// the capacity entry (fdgs_forward_batch_capacity): info[3] != 0 -- the instances do not fit the binning buffer, or their
+// total wraps the 32-bit offsets -- and no key is written (tile_scan_body<true> has emptied every tile's range)
+template <bool SMEM>
+__global__ void __launch_bounds__(BIN_THREADS) bin_scatter_cap_kernel(int P, int chunk, const uint4* __restrict__ binrec, int grid_x,
+                                                                      int num_tiles, uint32_t* __restrict__ matrix,
+                                                                      const uint32_t* __restrict__ tile_offset,
+                                                                      uint64_t* __restrict__ keys, const uint32_t* __restrict__ info) {
+    if (info[3] != 0u) return;
+    bin_pass_body<true, SMEM, true>(P, chunk, binrec, grid_x, num_tiles, matrix, tile_offset, keys);
+}
+
 // ---- 2. offsets ------------------------------------------------------------------------------------
 // 32 tiles x 8 row groups per CTA: every thread owns <= ceil(rows / 8) consecutive rows of one tile column
 // (kept in registers), the groups' partial sums are combined through shared memory.  Coalesced along tiles.
@@ -188,9 +199,12 @@ __global__ void __launch_bounds__(256) column_scan_kernel(int num_tiles, int row
     if (grp == 0) tile_total[t] = total;
 }
 
-__global__ void __launch_bounds__(SCAN_THREADS) tile_scan_kernel(int num_tiles, const uint32_t* __restrict__ tile_total,
-                                                                 uint32_t* __restrict__ tile_offset,
-                                                                 uint2* __restrict__ ranges, uint32_t* __restrict__ info) {
+// CAP (the capacity entry): also status = {R, largest tile, R > capacity, wrap} and info[3] = overflow or wrap; on either,
+// every tile's range is emptied afterwards, so the views render as if no Gaussian were listed
+template <bool CAP>
+__device__ __forceinline__ void tile_scan_body(int num_tiles, const uint32_t* __restrict__ tile_total,
+                                               uint32_t* __restrict__ tile_offset, uint2* __restrict__ ranges,
+                                               uint32_t* __restrict__ info, int capacity, int* __restrict__ status) {
     __shared__ uint32_t warp_sums[SCAN_THREADS / 32];
     __shared__ uint32_t carry;
     __shared__ uint32_t max_count;
@@ -238,6 +252,33 @@ __global__ void __launch_bounds__(SCAN_THREADS) tile_scan_kernel(int num_tiles, 
     __syncthreads();
     // info[2] != 0: more than 2^31 - 1 instances -- the 32-bit offsets / the int num_rendered of the API cannot hold it
     if (tid == 0) { info[0] = carry; info[1] = max_count; info[2] = (total64 > 0x7fffffffull) ? 1u : 0u; info[3] = 0u; }
+    if (CAP) {
+        if (tid == 0) {
+            const bool wrap = total64 > 0x7fffffffull, over = total64 > (unsigned long long)capacity;
+            status[0] = (int)min(total64, 0x7fffffffull);
+            status[1] = (int)max_count;
+            status[2] = over ? 1 : 0;
+            status[3] = wrap ? 1 : 0;
+            info[3] = (over || wrap) ? 1u : 0u;
+            warp_sums[0] = (over || wrap) ? 1u : 0u;   // the scan is done with it
+        }
+        __syncthreads();
+        if (warp_sums[0] != 0u)
+            for (int t = tid; t < num_tiles; t += SCAN_THREADS) ranges[t] = make_uint2(0u, 0u);
+    }
+}
+
+__global__ void __launch_bounds__(SCAN_THREADS) tile_scan_kernel(int num_tiles, const uint32_t* __restrict__ tile_total,
+                                                                 uint32_t* __restrict__ tile_offset,
+                                                                 uint2* __restrict__ ranges, uint32_t* __restrict__ info) {
+    tile_scan_body<false>(num_tiles, tile_total, tile_offset, ranges, info, 0, nullptr);
+}
+
+__global__ void __launch_bounds__(SCAN_THREADS) tile_scan_cap_kernel(int num_tiles, const uint32_t* __restrict__ tile_total,
+                                                                     uint32_t* __restrict__ tile_offset,
+                                                                     uint2* __restrict__ ranges, uint32_t* __restrict__ info,
+                                                                     int capacity, int* __restrict__ status) {
+    tile_scan_body<true>(num_tiles, tile_total, tile_offset, ranges, info, capacity, status);
 }
 
 // ---- 4. per-tile sort ------------------------------------------------------------------------------------
@@ -445,6 +486,22 @@ __global__ void __launch_bounds__(LARGE ? SORT_LARGE_THREADS : SORT_SMALL_THREAD
     tile_sort_body<LARGE, true>(ranges, keys, point_list, grec, recs, tiles_per_view, P);
 }
 
+// The capacity entry's per-view table from device arrays; the focal lengths are rounded as the host computes them for
+// fdgs_forward_batch (W / (2 tan), IEEE division), so both entries see bit-identical tables
+__global__ void view_table_kernel(int B, int W, int H, const float* __restrict__ timestamps, const float* __restrict__ tan_fovx,
+                                  const float* __restrict__ tan_fovy, ViewScalars* __restrict__ out) {
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= B) return;
+    ViewScalars s;
+    s.timestamp = timestamps[v];
+    s.tan_fovx = tan_fovx[v];
+    s.tan_fovy = tan_fovy[v];
+    s.focal_y = __fdiv_rn((float)H, __fmul_rn(2.0f, s.tan_fovy));
+    s.focal_x = __fdiv_rn((float)W, __fmul_rn(2.0f, s.tan_fovx));
+    s.pad[0] = s.pad[1] = s.pad[2] = 0.f;
+    out[v] = s;
+}
+
 // test hook: unpack the per-Gaussian records into the reference's plain arrays; `radii` is any
 // per-Gaussian int array that is > 0 exactly for the rendered Gaussians (radii or tiles_touched)
 __global__ void unpack_grec_kernel(int P, const InstRec* __restrict__ grec, const int* __restrict__ radii,
@@ -512,14 +569,34 @@ cudaError_t launch_bin_count(int P, const uint4* binrec, int grid_x, int grid_y,
 }
 
 cudaError_t launch_tile_scan(int num_tiles, uint32_t* matrix, uint32_t* tile_total, uint32_t* tile_offset, uint2* ranges,
-                             uint32_t* info, cudaStream_t stream) {
+                             uint32_t* info, cudaStream_t stream, int capacity, int* status) {
     column_scan_kernel<<<(num_tiles + 31) / 32, 256, 0, stream>>>(num_tiles, bin_cta_count(), matrix, tile_total);
-    tile_scan_kernel<<<1, SCAN_THREADS, 0, stream>>>(num_tiles, tile_total, tile_offset, ranges, info);
+    if (status) tile_scan_cap_kernel<<<1, SCAN_THREADS, 0, stream>>>(num_tiles, tile_total, tile_offset, ranges, info, capacity, status);
+    else tile_scan_kernel<<<1, SCAN_THREADS, 0, stream>>>(num_tiles, tile_total, tile_offset, ranges, info);
     return cudaGetLastError();
 }
 
 cudaError_t launch_bin_scatter(int P, const uint4* binrec, int grid_x, int grid_y, uint32_t* matrix,
-                               const uint32_t* tile_offset, uint64_t* keys, const ViewBatch& vb, cudaStream_t stream) {
+                               const uint32_t* tile_offset, uint64_t* keys, const ViewBatch& vb, cudaStream_t stream,
+                               const uint32_t* info) {
+    if (info) {
+        if (P <= 0) return cudaSuccess;
+        const int num_tiles = grid_x * grid_y, ctas = bin_cta_count();
+        const int chunk = (((P + ctas - 1) / ctas) + 31) & ~31;
+        const size_t smem = (size_t)num_tiles * sizeof(uint32_t);
+        const dim3 grid(ctas, vb.B);
+        if (smem <= BIN_SMEM_LIMIT) {
+            static PerDeviceOnce once;
+            cudaError_t e = ensure_dynamic_smem(bin_scatter_cap_kernel<true>, (int)BIN_SMEM_LIMIT, once);
+            if (e != cudaSuccess) return e;
+            bin_scatter_cap_kernel<true><<<grid, BIN_THREADS, smem, stream>>>(P, chunk, binrec, grid_x, num_tiles, matrix,
+                                                                             tile_offset, keys, info);
+        } else {
+            bin_scatter_cap_kernel<false><<<grid, BIN_THREADS, 0, stream>>>(P, chunk, binrec, grid_x, num_tiles, matrix,
+                                                                           tile_offset, keys, info);
+        }
+        return cudaGetLastError();
+    }
     if (vb.scalars) return launch_bin_pass<true, true>(P, vb.B, binrec, grid_x, grid_y, matrix, tile_offset, keys, stream);
     return launch_bin_pass<true, false>(P, 1, binrec, grid_x, grid_y, matrix, tile_offset, keys, stream);
 }
@@ -550,6 +627,12 @@ cudaError_t launch_tile_sort_pack(int num_tiles, int max_count, int R, const uin
     if (vb.scalars)
         return tile_sort_pack<true>(num_tiles, max_count, ranges, keys, grec, recs, point_list, num_tiles / vb.B, P, stream);
     return tile_sort_pack<false>(num_tiles, max_count, ranges, keys, grec, recs, point_list, 0, 0, stream);
+}
+
+cudaError_t launch_view_table(int B, int W, int H, const float* timestamps, const float* tan_fovx, const float* tan_fovy,
+                              ViewScalars* out, cudaStream_t stream) {
+    view_table_kernel<<<(B + 127) / 128, 128, 0, stream>>>(B, W, H, timestamps, tan_fovx, tan_fovy, out);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_unpack_grec(int P, const InstRec* grec, const int* radii, float* depths, float* means2D,

@@ -4,6 +4,7 @@
 // CudaRasterizer::Rasterizer::forward / backward / markVisible
 // (reference: rasterizer_impl.cu:199-364, :368-496, :142-154) and the GeometryState /
 // ImageState / BinningState chunk carving (rasterizer_impl.cu:156-195, rasterizer_impl.h:21-73).
+#include <limits.h>
 #include <math.h>
 #include <string.h>
 #include <atomic>
@@ -48,13 +49,19 @@ const bool g_trace = getenv("FDGS_TRACE") != nullptr;
 // (include/fdgs.h: fdgs_set_tile_cull)
 std::atomic<int> g_tile_cull{getenv("FDGS_TILE_CULL") ? atoi(getenv("FDGS_TILE_CULL")) : 1};
 
+bool stream_capturing(cudaStream_t s) {
+    cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+    return cudaStreamIsCapturing(s, &st) == cudaSuccess && st != cudaStreamCaptureStatusNone;
+}
+
 struct StageTimer {
     cudaEvent_t a = nullptr, b = nullptr;
     int stage;
     cudaStream_t stream;
     StageTimer(int stage_, cudaStream_t s, const char* name) : stage(stage_), stream(s) {
         nvtxRangePushA(name);   // one NVTX range per pipeline stage (nsys / ncu --nvtx)
-        if (g_prof_on) {
+        // a captured stage would record its events into the graph, not time this call
+        if (g_prof_on && !stream_capturing(stream)) {
             cudaEventCreate(&a);
             cudaEventCreate(&b);
             cudaEventRecord(a, stream);
@@ -302,16 +309,37 @@ int check_forward_args(const fdgs_forward_args* a) {
     return FDGS_OK;
 }
 
+// The capacity entry's sizing (fdgs_forward_batch_capacity): the binning buffer holds `capacity` instances and the
+// device status word reports the true count
+struct CapacityMode {
+    int capacity;
+    int* status;
+};
+
 // The forward's stages on the carved geometry and image buffers, for one view (vb = {1, NULL}) or for the batched
-// entry's B views (vb = {B, the uploaded view table}: every per-view array is then a [B] stack, and the camera tables and
-// scalars are the views').  Allocates the binning buffer after the one host synchronisation.
+// entry's B views (vb = {B, the view table}: every per-view array is then a [B] stack, and the camera tables and
+// scalars are the views').  Allocates the binning buffer after the one host synchronisation, or, with cap (a batch), at
+// cap->capacity instances before the first launch, and then does not synchronise.
 // zero_sh / zero_sh_rest (single view): the SH gradient rows the blend zeroes (fdgs_forward_zero_sh), or NULL.
 int forward_stages(const fdgs_forward_args* a, const float* bg_image, float* zero_sh, float* zero_sh_rest,
                    const fdgs::ViewBatch& vb, const GeomState& geom, const ImageState& img, fdgs_alloc_fn binning_alloc,
-                   void* binning_ctx, cudaStream_t stream, fdgs_forward_result* res) {
+                   void* binning_ctx, cudaStream_t stream, fdgs_forward_result* res, const CapacityMode* cap = nullptr) {
     const bool debug = a->debug != 0, batch = vb.scalars != nullptr;
     const int P = a->P, W = a->width, H = a->height;
     const int grid_x = (W + fdgs::TILE_X - 1) / fdgs::TILE_X, grid_y = (H + fdgs::TILE_Y - 1) / fdgs::TILE_Y;
+    BinningState bin;
+    auto alloc_binning = [&](int R) {
+        const size_t bin_bytes = fdgs_binning_bytes(R, W, H);
+        char* bin_raw = binning_alloc(binning_ctx, bin_bytes);
+        if (!bin_raw) return fail(FDGS_ERR_ALLOC, "binning buffer allocation failed");
+        bin = BinningState::carve(align128(bin_raw), R);
+        res->binning_buffer = bin_raw;
+        res->binning_bytes = bin_bytes;
+        res->num_rendered = R;
+        return (int)FDGS_OK;
+    };
+    if (cap)
+        if (int rc = alloc_binning(cap->capacity)) return rc;
     if (P > 0) {
         fdgs::PreprocessFwdParams pp;
         memset(&pp, 0, sizeof(pp));
@@ -344,33 +372,35 @@ int forward_stages(const fdgs_forward_args* a, const float* bg_image, float* zer
                    cudaError_t e = fdgs::launch_bin_count(P, geom.binrec, grid_x, grid_y, img.bin_matrix, vb, stream);
                    if (e != cudaSuccess) return e;
                    return fdgs::launch_tile_scan((int)img.tiles, img.bin_matrix, img.tile_total, img.tile_offset, img.ranges,
-                                                 img.bin_info, stream);
+                                                 img.bin_info, stream, cap ? cap->capacity : 0, cap ? cap->status : nullptr);
                }(),
                batch ? "bin_count + tile_scan (batch)" : "bin_count + tile_scan");
-    // the one host synchronisation of the forward (reference: rasterizer_impl.cu:302): R over all views, the largest
-    // tile of any view, the overflow flag
-    int bin_info[4] = {0, 0, 0, 0};
-    FDGS_CUDA(cudaMemcpyAsync(bin_info, img.bin_info, sizeof(bin_info), cudaMemcpyDeviceToHost, stream), "num_rendered copy");
-    FDGS_CUDA(cudaStreamSynchronize(stream), "num_rendered sync");
-    const int num_rendered = bin_info[0];
-    // bin_info[2]: the 64-bit total computed on the device exceeded 2^31 - 1 (a wrapped 32-bit total would look valid)
-    if (num_rendered < 0 || bin_info[2] != 0) return fail(FDGS_ERR_UNSUPPORTED, "more than 2^31 - 1 tile instances");
-    res->num_rendered = num_rendered;
-
-    const size_t bin_bytes = fdgs_binning_bytes(num_rendered, W, H);
-    char* bin_raw = binning_alloc(binning_ctx, bin_bytes);
-    if (!bin_raw) return fail(FDGS_ERR_ALLOC, "binning buffer allocation failed");
-    BinningState bin = BinningState::carve(align128(bin_raw), num_rendered);
-    res->binning_buffer = bin_raw;
-    res->binning_bytes = bin_bytes;
+    int num_rendered = 0, max_count = 0;
+    if (cap) {
+        // sized by the capacity: an overflow is handled on the device (no key written, every range empty), and only
+        // the device knows the largest tile, so both size classes of the tile sort run
+        num_rendered = cap->capacity;
+        max_count = INT_MAX;
+    } else {
+        // the one host synchronisation of the forward (reference: rasterizer_impl.cu:302): R over all views, the largest
+        // tile of any view, the overflow flag
+        int bin_info[4] = {0, 0, 0, 0};
+        FDGS_CUDA(cudaMemcpyAsync(bin_info, img.bin_info, sizeof(bin_info), cudaMemcpyDeviceToHost, stream), "num_rendered copy");
+        FDGS_CUDA(cudaStreamSynchronize(stream), "num_rendered sync");
+        num_rendered = bin_info[0];
+        max_count = bin_info[1];
+        // bin_info[2]: the 64-bit total computed on the device exceeded 2^31 - 1 (a wrapped 32-bit total would look valid)
+        if (num_rendered < 0 || bin_info[2] != 0) return fail(FDGS_ERR_UNSUPPORTED, "more than 2^31 - 1 tile instances");
+        if (int rc = alloc_binning(num_rendered)) return rc;
+    }
 
     if (num_rendered > 0) {
         FDGS_STAGE(2, 1,
                    fdgs::launch_bin_scatter(P, geom.binrec, grid_x, grid_y, img.bin_matrix, img.tile_offset, bin.keys, vb,
-                                            stream),
+                                            stream, cap ? img.bin_info : nullptr),
                    batch ? "bin_scatter (batch)" : "bin_scatter");
-        FDGS_STAGE(3, fdgs::tile_sort_pack_kernel_count(bin_info[1]),
-                   fdgs::launch_tile_sort_pack((int)img.tiles, bin_info[1], num_rendered, img.ranges, bin.keys, geom.grec, P,
+        FDGS_STAGE(3, fdgs::tile_sort_pack_kernel_count(max_count),
+                   fdgs::launch_tile_sort_pack((int)img.tiles, max_count, num_rendered, img.ranges, bin.keys, geom.grec, P,
                                                bin.recs, bin.point_list, vb, stream),
                    batch ? "tile_sort_pack (batch)" : "tile_sort_pack");
     }
@@ -526,15 +556,24 @@ int check_batch_views(int B, const float* bg_image, int bg_views) {
     return FDGS_OK;
 }
 
-int forward_batch_impl(const fdgs_forward_batch_args* b, fdgs_alloc_fn geom_alloc, void* geom_ctx, fdgs_alloc_fn binning_alloc,
-                       void* binning_ctx, fdgs_alloc_fn image_alloc, void* image_ctx, void* stream_v, fdgs_forward_result* res) {
+// cap: the capacity entry's arguments (b is then &cap->batch), or NULL for fdgs_forward_batch
+int forward_batch_impl(const fdgs_forward_batch_args* b, const fdgs_forward_capacity_args* cap, fdgs_alloc_fn geom_alloc,
+                       void* geom_ctx, fdgs_alloc_fn binning_alloc, void* binning_ctx, fdgs_alloc_fn image_alloc, void* image_ctx,
+                       void* stream_v, fdgs_forward_result* res) {
     g_last_error.clear();
     if (!b || !res || !geom_alloc || !binning_alloc || !image_alloc) return fail(FDGS_ERR_INVALID_ARG, "null argument");
     memset(res, 0, sizeof(*res));
     const fdgs_forward_args* a = &b->view;
     const int B = b->B;
+    if (cap) {
+        if (!cap->status) return fail(FDGS_ERR_INVALID_ARG, "the device status word must be set");
+        if (cap->capacity < 0) return fail(FDGS_ERR_INVALID_ARG, "capacity must be >= 0");
+    }
     if (int rc = check_batch_views(B, b->bg_image, b->bg_views)) return rc;
-    if (!a->viewmatrix || !a->projmatrix || !a->cam_pos || !b->timestamps || !b->tan_fovx || !b->tan_fovy)
+    // the capacity entry takes the per-view scalars from device arrays, fdgs_forward_batch from host arrays
+    const bool have_scalars = cap ? (cap->timestamps && cap->tan_fovx && cap->tan_fovy)
+                                  : (b->timestamps && b->tan_fovx && b->tan_fovy);
+    if (!a->viewmatrix || !a->projmatrix || !a->cam_pos || !have_scalars)
         return fail(FDGS_ERR_INVALID_ARG, "the per-view camera table (viewmatrix / projmatrix / cam_pos / timestamps / tan_fovx / "
                                           "tan_fovy) must be set");
     if (int rc = check_forward_args(a)) return rc;
@@ -545,6 +584,12 @@ int forward_batch_impl(const fdgs_forward_batch_args* b, fdgs_alloc_fn geom_allo
     const int grid_x = (W + fdgs::TILE_X - 1) / fdgs::TILE_X, grid_y = (H + fdgs::TILE_Y - 1) / fdgs::TILE_Y;
     if ((long long)grid_x * grid_y * B > 0x7fffffffLL || (long long)P * B > 0x7fffffffLL)
         return fail(FDGS_ERR_UNSUPPORTED, "B * tiles or B * P exceeds 2^31 - 1");
+    if (cap && a->debug) {
+        cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+        FDGS_CUDA(cudaStreamIsCapturing(stream, &st), "capture status query");
+        if (st != cudaStreamCaptureStatusNone)
+            return fail(FDGS_ERR_INVALID_ARG, "debug synchronises after every stage: not allowed while the stream is capturing");
+    }
 
     const size_t geom_bytes = fdgs_geom_batch_bytes(P, B);
     char* geom_raw = geom_alloc(geom_ctx, geom_bytes);
@@ -560,6 +605,14 @@ int forward_batch_impl(const fdgs_forward_batch_args* b, fdgs_alloc_fn geom_allo
     res->image_bytes = img_bytes;
     res->cov3D = geom.cov3D;
 
+    if (cap) {
+        const CapacityMode mode = {cap->capacity, cap->status};
+        FDGS_CUDA(fdgs::launch_view_table(B, W, H, cap->timestamps, cap->tan_fovx, cap->tan_fovy, geom.scalars, stream),
+                  "view table");
+        g_kernel_launches += 1;
+        return forward_stages(a, b->bg_image, nullptr, nullptr, {B, geom.scalars}, geom, img, binning_alloc, binning_ctx, stream,
+                              res, &mode);
+    }
     // the per-view scalars, focal lengths computed as the single-view entry computes them (reference: rasterizer_impl.cu:235-236);
     // a pageable host-to-device copy is staged before the call returns and does not synchronise
     std::vector<fdgs::ViewScalars> vs((size_t)B);
@@ -706,7 +759,14 @@ int fdgs_backward_zero_sh(const fdgs_backward_args* a, const float* bg_image, fl
 int fdgs_forward_batch(const fdgs_forward_batch_args* args, fdgs_alloc_fn geom_alloc, void* geom_ctx,
                        fdgs_alloc_fn binning_alloc, void* binning_ctx, fdgs_alloc_fn image_alloc, void* image_ctx, void* stream,
                        fdgs_forward_result* res) {
-    return forward_batch_impl(args, geom_alloc, geom_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, stream, res);
+    return forward_batch_impl(args, nullptr, geom_alloc, geom_ctx, binning_alloc, binning_ctx, image_alloc, image_ctx, stream, res);
+}
+
+int fdgs_forward_batch_capacity(const fdgs_forward_capacity_args* args, fdgs_alloc_fn geom_alloc, void* geom_ctx,
+                                fdgs_alloc_fn binning_alloc, void* binning_ctx, fdgs_alloc_fn image_alloc, void* image_ctx,
+                                void* stream, fdgs_forward_result* res) {
+    return forward_batch_impl(args ? &args->batch : nullptr, args, geom_alloc, geom_ctx, binning_alloc, binning_ctx, image_alloc,
+                              image_ctx, stream, res);
 }
 
 int fdgs_backward_batch(const fdgs_backward_batch_args* args, void* stream) { return backward_batch_impl(args, stream); }

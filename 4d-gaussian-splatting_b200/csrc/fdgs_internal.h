@@ -32,7 +32,8 @@ int device_sm_count();
 
 // ---- batched views (fdgs_forward_batch / fdgs_backward_batch) --------------------------------------------------
 // The per-view scalars of a batch, one 32-byte row per view in device memory (uploaded by the forward into the geometry
-// buffer).  focal_x / focal_y are computed on the host exactly as the single-view entry computes them.
+// buffer, or filled there by launch_view_table for the capacity entry).  focal_x / focal_y are computed exactly as the
+// single-view entry computes them.
 struct ViewScalars {
     float timestamp, tan_fovx, tan_fovy, focal_x, focal_y, pad[3];
 };
@@ -99,11 +100,18 @@ int bin_ctas();                                 // rows of the [bin_ctas()][num_
 // tiles are the columns v * tiles .. v * tiles + tiles - 1
 cudaError_t launch_bin_count(int P, const uint4* binrec, int grid_x, int grid_y, uint32_t* matrix, const ViewBatch& vb,
                              cudaStream_t stream);
-// matrix -> per-CTA column prefixes; tile_offset / ranges; info[0] = total instances R, info[1] = largest tile
+// matrix -> per-CTA column prefixes; tile_offset / ranges; info[0] = total instances R, info[1] = largest tile.
+// status != NULL (the capacity entry): also status[4] = {R, largest tile, R > capacity, wrap} and info[3] = overflow or
+// wrap, in which case every tile's range is left empty
 cudaError_t launch_tile_scan(int num_tiles, uint32_t* matrix, uint32_t* tile_total, uint32_t* tile_offset, uint2* ranges,
-                             uint32_t* info, cudaStream_t stream);
+                             uint32_t* info, cudaStream_t stream, int capacity = 0, int* status = nullptr);
+// info != NULL (the capacity entry, a batch): the tile_scan's info; the pass writes no key when info[3] != 0
 cudaError_t launch_bin_scatter(int P, const uint4* binrec, int grid_x, int grid_y, uint32_t* matrix,
-                               const uint32_t* tile_offset, uint64_t* keys, const ViewBatch& vb, cudaStream_t stream);
+                               const uint32_t* tile_offset, uint64_t* keys, const ViewBatch& vb, cudaStream_t stream,
+                               const uint32_t* info = nullptr);
+// the capacity entry's view table from device [B] arrays, focal lengths as the host computes them
+cudaError_t launch_view_table(int B, int W, int H, const float* timestamps, const float* tan_fovx, const float* tan_fovy,
+                              ViewScalars* out, cudaStream_t stream);
 // sorts every tile's keys and writes the 64-byte instance records + the sorted index list.  A batch: num_tiles =
 // vb.B * tiles per view, and every tile gathers from the slice of its view in grec, a [vb.B][P] stack
 int tile_sort_pack_kernel_count(int max_count);

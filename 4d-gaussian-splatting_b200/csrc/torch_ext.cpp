@@ -20,6 +20,9 @@
 //
 //   rasterize_gaussians_batch / rasterize_gaussians_backward_batch
 //
+// and the batched forward sized by an instance capacity, which never synchronises (include/fdgs.h:
+// fdgs_forward_batch_capacity): rasterize_gaussians_batch_capacity
+//
 // PyTorch is plumbing only: it owns the memory (tensors, the three growable byte buffers handed
 // to the library through the allocation callback) and supplies the current CUDA stream.  No
 // arithmetic happens here.  Differences from the reference shim, all performance-motivated and
@@ -444,8 +447,8 @@ RasterizeGaussiansBackwardCUDA(const torch::Tensor& background, const torch::Ten
 
 // ---- batched views (include/fdgs.h: fdgs_forward_batch / fdgs_backward_batch) ---------------------------------------
 // The cameras are strict: viewmatrix / projmatrix [B,16] (or [B,4,4]) and campos [B,3] float32 CUDA tensors on the
-// Gaussians' device, timestamps / tanfovx / tanfovy [B] float32 CPU tensors; bg_image empty or [B,3,H,W].  Checked before
-// anything is allocated or launched.
+// Gaussians' device, timestamps / tanfovx / tanfovy [B] float32 CPU tensors (CUDA tensors on that device for the capacity
+// entry: device_scalars); bg_image empty or [B,3,H,W].  Checked before anything is allocated or launched.
 namespace {
 struct BatchCams {
     int B;
@@ -454,7 +457,7 @@ struct BatchCams {
 
 BatchCams batch_cameras(const torch::Tensor& means3D, const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix,
                         const torch::Tensor& campos, const torch::Tensor& timestamps, const torch::Tensor& tanfovx,
-                        const torch::Tensor& tanfovy) {
+                        const torch::Tensor& tanfovy, bool device_scalars = false) {
     TORCH_CHECK(viewmatrix.defined() && viewmatrix.dim() >= 1, "fdgs: viewmatrix must be [B,16]");
     BatchCams c;
     const int64_t B = viewmatrix.size(0);
@@ -466,10 +469,18 @@ BatchCams batch_cameras(const torch::Tensor& means3D, const torch::Tensor& viewm
     c.timestamps = arg<float>(timestamps, "timestamps", B, B, REQUIRED);
     c.tanfovx = arg<float>(tanfovx, "tanfovx", B, B, REQUIRED);
     c.tanfovy = arg<float>(tanfovy, "tanfovy", B, B, REQUIRED);
-    TORCH_CHECK(!timestamps.is_cuda() && !tanfovx.is_cuda() && !tanfovy.is_cuda(),
-                "fdgs: timestamps / tanfovx / tanfovy must be CPU tensors");
+    if (device_scalars) {
+        TORCH_CHECK(timestamps.is_cuda() && tanfovx.is_cuda() && tanfovy.is_cuda(),
+                    "fdgs: timestamps / tanfovx / tanfovy must be CUDA tensors");
+    } else {
+        TORCH_CHECK(!timestamps.is_cuda() && !tanfovx.is_cuda() && !tanfovy.is_cuda(),
+                    "fdgs: timestamps / tanfovx / tanfovy must be CPU tensors");
+    }
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor");
-    same_cuda_device("batched camera", {means3D, viewmatrix, projmatrix, campos});
+    if (device_scalars)
+        same_cuda_device("batched camera", {means3D, viewmatrix, projmatrix, campos, timestamps, tanfovx, tanfovy});
+    else
+        same_cuda_device("batched camera", {means3D, viewmatrix, projmatrix, campos});
     return c;
 }
 
@@ -487,20 +498,24 @@ const float* batch_bg_image(const torch::Tensor& bg_image, const torch::Tensor& 
 // B views of the same Gaussians: (num_rendered, color [B,3,H,W], flow [B,2,H,W], depth [B,1,H,W], T [B,1,H,W],
 // radii [B,P], geomBuffer, binningBuffer, imgBuffer, out_means3D [B,P,3]).  Gaussian inputs as in rasterize_gaussians_ext
 // (SH and scales / rotations only: no precomputed colours or covariances).
-std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor,
-           torch::Tensor, torch::Tensor>
-RasterizeGaussiansBatch(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& flows,
-                        const torch::Tensor& opacity, const torch::Tensor& ts, const torch::Tensor& scales,
-                        const torch::Tensor& scales_t, const torch::Tensor& rotations, const torch::Tensor& rotations_r,
-                        const float scale_modifier, const float prefilter_var, const torch::Tensor& viewmatrix,
-                        const torch::Tensor& projmatrix, const torch::Tensor& campos, const torch::Tensor& timestamps,
-                        const torch::Tensor& tanfovx, const torch::Tensor& tanfovy, const int image_height,
-                        const int image_width, const torch::Tensor& sh, const torch::Tensor& sh_rest, const int degree,
-                        const int degree_t, const float time_duration, const bool rot_4d, const int gaussian_dim,
-                        const bool force_sh_3d, const bool prefiltered, const bool debug, const bool raw_params,
-                        const torch::Tensor& bg_image) {
+namespace {
+using BatchForwardOut = std::tuple<int, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor,
+                                   torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>;
+
+// capacity < 0: fdgs_forward_batch; else fdgs_forward_batch_capacity, which writes `status` (int32 [4] on the device)
+BatchForwardOut batch_forward(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& flows,
+                              const torch::Tensor& opacity, const torch::Tensor& ts, const torch::Tensor& scales,
+                              const torch::Tensor& scales_t, const torch::Tensor& rotations, const torch::Tensor& rotations_r,
+                              const float scale_modifier, const float prefilter_var, const torch::Tensor& viewmatrix,
+                              const torch::Tensor& projmatrix, const torch::Tensor& campos, const torch::Tensor& timestamps,
+                              const torch::Tensor& tanfovx, const torch::Tensor& tanfovy, const int image_height,
+                              const int image_width, const torch::Tensor& sh, const torch::Tensor& sh_rest, const int degree,
+                              const int degree_t, const float time_duration, const bool rot_4d, const int gaussian_dim,
+                              const bool force_sh_3d, const bool prefiltered, const bool debug, const bool raw_params,
+                              const torch::Tensor& bg_image, int64_t capacity, torch::Tensor* status) {
     TORCH_CHECK(means3D.dim() == 2 && means3D.size(1) == 3, "means3D must have dimensions (num_points, 3)");
-    const BatchCams cams = batch_cameras(means3D, viewmatrix, projmatrix, campos, timestamps, tanfovx, tanfovy);
+    const bool cap = capacity >= 0;
+    const BatchCams cams = batch_cameras(means3D, viewmatrix, projmatrix, campos, timestamps, tanfovx, tanfovy, cap);
     const int B = cams.B, P = means3D.size(0), H = image_height, W = image_width;
     TORCH_CHECK(H > 0 && W > 0, "fdgs: bad image size");
     const float* bgi = batch_bg_image(bg_image, means3D, B, H, W);
@@ -526,13 +541,71 @@ RasterizeGaussiansBatch(const torch::Tensor& background, const torch::Tensor& me
     a.out_means3D = out_means3D.data_ptr<float>(); a.out_color = out_color.data_ptr<float>();
     a.out_flow = out_flow.data_ptr<float>(); a.out_depth = out_depth.data_ptr<float>();
     a.out_T = out_T.data_ptr<float>(); a.radii = radii.data_ptr<int>();
-    b.B = B; b.timestamps = cams.timestamps; b.tan_fovx = cams.tanfovx; b.tan_fovy = cams.tanfovy;
-    b.bg_image = bgi; b.bg_views = bgi ? B : 0;
+    b.B = B; b.bg_image = bgi; b.bg_views = bgi ? B : 0;
     fdgs_forward_result r;
-    check(fdgs_forward_batch(&b, resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer, (void*)on.stream, &r),
-          "forward_batch");
+    if (cap) {
+        *status = torch::empty({4}, means3D.options().dtype(torch::kInt32));
+        fdgs_forward_capacity_args c;
+        memset(&c, 0, sizeof(c));
+        c.batch = b;
+        c.timestamps = cams.timestamps; c.tan_fovx = cams.tanfovx; c.tan_fovy = cams.tanfovy;
+        c.capacity = (int)capacity; c.status = status->data_ptr<int>();
+        check(fdgs_forward_batch_capacity(&c, resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer,
+                                          (void*)on.stream, &r),
+              "forward_batch_capacity");
+    } else {
+        b.timestamps = cams.timestamps; b.tan_fovx = cams.tanfovx; b.tan_fovy = cams.tanfovy;
+        check(fdgs_forward_batch(&b, resize_cb, &geomBuffer, resize_cb, &binningBuffer, resize_cb, &imgBuffer, (void*)on.stream,
+                                 &r),
+              "forward_batch");
+    }
     return std::make_tuple(r.num_rendered, out_color, out_flow, out_depth, out_T, radii, geomBuffer, binningBuffer, imgBuffer,
                            out_means3D);
+}
+}  // namespace
+
+BatchForwardOut RasterizeGaussiansBatch(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& flows,
+                                        const torch::Tensor& opacity, const torch::Tensor& ts, const torch::Tensor& scales,
+                                        const torch::Tensor& scales_t, const torch::Tensor& rotations,
+                                        const torch::Tensor& rotations_r, const float scale_modifier, const float prefilter_var,
+                                        const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix,
+                                        const torch::Tensor& campos, const torch::Tensor& timestamps,
+                                        const torch::Tensor& tanfovx, const torch::Tensor& tanfovy, const int image_height,
+                                        const int image_width, const torch::Tensor& sh, const torch::Tensor& sh_rest,
+                                        const int degree, const int degree_t, const float time_duration, const bool rot_4d,
+                                        const int gaussian_dim, const bool force_sh_3d, const bool prefiltered, const bool debug,
+                                        const bool raw_params, const torch::Tensor& bg_image) {
+    return batch_forward(background, means3D, flows, opacity, ts, scales, scales_t, rotations, rotations_r, scale_modifier,
+                         prefilter_var, viewmatrix, projmatrix, campos, timestamps, tanfovx, tanfovy, image_height, image_width,
+                         sh, sh_rest, degree, degree_t, time_duration, rot_4d, gaussian_dim, force_sh_3d, prefiltered, debug,
+                         raw_params, bg_image, -1, nullptr);
+}
+
+// rasterize_gaussians_batch sized by `capacity` instances (include/fdgs.h: fdgs_forward_batch_capacity): the same
+// arguments, except that timestamps / tanfovx / tanfovy are float32 CUDA tensors [B] on the Gaussians' device, and the
+// same tuple with status (int32 [4] on the device: R, largest tile, overflow, wrap) in place of num_rendered.  The
+// backward is rasterize_gaussians_backward_batch with R = capacity.  No host synchronisation.
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor,
+           torch::Tensor, torch::Tensor, torch::Tensor>
+RasterizeGaussiansBatchCapacity(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& flows,
+                                const torch::Tensor& opacity, const torch::Tensor& ts, const torch::Tensor& scales,
+                                const torch::Tensor& scales_t, const torch::Tensor& rotations, const torch::Tensor& rotations_r,
+                                const float scale_modifier, const float prefilter_var, const torch::Tensor& viewmatrix,
+                                const torch::Tensor& projmatrix, const torch::Tensor& campos, const torch::Tensor& timestamps,
+                                const torch::Tensor& tanfovx, const torch::Tensor& tanfovy, const int image_height,
+                                const int image_width, const torch::Tensor& sh, const torch::Tensor& sh_rest, const int degree,
+                                const int degree_t, const float time_duration, const bool rot_4d, const int gaussian_dim,
+                                const bool force_sh_3d, const bool prefiltered, const bool debug, const bool raw_params,
+                                const torch::Tensor& bg_image, const int64_t capacity) {
+    TORCH_CHECK(capacity >= 0 && capacity <= 0x7fffffffLL, "fdgs: capacity must be in [0, 2^31 - 1]");
+    torch::Tensor status;
+    const BatchForwardOut o = batch_forward(background, means3D, flows, opacity, ts, scales, scales_t, rotations, rotations_r,
+                                            scale_modifier, prefilter_var, viewmatrix, projmatrix, campos, timestamps, tanfovx,
+                                            tanfovy, image_height, image_width, sh, sh_rest, degree, degree_t, time_duration,
+                                            rot_4d, gaussian_dim, force_sh_3d, prefiltered, debug, raw_params, bg_image,
+                                            capacity, &status);
+    return std::make_tuple(status, std::get<1>(o), std::get<2>(o), std::get<3>(o), std::get<4>(o), std::get<5>(o),
+                           std::get<6>(o), std::get<7>(o), std::get<8>(o), std::get<9>(o));
 }
 
 // Backward of rasterize_gaussians_batch.  Returns 11 tensors: dL_dmeans2D [B,P,3] per view, then the view sums
@@ -1201,6 +1274,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("rasterize_gaussians_backward_ext", &RasterizeGaussiansBackwardExtZeroSh);
     m.def("rasterize_gaussians_batch", &RasterizeGaussiansBatch);
     m.def("rasterize_gaussians_backward_batch", &RasterizeGaussiansBackwardBatch);
+    m.def("rasterize_gaussians_batch_capacity", &RasterizeGaussiansBatchCapacity);
     m.def("debug_export_binning_view", &DebugExportBinningView);
     m.def("sky_forward", &SkyForward);
     m.def("sky_backward", &SkyBackward);

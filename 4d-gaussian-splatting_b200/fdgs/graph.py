@@ -1,0 +1,174 @@
+"""The training step as one CUDA graph.
+
+At the image sizes the dnerf scenes train at (400x400, 1 to 24 views per step) a step of render_batch + loss + backward
+waits on the host -- kernel launches, Python and autograd -- more than on the GPU.  A CUDA graph replays the whole step
+with one launch, but a captured step must not synchronise and must not bake host values into the graph:
+
+  StaticViews   device tensors that hold a step's cameras; render_batch(views, ...) reads the cameras from them and
+                calls the rasterizer entry sized by an instance capacity (include/fdgs.h:
+                fdgs_forward_batch_capacity), which never synchronises.  Its "status" output reports the true instance
+                count R and whether it overflowed the capacity (the views then render as if no Gaussian were listed).
+  GraphedStep   captures a user step fn(views, gt) -> (loss, pkg) once and replays it with new cameras and ground truth;
+                it reads the status once per step, after all of the step's work is queued, and on overflow re-captures
+                with a larger capacity and replays the same inputs.
+
+The optimiser, the densification statistics and densification itself run eagerly on the graph's static outputs.
+"""
+import math
+from typing import Callable, Iterable, List, Optional
+
+import torch
+
+
+class StaticViews:
+    """B cameras of one image size in device tensors: viewmatrix / projmatrix [B,4,4], campos [B,3], timestamp /
+    tanfovx / tanfovy [B] (float32), and `capacity`, the instances the rasterizer's binning buffer holds summed over the
+    views.  render_batch(views, ...) reads whatever load() last copied in."""
+
+    def __init__(self, B: int, H: int, W: int, device):
+        if B < 1 or H < 1 or W < 1:
+            raise ValueError("StaticViews needs B, H, W >= 1, got %d, %d, %d" % (B, H, W))
+        self.B, self.H, self.W = int(B), int(H), int(W)
+        self.device = torch.device(device)
+        f = dict(dtype=torch.float32, device=self.device)
+        self.viewmatrix = torch.zeros(self.B, 4, 4, **f)
+        self.projmatrix = torch.zeros(self.B, 4, 4, **f)
+        self.campos = torch.zeros(self.B, 3, **f)
+        self._scalars = torch.zeros(3, self.B, **f)
+        self.timestamp, self.tanfovx, self.tanfovy = self._scalars.unbind(0)
+        self._host = torch.zeros(3, self.B, dtype=torch.float32, pin_memory=True)
+        self._copied: Optional[torch.cuda.Event] = None
+        self.capacity = 0
+
+    def load(self, cams) -> None:
+        """Copy the reference Cameras `cams` (B of them, this image size) into the tensors, in place, on the current
+        stream.  The scalars go through one pinned host buffer; it is rewritten only after the previous load's copy out
+        of it has completed."""
+        cams = list(cams)
+        if len(cams) != self.B:
+            raise ValueError("StaticViews holds %d views, got %d cameras" % (self.B, len(cams)))
+        for c in cams:
+            if (int(c.image_height), int(c.image_width)) != (self.H, self.W):
+                raise ValueError("StaticViews holds %dx%d views, got a %dx%d camera"
+                                 % (self.W, self.H, int(c.image_width), int(c.image_height)))
+        if self._copied is not None:
+            self._copied.synchronize()
+        # the host values render_batch computes for a camera list, rounded to float32 the same way
+        self._host.copy_(torch.tensor([[float(c.timestamp) for c in cams], [math.tan(c.FoVx * 0.5) for c in cams],
+                                       [math.tan(c.FoVy * 0.5) for c in cams]], dtype=torch.float32))
+        self._scalars.copy_(self._host, non_blocking=True)
+        self._copied = torch.cuda.Event()
+        self._copied.record()
+        for dst, name in ((self.viewmatrix, "world_view_transform"), (self.projmatrix, "full_proj_transform"),
+                          (self.campos, "camera_center")):
+            dst.copy_(torch.stack([getattr(c, name).to(self.device) for c in cams]))
+
+
+def _leaves(params) -> List[torch.Tensor]:
+    src = params() if callable(params) else params
+    opt = getattr(src, "optimizer", src)
+    if hasattr(opt, "param_groups"):
+        return [p for g in opt.param_groups for p in g["params"]]
+    return list(src)
+
+
+class GraphedStep:
+    """One training step, captured once and replayed: `step(cams, gt)` runs `fn(views, gt)` -- which calls
+    render_batch(views, ...), computes its loss and calls backward() -- and returns fn's (loss, pkg), static tensors that
+    every replay overwrites.  After the call each leaf's .grad holds the step's gradient.
+
+    params: the Gaussian model (an object with an `optimizer` whose param groups hold the leaves, and
+    `active_sh_degree` / `active_sh_degree_t`, like the reference's GaussianModel), an optimiser, a list of leaves, or a
+    callable returning one of those.  The leaves are read on every call: a new leaf (densification, pruning), a new SH
+    degree, or a new B, H or W re-captures.  margin: the capacity is margin x the instance count it is sized from.
+
+    The first call warms up eagerly on a side stream, first at capacity 0 (a background-only render whose status reports
+    the true R), then at ceil(margin R); each capture starts with every leaf's .grad set to None, so replays assign
+    the gradients rather than accumulate them.  The step's one host synchronisation reads the status after the replay;
+    on overflow the step re-captures at ceil(margin R) and replays the same inputs (the optimiser runs outside the graph,
+    so the parameters have not moved).  `info` counts captures and overflows and holds the capacity."""
+
+    def __init__(self, fn: Callable, params, margin: float = 1.25):
+        if not margin >= 1.0:
+            raise ValueError("margin must be >= 1, got %r" % (margin,))
+        self.fn, self.params, self.margin = fn, params, float(margin)
+        self.views: Optional[StaticViews] = None
+        self.gt: Optional[torch.Tensor] = None
+        self.info = {"captures": 0, "overflows": 0, "capacity": None}
+        self._graph = None
+        self._key = None
+        self._out = None
+        self._grads: List[Optional[torch.Tensor]] = []
+
+    def _sized(self, R: int) -> int:
+        return int(math.ceil(self.margin * R))
+
+    def _drop(self):
+        """Free the graph and its static outputs before another capture."""
+        self._graph, self._out, self._grads = None, None, []
+
+    def _warm_up(self, leaves):
+        side = torch.cuda.Stream(device=self.views.device)
+        side.wait_stream(torch.cuda.current_stream(self.views.device))
+        with torch.cuda.stream(side):
+            self.views.capacity = 0
+            _, pkg = self.fn(self.views, self.gt)
+            R = int(pkg["status"][0])
+            self.views.capacity = self._sized(R)
+            self.fn(self.views, self.gt)
+        torch.cuda.current_stream(self.views.device).wait_stream(side)
+        for p in leaves:
+            p.grad = None
+        self.info["capacity"] = self.views.capacity
+
+    def _capture(self, leaves):
+        self._drop()
+        for p in leaves:
+            p.grad = None
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            out = self.fn(self.views, self.gt)
+        self._graph, self._out = graph, out
+        self._grads = [p.grad for p in leaves]
+        self.info["captures"] += 1
+        self.info["capacity"] = self.views.capacity
+
+    def _replay(self, leaves):
+        self._graph.replay()
+        for p, g in zip(leaves, self._grads):
+            p.grad = g
+        status = self._out[1]["status"].tolist()
+        if status[3]:
+            raise RuntimeError("GraphedStep: more than 2^31 - 1 tile instances in one step")
+        return status
+
+    def __call__(self, cams, gt: torch.Tensor):
+        cams = list(cams)
+        if not cams:
+            raise ValueError("GraphedStep needs at least one camera")
+        B, H, W = len(cams), int(cams[0].image_height), int(cams[0].image_width)
+        if self.views is None or (self.views.B, self.views.H, self.views.W) != (B, H, W) or self.gt.shape != gt.shape:
+            capacity = self.views.capacity if self.views is not None else None
+            self._drop()
+            self.views = StaticViews(B, H, W, gt.device)
+            self.gt = torch.empty_like(gt)
+            if capacity is not None:
+                self.views.capacity = capacity
+        self.views.load(cams)
+        self.gt.copy_(gt)
+        leaves = _leaves(self.params)
+        model = self.params() if callable(self.params) else self.params
+        key = (B, H, W, tuple(p.shape[0] for p in leaves[:1]), tuple(p.data_ptr() for p in leaves),
+               getattr(model, "active_sh_degree", None), getattr(model, "active_sh_degree_t", None))
+        if self._graph is None or key != self._key:
+            if self.info["capacity"] is None:
+                self._warm_up(leaves)
+            self._capture(leaves)
+            self._key = key
+        status = self._replay(leaves)
+        if status[2]:
+            self.info["overflows"] += 1
+            self.views.capacity = self._sized(status[0])
+            self._capture(leaves)
+            status = self._replay(leaves)
+        return self._out

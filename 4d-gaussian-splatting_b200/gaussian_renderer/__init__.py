@@ -207,9 +207,18 @@ def render_batch(viewpoint_cameras, pc, pipe, bg_color: torch.Tensor, scaling_mo
     backward() per view would accumulate it.
 
     The views must share the image size; precomputed colours or covariances (override_color, compute_cov3D_python,
-    convert_SHs_python) and a call inside an active ViewParallelStep are not supported (ValueError)."""
-    cams = list(viewpoint_cameras)
-    if not cams:
+    convert_SHs_python) and a call inside an active ViewParallelStep are not supported (ValueError).
+
+    `viewpoint_cameras` may also be an fdgs.graph.StaticViews: the cameras then come from its device tensors, the
+    rasterizer is sized by its instance capacity and never synchronises with the host (the call can be captured in a CUDA
+    graph), and the result has an eighth key, "status" (int32 [4] on the device: instances R, largest tile, overflow,
+    wrap; on overflow every view renders as if no Gaussian were listed).  An environment map and pipe.debug are not
+    supported then (ValueError): the sky sampler inverts the cameras and checks its miss flag on the host, and debug
+    synchronises after every stage."""
+    from fdgs.graph import StaticViews
+    views = viewpoint_cameras if isinstance(viewpoint_cameras, StaticViews) else None
+    cams = None if views is not None else list(viewpoint_cameras)
+    if views is None and not cams:
         raise ValueError("render_batch needs at least one camera")
     if override_color is not None:
         raise ValueError("render_batch does not take override_color (precomputed colours); use render()")
@@ -220,33 +229,45 @@ def render_batch(viewpoint_cameras, pc, pipe, bg_color: torch.Tensor, scaling_mo
     from fdgs.dist import ViewParallelStep
     if ViewParallelStep.current() is not None:
         raise ValueError("render_batch cannot run inside an active ViewParallelStep; render its views with render()")
-    H, W = int(cams[0].image_height), int(cams[0].image_width)
-    for c in cams[1:]:
-        if (int(c.image_height), int(c.image_width)) != (H, W):
-            raise ValueError("render_batch views must share the image size: %dx%d and %dx%d"
-                             % (W, H, int(c.image_width), int(c.image_height)))
+    env_map_res = getattr(pipe, "env_map_res", 0)
+    if views is not None:
+        if env_map_res:
+            raise ValueError("render_batch with StaticViews does not support an environment map (its sampler synchronises)")
+        if pipe.debug:
+            raise ValueError("render_batch with StaticViews does not support pipe.debug (it synchronises after every stage)")
+        B, H, W = views.B, views.H, views.W
+    else:
+        B, H, W = len(cams), int(cams[0].image_height), int(cams[0].image_width)
+        for c in cams[1:]:
+            if (int(c.image_height), int(c.image_width)) != (H, W):
+                raise ValueError("render_batch views must share the image size: %dx%d and %dx%d"
+                                 % (W, H, int(c.image_width), int(c.image_height)))
 
     xyz = pc.get_xyz
     dev = xyz.device
-    B, P = len(cams), xyz.shape[0]
+    P = xyz.shape[0]
     screenspace_points = torch.zeros((B, P, 3), dtype=xyz.dtype, requires_grad=True, device=dev) + 0
     screenspace_points.retain_grad()
 
-    env_map_res = getattr(pipe, "env_map_res", 0)
+    if views is not None:
+        cameras = dict(tanfovx=views.tanfovx, tanfovy=views.tanfovy, viewmatrix=views.viewmatrix,
+                       projmatrix=views.projmatrix, campos=views.campos, timestamp=views.timestamp)
+    else:
+        cameras = dict(tanfovx=tuple(math.tan(c.FoVx * 0.5) for c in cams),
+                       tanfovy=tuple(math.tan(c.FoVy * 0.5) for c in cams),
+                       viewmatrix=torch.stack([c.world_view_transform for c in cams]),
+                       projmatrix=torch.stack([c.full_proj_transform for c in cams]),
+                       campos=torch.stack([c.camera_center for c in cams]),
+                       timestamp=tuple(float(c.timestamp) for c in cams))
     settings = BatchRasterizationSettings(
         image_height=H, image_width=W,
-        tanfovx=tuple(math.tan(c.FoVx * 0.5) for c in cams),
-        tanfovy=tuple(math.tan(c.FoVy * 0.5) for c in cams),
         bg=bg_color if not env_map_res else torch.zeros(3, device=dev),
         scale_modifier=scaling_modifier,
-        viewmatrix=torch.stack([c.world_view_transform for c in cams]),
-        projmatrix=torch.stack([c.full_proj_transform for c in cams]),
         sh_degree=pc.active_sh_degree, sh_degree_t=pc.active_sh_degree_t,
-        campos=torch.stack([c.camera_center for c in cams]),
-        timestamp=tuple(float(c.timestamp) for c in cams),
         time_duration=pc.time_duration[1] - pc.time_duration[0],
         rot_4d=pc.rot_4d, gaussian_dim=pc.gaussian_dim, force_sh_3d=pc.force_sh_3d,
-        prefiltered=False, debug=pipe.debug)
+        prefiltered=False, debug=pipe.debug, **cameras)
+    capacity = None if views is None else views.capacity
 
     sky = None
     misses = []
@@ -261,19 +282,25 @@ def render_batch(viewpoint_cameras, pc, pipe, bg_color: torch.Tensor, scaling_mo
 
     four_d = pc.gaussian_dim == 4
     if _fused_prologue_ok(pc, pipe, None):
-        color, radii, depth, alpha, flow = rasterize_gaussians_batch(
+        out = rasterize_gaussians_batch(
             xyz, screenspace_points, pc._opacity, pc._features_dc, pc._scaling, pc._rotation, settings,
             sh_rest=pc._features_rest if pc._features_rest.numel() else None, flow_2d=torch.zeros_like(xyz[:, :2]),
             ts=pc._t if four_d else None, scales_t=pc._scaling_t if four_d else None,
             rotations_r=pc._rotation_r if pc.rot_4d else None,
-            prefilter_var=pc.prefilter_var if (four_d and pc.prefilter_var > 0.0) else -1.0, raw=True, bg_image=sky)
+            prefilter_var=pc.prefilter_var if (four_d and pc.prefilter_var > 0.0) else -1.0, raw=True, bg_image=sky,
+            capacity=capacity)
     else:
-        color, radii, depth, alpha, flow = rasterize_gaussians_batch(
+        out = rasterize_gaussians_batch(
             xyz, screenspace_points, pc.get_opacity, pc.get_features, pc.get_scaling, pc.get_rotation, settings,
             flow_2d=torch.zeros_like(xyz[:, :2]), ts=pc.get_t if four_d else None,
             scales_t=pc.get_scaling_t if four_d else None, rotations_r=pc.get_rotation_r if pc.rot_4d else None,
-            prefilter_var=pc.prefilter_var if (four_d and pc.prefilter_var > 0.0) else -1.0, bg_image=sky)
+            prefilter_var=pc.prefilter_var if (four_d and pc.prefilter_var > 0.0) else -1.0, bg_image=sky,
+            capacity=capacity)
     for miss in misses:
         miss.check()
-    return {"render": color, "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii,
-            "depth": depth, "alpha": alpha, "flow": flow}
+    color, radii, depth, alpha, flow = out[:5]
+    pkg = {"render": color, "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii,
+           "depth": depth, "alpha": alpha, "flow": flow}
+    if views is not None:
+        pkg["status"] = out[5]
+    return pkg

@@ -308,35 +308,56 @@ class _RasterizeGaussiansBatch(torch.autograd.Function):
     order: means3D, means2D [B,P,3], sh, sh_rest, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
     prefilter_var, settings (BatchRasterizationSettings), raw, bg_image ([B,3,H,W] or None).  raw and sh / sh_rest as in
     _RasterizeGaussians.  Returns color [B,3,H,W], radii [B,P], depth [B,1,H,W], alpha [B,1,H,W], flow [B,2,H,W].
-    Every per-Gaussian gradient is the sum of the views' gradients in view order; means2D's gradient stays per view."""
+    Every per-Gaussian gradient is the sum of the views' gradients in view order; means2D's gradient stays per view.
+
+    capacity (an int >= 0) selects the entry sized by an instance capacity (_C.rasterize_gaussians_batch_capacity), which
+    never synchronises with the host and can be captured in a CUDA graph: settings.timestamp / tanfovx / tanfovy are then
+    float32 CUDA tensors [B], and a sixth output, status (int32 [4] on the device: R, largest tile, overflow, wrap),
+    follows the five images.  On overflow the views render as if no Gaussian were listed, and the gradients are zero."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, sh_rest, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
-                prefilter_var, settings, raw, bg_image):
+                prefilter_var, settings, raw, bg_image, capacity=None):
         s = settings
-        cams = (s.viewmatrix, s.projmatrix, s.campos) + tuple(
-            torch.tensor(list(v), dtype=torch.float32) for v in (s.timestamp, s.tanfovx, s.tanfovy))
+        if capacity is None:
+            cams = (s.viewmatrix, s.projmatrix, s.campos) + tuple(
+                torch.tensor(list(v), dtype=torch.float32) for v in (s.timestamp, s.tanfovx, s.tanfovy))
+        else:
+            cams = (s.viewmatrix, s.projmatrix, s.campos, s.timestamp, s.tanfovx, s.tanfovy)
         args = (s.bg, means3D, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r, s.scale_modifier,
                 prefilter_var) + cams + (s.image_height, s.image_width, sh, sh_rest, s.sh_degree, s.sh_degree_t,
                                          s.time_duration, s.rot_4d, s.gaussian_dim, s.force_sh_3d, s.prefiltered, s.debug,
                                          raw, _NONE if bg_image is None else bg_image)
-        (num_rendered, color, flow, depth, T, radii, geom_buf, binning_buf, img_buf,
-         out_means3D) = _invoke(_C.rasterize_gaussians_batch, args, s.debug, "snapshot_fw.dump")
+        if capacity is None:
+            (num_rendered, color, flow, depth, T, radii, geom_buf, binning_buf, img_buf,
+             out_means3D) = _invoke(_C.rasterize_gaussians_batch, args, s.debug, "snapshot_fw.dump")
+        else:
+            (status, color, flow, depth, T, radii, geom_buf, binning_buf, img_buf,
+             out_means3D) = _invoke(_C.rasterize_gaussians_batch_capacity, args + (int(capacity),), s.debug,
+                                    "snapshot_fw.dump")
+            # the backward reads the per-view scalars from the forward's geometry buffer; its binding still takes host
+            # tables of the right shape
+            cams = cams[:3] + (_host_placeholder(int(s.viewmatrix.shape[0])),) * 3
+            num_rendered = int(capacity)
         ctx.cams = cams
         ctx.settings = s
         ctx.raw = raw
         ctx.bg_image = bg_image
         ctx.num_rendered = num_rendered
+        ctx.capacity = capacity is not None
         ctx.prefilter_var = prefilter_var
         ctx.save_for_backward(means3D, out_means3D, radii, sh, sh_rest, flow_2d, opacities, ts, scales, scales_t,
                               rotations, rotations_r, geom_buf, binning_buf, img_buf)
         ctx.mark_non_differentiable(radii)
         ctx.set_materialize_grads(False)
         ctx.image_shape = tuple(color.shape)
-        return color, radii, depth, 1 - T, flow
+        if capacity is None:
+            return color, radii, depth, 1 - T, flow
+        ctx.mark_non_differentiable(status)
+        return color, radii, depth, 1 - T, flow, status
 
     @staticmethod
-    def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha, grad_flow):
+    def backward(ctx, grad_color, grad_radii, grad_depth, grad_alpha, grad_flow, grad_status=None):
         s = ctx.settings
         (means3D, out_means3D, radii, sh, sh_rest, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
          geom_buf, binning_buf, img_buf) = ctx.saved_tensors
@@ -360,14 +381,29 @@ class _RasterizeGaussiansBatch(torch.autograd.Function):
 
         return (g_means3D, g_means2D, g_sh, for_input(g_sh_rest, sh_rest), None, g_opacities, for_input(g_ts, ts),
                 g_scales, for_input(g_scales_t, scales_t), g_rot, for_input(g_rot_r, rotations_r), None, None, None,
-                g_bg if want_bg else None)
+                g_bg if want_bg else None) + ((None,) if ctx.capacity else ())
+
+
+_HOST_PLACEHOLDERS = {}
+
+
+def _host_placeholder(B):
+    """A float32 CPU tensor [B], built once per B: what the backward binding's host camera tables are given in capacity
+    mode (the values are not read)."""
+    t = _HOST_PLACEHOLDERS.get(B)
+    if t is None:
+        t = _HOST_PLACEHOLDERS[B] = torch.zeros(B, dtype=torch.float32)
+    return t
 
 
 def rasterize_gaussians_batch(means3D, means2D, opacities, sh, scales, rotations, settings, sh_rest=None, flow_2d=None,
-                              ts=None, scales_t=None, rotations_r=None, prefilter_var=-1.0, raw=False, bg_image=None):
+                              ts=None, scales_t=None, rotations_r=None, prefilter_var=-1.0, raw=False, bg_image=None,
+                              capacity=None):
     """Rasterize B views of the same Gaussians in one call (see _RasterizeGaussiansBatch).  raw: the inputs are the
     optimiser's raw parameters (forward_raw's convention: sh = features_dc, sh_rest = features_rest).  bg_image: per-view
-    background images [B,3,H,W] behind the Gaussians, or None."""
+    background images [B,3,H,W] behind the Gaussians, or None.  capacity: None, or the instance capacity of the entry
+    that does not synchronise (the per-view scalars of `settings` are then CUDA tensors [B] and a sixth output, the
+    device status, is returned)."""
     B = int(settings.viewmatrix.shape[0])
     P = int(means3D.shape[0])
     if tuple(means2D.shape) != (B, P, 3):
@@ -385,6 +421,10 @@ def rasterize_gaussians_batch(means3D, means2D, opacities, sh, scales, rotations
     def opt(t):
         return _NONE if t is None else t
 
+    if capacity is None:
+        return _RasterizeGaussiansBatch.apply(means3D, means2D, sh, opt(sh_rest), opt(flow_2d), opacities, opt(ts), scales,
+                                              opt(scales_t), rotations, opt(rotations_r), prefilter_var, settings, raw,
+                                              bg_image)
     return _RasterizeGaussiansBatch.apply(means3D, means2D, sh, opt(sh_rest), opt(flow_2d), opacities, opt(ts), scales,
                                           opt(scales_t), rotations, opt(rotations_r), prefilter_var, settings, raw,
-                                          bg_image)
+                                          bg_image, int(capacity))

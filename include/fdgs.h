@@ -290,6 +290,33 @@ int fdgs_forward_batch(const fdgs_forward_batch_args* args,
                        fdgs_forward_result* result);
 int fdgs_backward_batch(const fdgs_backward_batch_args* args, void* stream);
 
+/* The batched forward sized by an instance capacity instead of the exact count: no host synchronisation, no read of
+ * device memory on the host and no upload of host data, so the call can be captured in a CUDA graph and replayed with
+ * new cameras.  `batch` as in fdgs_forward_batch, except that its host timestamps / tan_fovx / tan_fovy are ignored: the
+ * per-view scalars come from the device arrays below.  The binning buffer is requested once, before the first launch,
+ * at fdgs_binning_bytes(capacity, W, H) bytes, and result->num_rendered is set to `capacity`.
+ *
+ * status (device int[4]) receives {R, largest tile, overflow = R > capacity, wrap = R > 2^31 - 1}; R saturates at
+ * 2^31 - 1.  Without overflow or wrap every output is bit-identical to fdgs_forward_batch's.  With either, the views
+ * render as if no Gaussian were listed: the colour is the background (with bg_image: background + bg_image, as for an
+ * empty tile), depth, flow, alpha and n_contrib are 0, radii and out_means3D are still the preprocess's; no write falls
+ * outside the binning buffer.  The backward is fdgs_backward_batch with R = capacity; after an overflow it returns zero
+ * per-Gaussian gradients.  debug != 0 is rejected while `stream` is capturing (debug synchronises after every stage). */
+typedef struct fdgs_forward_capacity_args {
+    fdgs_forward_batch_args batch;
+    const float* timestamps;   /* device [B] */
+    const float* tan_fovx;     /* device [B] */
+    const float* tan_fovy;     /* device [B] */
+    int capacity;              /* instances the binning buffer holds, summed over the B views */
+    int* status;               /* device int[4] */
+} fdgs_forward_capacity_args;
+int fdgs_forward_batch_capacity(const fdgs_forward_capacity_args* args,
+                                fdgs_alloc_fn geom_alloc, void* geom_ctx,
+                                fdgs_alloc_fn binning_alloc, void* binning_ctx,
+                                fdgs_alloc_fn image_alloc, void* image_ctx,
+                                void* stream,
+                                fdgs_forward_result* result);
+
 /* Environment-map sky sphere (the reference's sky for scenes with an environment map: gaussian_renderer/__init__.py
  * and Camera.get_rays).  Each pixel's ray -- the pixel centre ((x + 0.5 - cx) / fl_x, (y + 0.5 - cy) / fl_y, 1, 1)
  * through c2w, minus campos, normalised -- is intersected with the sphere |X| = radius; the hit point gives
@@ -590,7 +617,8 @@ int fdgs_set_tile_cull(int mode);
  * (it times whole iterations from Python, train.py:57-58,89,185). */
 #define FDGS_NUM_STAGES 8
 /* stage ids: 0 preprocess_fwd, 1 scan, 2 emit_keys, 3 sort, 4 pack_instances, 5 blend_fwd,
- *            6 blend_bwd, 7 preprocess_bwd */
+ *            6 blend_bwd, 7 preprocess_bwd
+ * Stages launched on a stream that is capturing a CUDA graph record no events. */
 int fdgs_profile_enable(int on);
 /* Synchronises the recorded events, adds up the milliseconds and call counts per stage since the
  * last read, then resets the accumulators. */
