@@ -947,6 +947,13 @@ int fdgs_reset_opacity(long long P, float* opacity, float* exp_avg, float* exp_a
 int fdgs_densify_stats(long long P, int batch_size, const float* point_grad, int point_grad_stride, const float* visibility_count,
                        const int* radii, const float* t_grad, float* xyz_gradient_accum, float* denom, float* t_gradient_accum,
                        float* max_radii2D, void* stream_v) {
+    return fdgs_densify_stats_status(P, batch_size, point_grad, point_grad_stride, visibility_count, radii, t_grad,
+                                     xyz_gradient_accum, denom, t_gradient_accum, max_radii2D, nullptr, stream_v);
+}
+
+int fdgs_densify_stats_status(long long P, int batch_size, const float* point_grad, int point_grad_stride,
+                              const float* visibility_count, const int* radii, const float* t_grad, float* xyz_gradient_accum,
+                              float* denom, float* t_gradient_accum, float* max_radii2D, const int* status, void* stream_v) {
     g_last_error.clear();
     if (P < 0 || batch_size < 1) return fail(FDGS_ERR_INVALID_ARG, "bad P / batch size");
     if (batch_size == 1 ? point_grad_stride < 2 : point_grad_stride != 1) return fail(FDGS_ERR_INVALID_ARG, "bad gradient row stride");
@@ -955,7 +962,7 @@ int fdgs_densify_stats(long long P, int batch_size, const float* point_grad, int
         return fail(FDGS_ERR_INVALID_ARG, "null argument");
     if (!t_grad != !t_gradient_accum) return fail(FDGS_ERR_INVALID_ARG, "t_grad and t_gradient_accum go together");
     FDGS_CUDA(fdgs::launch_densify_stats(P, batch_size, point_grad, point_grad_stride, visibility_count, radii, t_grad,
-                                         xyz_gradient_accum, denom, t_gradient_accum, max_radii2D,
+                                         xyz_gradient_accum, denom, t_gradient_accum, max_radii2D, status,
                                          reinterpret_cast<cudaStream_t>(stream_v)), "densify_stats");
     g_kernel_launches += 1;
     return FDGS_OK;
@@ -995,6 +1002,26 @@ int fdgs_l1_ssim_backward(const float* x, const float* y, int C, int H, int W, c
     return FDGS_OK;
 }
 
+int fdgs_adam_scalars(int n, const float* lrs, const long long* steps, const int* enable, double beta1, double beta2,
+                      float* table) {
+    g_last_error.clear();
+    if (n < 0 || n > FDGS_MAX_PACK) return fail(FDGS_ERR_INVALID_ARG, "bad tensor count");
+    if (n == 0) return FDGS_OK;
+    if (!lrs || !steps || !enable || !table) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    for (int i = 0; i < n; ++i)
+        if (enable[i] && steps[i] < 1) return fail(FDGS_ERR_INVALID_ARG, "bad step count");
+    for (int i = 0; i < n; ++i) {
+        table[3 * i] = 0.f; table[3 * i + 1] = 1.f; table[3 * i + 2] = 0.f;
+        if (!enable[i]) continue;
+        // bias corrections in double on the host, like torch.optim.Adam's single-tensor path
+        const double bc1 = 1.0 - pow(beta1, (double)steps[i]), bc2 = 1.0 - pow(beta2, (double)steps[i]);
+        table[3 * i] = (float)((double)lrs[i] / bc1);
+        table[3 * i + 1] = (float)sqrt(bc2);
+        table[3 * i + 2] = 1.f;
+    }
+    return FDGS_OK;
+}
+
 int fdgs_adam_step(int n, float* const* params, float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,
                    const int* widths, const float* lrs, long long P, const long long* rows, long long num_rows, long long step,
                    double beta1, double beta2, double eps, int zero_grad, void* stream_v) {
@@ -1003,17 +1030,35 @@ int fdgs_adam_step(int n, float* const* params, float* const* grads, float* cons
         return fail(FDGS_ERR_INVALID_ARG, "bad tensor count / row count / step");
     if (n == 0 || P == 0 || (rows && num_rows == 0)) return FDGS_OK;
     if (!params || !grads || !exp_avg || !exp_avg_sq || !widths || !lrs) return fail(FDGS_ERR_INVALID_ARG, "null argument");
-    float step_sizes[FDGS_MAX_PACK];
-    // bias corrections in double on the host, like torch.optim.Adam's single-tensor path
-    const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
-    for (int i = 0; i < n; ++i) {
+    for (int i = 0; i < n; ++i)
         if (!params[i] || !grads[i] || !exp_avg[i] || !exp_avg_sq[i] || widths[i] <= 0)
             return fail(FDGS_ERR_INVALID_ARG, "bad tensor table entry");
-        step_sizes[i] = (float)((double)lrs[i] / bc1);
-    }
+    long long steps[FDGS_MAX_PACK];
+    int enable[FDGS_MAX_PACK];
+    float table[3 * FDGS_MAX_PACK], step_sizes[FDGS_MAX_PACK];
+    for (int i = 0; i < n; ++i) { steps[i] = step; enable[i] = 1; }
+    fdgs_adam_scalars(n, lrs, steps, enable, beta1, beta2, table);
+    for (int i = 0; i < n; ++i) step_sizes[i] = table[3 * i];
     FDGS_CUDA(fdgs::launch_adam(n, params, grads, exp_avg, exp_avg_sq, widths, step_sizes, rows ? num_rows : P, rows, (float)(1.0 - beta1),
-                                (float)beta2, (float)(1.0 - beta2), (float)eps, (float)sqrt(bc2), zero_grad, reinterpret_cast<cudaStream_t>(stream_v)),
+                                (float)beta2, (float)(1.0 - beta2), (float)eps, table[1], zero_grad, reinterpret_cast<cudaStream_t>(stream_v)),
               "adam_step");
+    g_kernel_launches += 1;
+    return FDGS_OK;
+}
+
+int fdgs_adam_step_staged(int n, float* const* params, float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,
+                          const int* widths, long long P, const float* scalars, const int* status, double beta1, double beta2,
+                          double eps, void* stream_v) {
+    g_last_error.clear();
+    if (n < 0 || n > FDGS_MAX_PACK || P < 0) return fail(FDGS_ERR_INVALID_ARG, "bad tensor count / row count");
+    if (n == 0 || P == 0) return FDGS_OK;
+    if (!params || !grads || !exp_avg || !exp_avg_sq || !widths || !scalars) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    for (int i = 0; i < n; ++i)
+        if (!params[i] || !grads[i] || !exp_avg[i] || !exp_avg_sq[i] || widths[i] <= 0)
+            return fail(FDGS_ERR_INVALID_ARG, "bad tensor table entry");
+    FDGS_CUDA(fdgs::launch_adam_staged(n, params, grads, exp_avg, exp_avg_sq, widths, P, scalars, status, (float)(1.0 - beta1),
+                                       (float)beta2, (float)(1.0 - beta2), (float)eps, reinterpret_cast<cudaStream_t>(stream_v)),
+              "adam_step_staged");
     g_kernel_launches += 1;
     return FDGS_OK;
 }

@@ -282,6 +282,10 @@ cudaError_t launch_l1_ssim_bwd(const float* x, const float* y, int C, int H, int
 cudaError_t launch_adam(int n, float* const* params, float* const* grads, float* const* m, float* const* v, const int* widths,
                         const float* step_sizes, long long rows, const long long* row_idx, float w1, float beta2, float w2,
                         float eps, float sqrt_bc2, int zero_grad, cudaStream_t stream);
+// dense, per-tensor lr / bc1, sqrt(bc2) and enable flag from the device table `scalars`; nothing on a status overflow
+cudaError_t launch_adam_staged(int n, float* const* params, float* const* grads, float* const* m, float* const* v,
+                               const int* widths, long long rows, const float* scalars, const int* status, float w1,
+                               float beta2, float w2, float eps, cudaStream_t stream);
 // uniform-grid k nearest neighbours: knn.cu
 size_t knn_scratch_bytes(int n);
 cudaError_t launch_knn(int n, int k, const float* xyz, char* scratch, int* idx, float* dist2, cudaStream_t stream);
@@ -324,7 +328,7 @@ cudaError_t launch_densify_apply(const fdgs_densify_args& a, const char* scratch
 cudaError_t launch_reset_opacity(long long P, float* opacity, float* m, float* v, cudaStream_t stream);
 cudaError_t launch_densify_stats(long long P, int B, const float* pgrad, int stride, const float* vis, const int* radii,
                                  const float* tgrad, float* accum, float* denom, float* taccum, float* max_radii2D,
-                                 cudaStream_t stream);
+                                 const int* status, cudaStream_t stream);
 
 // ---- environment-map sky (sky.cu) ------------------------------------------------------------------
 struct SkyParams {

@@ -992,6 +992,53 @@ void AdamStep(std::vector<torch::Tensor> params, std::vector<torch::Tensor> grad
           "adam_step");
 }
 
+// Adam's per-tensor scalars for a staged step (include/fdgs.h: fdgs_adam_scalars), written into `table`, a CPU float32
+// tensor of 3 n elements (a pinned staging buffer): lr / bc1, sqrt(bc2), enable.
+void AdamScalars(std::vector<double> lrs, std::vector<int64_t> steps, std::vector<int64_t> enable, const double beta1,
+                 const double beta2, torch::Tensor& table) {
+    const size_t n = lrs.size();
+    TORCH_CHECK(n <= FDGS_MAX_PACK && steps.size() == n && enable.size() == n, "fdgs: adam_scalars table mismatch");
+    TORCH_CHECK(table.defined() && !table.is_cuda(), "fdgs: adam_scalars writes a host table");
+    float* out = arg<float>(table, "adam scalar table", -1, 3 * (int64_t)n, REQUIRED);
+    std::vector<float> lr(n);
+    std::vector<long long> st(n);
+    std::vector<int> en(n);
+    for (size_t i = 0; i < n; ++i) { lr[i] = (float)lrs[i]; st[i] = steps[i]; en[i] = enable[i] != 0; }
+    check(fdgs_adam_scalars((int)n, lr.data(), st.data(), en.data(), beta1, beta2, out), "adam_scalars");
+}
+
+// Dense Adam with the scalars read on the device (include/fdgs.h: fdgs_adam_step_staged): scalars = CUDA float32 [3 n]
+// as adam_scalars fills it, status = the rasterizer's int32 [4] or empty.  Capturable in a CUDA graph.
+void AdamStepStaged(std::vector<torch::Tensor> params, std::vector<torch::Tensor> grads, std::vector<torch::Tensor> exp_avg,
+                    std::vector<torch::Tensor> exp_avg_sq, const torch::Tensor& scalars, const torch::Tensor& status,
+                    const double beta1, const double beta2, const double eps) {
+    const size_t n = params.size();
+    TORCH_CHECK(n <= FDGS_MAX_PACK && grads.size() == n && exp_avg.size() == n && exp_avg_sq.size() == n,
+                "fdgs: adam_step_staged table mismatch");
+    if (n == 0) return;
+    const long long P = params[0].size(0);
+    std::vector<float*> p, g, m, v;
+    std::vector<int> widths;
+    for (size_t i = 0; i < n; ++i) {
+        const int64_t numel = params[i].numel();
+        p.push_back(arg<float>(params[i], "adam tensor", P, numel, REQUIRED));
+        g.push_back(arg<float>(grads[i], "adam tensor", P, numel, REQUIRED));
+        m.push_back(arg<float>(exp_avg[i], "adam tensor", P, numel, REQUIRED));
+        v.push_back(arg<float>(exp_avg_sq[i], "adam tensor", P, numel, REQUIRED));
+        widths.push_back(P > 0 ? (int)(numel / P) : 1);
+    }
+    const float* sc = arg<float>(scalars, "adam scalar table", -1, 3 * (int64_t)n, REQUIRED);
+    const int* st = arg<int>(status, "status", -1, 4);
+    std::vector<torch::Tensor> dev;
+    for (size_t i = 0; i < n; ++i) dev.insert(dev.end(), {params[i], grads[i], exp_avg[i], exp_avg_sq[i]});
+    dev.insert(dev.end(), {scalars, status});
+    same_cuda_device("adam", dev);
+    const DeviceStream on(params[0]);
+    check(fdgs_adam_step_staged((int)n, p.data(), g.data(), m.data(), v.data(), widths.data(), P, sc, st, beta1, beta2, eps,
+                                (void*)on.stream),
+          "adam_step_staged");
+}
+
 // ---- densification (include/fdgs.h: fdgs_densify_*, fdgs_reset_opacity) --------------------------------------------
 // geo = [xyz, t, scaling, scaling_t, rotation, rotation_r, opacity]; stats = [xyz_gradient_accum, denom, max_radii2D];
 // thresholds = [max_grad, min_opacity, percent_dense * extent, 0.1 * extent, max_screen_size] (rounded to fp32 here,
@@ -1081,9 +1128,11 @@ void ResetOpacity(torch::Tensor& opacity, torch::Tensor& exp_avg, torch::Tensor&
 
 // batch_size 1: point_grad = viewspace_points.grad [P, >= 2], visibility_count empty; batch_size > 1: point_grad =
 // the summed norms [P] and visibility_count [P] (fdgs.dist.ViewBatchStats).  t_grad / t_gradient_accum empty for 3D.
-void DensifyStats(int64_t batch_size, const torch::Tensor& point_grad, const torch::Tensor& visibility_count,
-                  const torch::Tensor& radii, const torch::Tensor& t_grad, torch::Tensor& xyz_gradient_accum, torch::Tensor& denom,
-                  torch::Tensor& t_gradient_accum, torch::Tensor& max_radii2D) {
+// status: the rasterizer's int32 [4] (render_batch's pkg["status"]) or empty: nothing is written on overflow or wrap.
+void DensifyStatsStatus(int64_t batch_size, const torch::Tensor& point_grad, const torch::Tensor& visibility_count,
+                        const torch::Tensor& radii, const torch::Tensor& t_grad, torch::Tensor& xyz_gradient_accum,
+                        torch::Tensor& denom, torch::Tensor& t_gradient_accum, torch::Tensor& max_radii2D,
+                        const torch::Tensor& status) {
     const long long P = xyz_gradient_accum.size(0);
     float* acc = arg<float>(xyz_gradient_accum, "xyz_gradient_accum", P, P);
     float* den = arg<float>(denom, "denom", P, P);
@@ -1094,13 +1143,22 @@ void DensifyStats(int64_t batch_size, const torch::Tensor& point_grad, const tor
     const float* pg = arg<float>(point_grad, "point_grad", P, batch_size == 1 ? -1 : P);
     TORCH_CHECK(point_grad.defined() && (batch_size > 1 || point_grad.dim() == 2), "fdgs: point_grad must be [P, >= 2] for one view");
     const int* r = arg<int>(radii, "radii", -1, P, REQUIRED);
+    const int* st = arg<int>(status, "status", -1, 4);
     same_cuda_device("densification",
-                     {xyz_gradient_accum, denom, t_gradient_accum, max_radii2D, t_grad, visibility_count, point_grad, radii});
+                     {xyz_gradient_accum, denom, t_gradient_accum, max_radii2D, t_grad, visibility_count, point_grad, radii,
+                      status});
     const int stride = batch_size == 1 ? (int)(point_grad.dim() == 2 ? point_grad.size(1) : 0) : 1;
     if (P == 0) return;
     const DeviceStream on(xyz_gradient_accum);
-    check(fdgs_densify_stats(P, (int)batch_size, pg, stride, vis, r, tg, acc, den, tacc, mr, (void*)on.stream),
+    check(fdgs_densify_stats_status(P, (int)batch_size, pg, stride, vis, r, tg, acc, den, tacc, mr, st, (void*)on.stream),
           "densify_stats");
+}
+
+void DensifyStats(int64_t batch_size, const torch::Tensor& point_grad, const torch::Tensor& visibility_count,
+                  const torch::Tensor& radii, const torch::Tensor& t_grad, torch::Tensor& xyz_gradient_accum, torch::Tensor& denom,
+                  torch::Tensor& t_gradient_accum, torch::Tensor& max_radii2D) {
+    DensifyStatsStatus(batch_size, point_grad, visibility_count, radii, t_grad, xyz_gradient_accum, denom, t_gradient_accum,
+                       max_radii2D, torch::Tensor());
 }
 
 // ---- k nearest neighbours (include/fdgs.h: fdgs_knn) ---------------------------------------------------------------
@@ -1255,6 +1313,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("l1_ssim_forward", &L1SsimForward);
     m.def("l1_ssim_backward", &L1SsimBackward);
     m.def("adam_step", &AdamStep);
+    m.def("adam_scalars", &AdamScalars);
+    m.def("adam_step_staged", &AdamStepStaged);
     m.def("knn", &Knn);
     m.def("rigid_neighbours", &RigidNeighbours);
     m.def("rigid_forward", &RigidForward);
@@ -1264,6 +1324,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("densify_apply", &DensifyApply);
     m.def("reset_opacity", &ResetOpacity);
     m.def("densify_stats", &DensifyStats);
+    m.def("densify_stats", &DensifyStatsStatus);
     m.def("pack_rows", &PackRows);
     m.def("unpack_rows", &UnpackRows);
     m.def("rasterize_gaussians", &RasterizeGaussiansCUDA);

@@ -155,23 +155,26 @@ def reset_opacity(gaussians):
 
 @torch.no_grad()
 def add_densification_stats(gaussians, viewspace_grad: Optional[torch.Tensor] = None, radii: Optional[torch.Tensor] = None,
-                            t_grad: Optional[torch.Tensor] = None, batch_stats=None, batch_size: int = 1):
+                            t_grad: Optional[torch.Tensor] = None, batch_stats=None, batch_size: int = 1,
+                            status: Optional[torch.Tensor] = None):
     """The densification statistics of one optimisation step in one kernel: train.py's max_radii2D update and
     `add_densification_stats` (one view: `viewspace_grad` = viewspace_points.grad, `radii` of the view) or
     `add_densification_stats_grad` with the batch rescale (`batch_stats` = fdgs.dist.ViewBatchStats of `batch_size`
-    views).  `t_grad`: `_t.grad` for 4D Gaussians."""
+    views).  `t_grad`: `_t.grad` for 4D Gaussians.  `status`: render_batch's pkg["status"] of a step sized by an
+    instance capacity (fdgs.graph): when it reports an overflow nothing is accumulated."""
     C = fdgs.ext()
     dim = int(getattr(gaussians, "gaussian_dim", 3))
     t_acc = gaussians.t_gradient_accum if dim == 4 else torch.empty(0)
     tg = t_grad.reshape(-1) if (dim == 4 and t_grad is not None) else torch.empty(0)
     if dim == 4 and t_grad is None:
         raise ValueError("4D Gaussians need t_grad (the _t gradient)")
+    status_arg = () if status is None else (status,)
     if batch_stats is not None:
         if batch_size < 2:
             raise ValueError("batch_stats needs batch_size >= 2")
         C.densify_stats(batch_size, batch_stats.grad_norm_sum.reshape(-1), batch_stats.visibility_count.reshape(-1),
                         batch_stats.max_radii.to(torch.int32).contiguous(), tg, gaussians.xyz_gradient_accum,
-                        gaussians.denom, t_acc, gaussians.max_radii2D)
+                        gaussians.denom, t_acc, gaussians.max_radii2D, *status_arg)
     else:
         if batch_size != 1 or viewspace_grad is None or radii is None:
             raise ValueError("one view needs viewspace_grad and radii (or pass batch_stats and batch_size)")
@@ -181,4 +184,4 @@ def add_densification_stats(gaussians, viewspace_grad: Optional[torch.Tensor] = 
         if radii.dtype == torch.bool:
             raise ValueError("radii must be the view's integer radii, not the bool visibility filter")
         C.densify_stats(1, viewspace_grad, torch.empty(0), radii.to(torch.int32).contiguous(), tg,
-                        gaussians.xyz_gradient_accum, gaussians.denom, t_acc, gaussians.max_radii2D)
+                        gaussians.xyz_gradient_accum, gaussians.denom, t_acc, gaussians.max_radii2D, *status_arg)

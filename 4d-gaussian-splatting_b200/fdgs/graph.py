@@ -10,9 +10,12 @@ with one launch, but a captured step must not synchronise and must not bake host
                 count R and whether it overflowed the capacity (the views then render as if no Gaussian were listed).
   GraphedStep   captures a user step fn(views, gt) -> (loss, pkg) once and replays it with new cameras and ground truth;
                 it reads the status once per step, after all of the step's work is queued, and on overflow re-captures
-                with a larger capacity and replays the same inputs.
+                with a larger capacity and replays the same inputs.  Optionally the capture also runs the densification
+                statistics and a fused Adam step (fdgs.optim.FusedAdam) whose learning rates and step counts are staged
+                in device memory before each replay; both are predicated on the status, so an overflowed replay changes
+                nothing and the replay after the re-capture applies them once.
 
-The optimiser, the densification statistics and densification itself run eagerly on the graph's static outputs.
+Densification itself (and the opacity reset) runs eagerly after the call.
 """
 import math
 from typing import Callable, Iterable, List, Optional
@@ -72,6 +75,9 @@ def _leaves(params) -> List[torch.Tensor]:
     return list(src)
 
 
+_STATS = ("xyz_gradient_accum", "denom", "max_radii2D", "t_gradient_accum")
+
+
 class GraphedStep:
     """One training step, captured once and replayed: `step(cams, gt)` runs `fn(views, gt)` -- which calls
     render_batch(views, ...), computes its loss and calls backward() -- and returns fn's (loss, pkg), static tensors that
@@ -85,13 +91,26 @@ class GraphedStep:
     The first call warms up eagerly on a side stream, first at capacity 0 (a background-only render whose status reports
     the true R), then at ceil(margin R); each capture starts with every leaf's .grad set to None, so replays assign
     the gradients rather than accumulate them.  The step's one host synchronisation reads the status after the replay;
-    on overflow the step re-captures at ceil(margin R) and replays the same inputs (the optimiser runs outside the graph,
-    so the parameters have not moved).  `info` counts captures and overflows and holds the capacity."""
+    on overflow the step re-captures at ceil(margin R) and replays the same inputs (the statistics and the optimiser
+    step below are skipped by an overflowed replay, so nothing has moved).  `info` counts captures and overflows and
+    holds the capacity.
 
-    def __init__(self, fn: Callable, params, margin: float = 1.25):
+    `step(cams, gt, densify_stats=True)` also captures the densification statistics after fn, from the replay's own
+    pkg: one view, `add_densification_stats(model, viewspace_grad, radii)`; B >= 2 views, a ViewBatchStats over the views
+    and the batch form; `params` must then be the Gaussian model (xyz_gradient_accum, denom, max_radii2D and, for 4D
+    Gaussians, t_gradient_accum and _t).  optimizer: a fdgs.optim.FusedAdam over exactly the step's leaves; the capture
+    ends with its dense step over every leaf that has a gradient, and the leaves' step counts advance after each call.
+    `hold` keeps tensors from stepping in this call without re-capturing: True (none steps: densification iterations,
+    whose new leaves the reference's Adam skips, and the last iteration) or a collection of group names (e.g.
+    {"opacity"} on an opacity-reset iteration).  Do not call optimizer.step() as well.  The warm-up runs fn only."""
+
+    def __init__(self, fn: Callable, params, margin: float = 1.25, optimizer=None):
+        from fdgs.optim import FusedAdam
         if not margin >= 1.0:
             raise ValueError("margin must be >= 1, got %r" % (margin,))
-        self.fn, self.params, self.margin = fn, params, float(margin)
+        if optimizer is not None and not isinstance(optimizer, FusedAdam):
+            raise ValueError("GraphedStep captures the step of a fdgs.optim.FusedAdam only, got %s" % type(optimizer).__name__)
+        self.fn, self.params, self.margin, self.optimizer = fn, params, float(margin), optimizer
         self.views: Optional[StaticViews] = None
         self.gt: Optional[torch.Tensor] = None
         self.info = {"captures": 0, "overflows": 0, "capacity": None}
@@ -99,13 +118,14 @@ class GraphedStep:
         self._key = None
         self._out = None
         self._grads: List[Optional[torch.Tensor]] = []
+        self._stepped: List[torch.Tensor] = []    # the leaves the captured optimiser step updates
 
     def _sized(self, R: int) -> int:
         return int(math.ceil(self.margin * R))
 
     def _drop(self):
         """Free the graph and its static outputs before another capture."""
-        self._graph, self._out, self._grads = None, None, []
+        self._graph, self._out, self._grads, self._stepped = None, None, [], []
 
     def _warm_up(self, leaves):
         side = torch.cuda.Stream(device=self.views.device)
@@ -121,19 +141,47 @@ class GraphedStep:
             p.grad = None
         self.info["capacity"] = self.views.capacity
 
-    def _capture(self, leaves):
+    def _model(self):
+        return self.params() if callable(self.params) else self.params
+
+    def _stats(self, pkg):
+        """The densification statistics of the step in pkg, skipped on overflow (captured after fn)."""
+        from fdgs import densify as D
+        from fdgs.dist import ViewBatchStats
+        model = self._model()
+        vs = pkg["viewspace_points"].grad
+        if vs is None:
+            raise ValueError("densify_stats needs pkg['viewspace_points'].grad: fn must call backward()")
+        t_grad = model._t.grad if int(getattr(model, "gaussian_dim", 3)) == 4 else None
+        B = self.views.B
+        if B == 1:
+            D.add_densification_stats(model, vs[0], pkg["radii"][0], t_grad=t_grad, status=pkg["status"])
+        else:
+            stats = ViewBatchStats(vs.shape[1], vs.device)
+            for k in range(B):
+                stats.add_view(vs[k], pkg["radii"][k])
+            D.add_densification_stats(model, t_grad=t_grad, batch_stats=stats, batch_size=B, status=pkg["status"])
+
+    def _capture(self, leaves, densify_stats=False):
         self._drop()
         for p in leaves:
             p.grad = None
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
             out = self.fn(self.views, self.gt)
+            if densify_stats:
+                self._stats(out[1])
+            if self.optimizer is not None:
+                self._stepped = [p for p in leaves if p.grad is not None]
+                self.optimizer.step_staged(self._stepped, out[1]["status"])
         self._graph, self._out = graph, out
         self._grads = [p.grad for p in leaves]
         self.info["captures"] += 1
         self.info["capacity"] = self.views.capacity
 
-    def _replay(self, leaves):
+    def _replay(self, leaves, hold=()):
+        if self.optimizer is not None:
+            self.optimizer.stage(self._stepped, hold)
         self._graph.replay()
         for p, g in zip(leaves, self._grads):
             p.grad = g
@@ -142,10 +190,31 @@ class GraphedStep:
             raise RuntimeError("GraphedStep: more than 2^31 - 1 tile instances in one step")
         return status
 
-    def __call__(self, cams, gt: torch.Tensor):
+    def _check(self, leaves, densify_stats, hold):
+        """The new arguments' rejections, before any GPU work."""
+        opt = self.optimizer
+        if opt is None:
+            if hold:
+                raise ValueError("hold needs GraphedStep(..., optimizer=)")
+        else:
+            mine = opt._leaves()
+            if len(mine) != len(leaves) or {id(p) for p in mine} != {id(p) for p in leaves}:
+                raise ValueError("optimizer must be a FusedAdam over exactly the step's leaves")
+            opt.held(hold)
+        if densify_stats:
+            model = self._model()
+            dim = int(getattr(model, "gaussian_dim", 3))
+            need = _STATS[:3] + ((_STATS[3], "_t") if dim == 4 else ())
+            missing = [n for n in need if getattr(model, n, None) is None]
+            if missing:
+                raise ValueError("densify_stats needs the Gaussian model as params (missing: %s)" % ", ".join(missing))
+
+    def __call__(self, cams, gt: torch.Tensor, densify_stats: bool = False, hold=()):
         cams = list(cams)
         if not cams:
             raise ValueError("GraphedStep needs at least one camera")
+        leaves = _leaves(self.params)
+        self._check(leaves, densify_stats, hold)
         B, H, W = len(cams), int(cams[0].image_height), int(cams[0].image_width)
         if self.views is None or (self.views.B, self.views.H, self.views.W) != (B, H, W) or self.gt.shape != gt.shape:
             capacity = self.views.capacity if self.views is not None else None
@@ -156,19 +225,27 @@ class GraphedStep:
                 self.views.capacity = capacity
         self.views.load(cams)
         self.gt.copy_(gt)
-        leaves = _leaves(self.params)
-        model = self.params() if callable(self.params) else self.params
+        model = self._model()
         key = (B, H, W, tuple(p.shape[0] for p in leaves[:1]), tuple(p.data_ptr() for p in leaves),
-               getattr(model, "active_sh_degree", None), getattr(model, "active_sh_degree_t", None))
+               getattr(model, "active_sh_degree", None), getattr(model, "active_sh_degree_t", None), bool(densify_stats))
+        if densify_stats:
+            key += tuple(getattr(model, n).data_ptr() if getattr(model, n, None) is not None else None for n in _STATS)
+        if self.optimizer is not None:
+            self.optimizer.init_state()
+            st = self.optimizer.state
+            key += (self.optimizer._table.data_ptr(),) + tuple(
+                (st[p]["exp_avg"].data_ptr(), st[p]["exp_avg_sq"].data_ptr()) for p in leaves)
         if self._graph is None or key != self._key:
             if self.info["capacity"] is None:
                 self._warm_up(leaves)
-            self._capture(leaves)
+            self._capture(leaves, densify_stats)
             self._key = key
-        status = self._replay(leaves)
+        status = self._replay(leaves, hold)
         if status[2]:
             self.info["overflows"] += 1
             self.views.capacity = self._sized(status[0])
-            self._capture(leaves)
-            status = self._replay(leaves)
+            self._capture(leaves, densify_stats)
+            status = self._replay(leaves, hold)
+        if self.optimizer is not None and not status[2]:
+            self.optimizer.commit(self._stepped, hold)
         return self._out

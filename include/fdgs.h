@@ -408,6 +408,12 @@ int fdgs_view_stats(long long P, const float* viewspace_grad, int grad_stride, c
 int fdgs_densify_stats(long long P, int batch_size, const float* point_grad, int point_grad_stride,
                        const float* visibility_count, const int* radii, const float* t_grad, float* xyz_gradient_accum,
                        float* denom, float* t_gradient_accum, float* max_radii2D, void* stream);
+/* The same, predicated on the rasterizer's status (device int[4] {R, largest tile, overflow, wrap}, as
+ * fdgs_forward_batch_capacity writes it; NULL = fdgs_densify_stats): with overflow or wrap set nothing is written, so a
+ * CUDA graph whose forward overflowed can be replayed again without counting the step twice. */
+int fdgs_densify_stats_status(long long P, int batch_size, const float* point_grad, int point_grad_stride,
+                              const float* visibility_count, const int* radii, const float* t_grad, float* xyz_gradient_accum,
+                              float* denom, float* t_gradient_accum, float* max_radii2D, const int* status, void* stream);
 
 /* Densify and prune (reference: scene/gaussian_model.py:486-577 densify_and_prune with densify_and_clone,
  * densify_and_split and prune_points) as one compaction of every parameter row and Adam-moment row into new tensors.
@@ -499,6 +505,22 @@ int fdgs_l1_ssim_backward(const float* x, const float* y, int C, int H, int W, c
 int fdgs_adam_step(int n, float* const* params, float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,
                    const int* widths, const float* lrs, long long P, const long long* rows, long long num_rows,
                    long long step, double beta1, double beta2, double eps, int zero_grad, void* stream);
+
+/* Adam's per-tensor scalars, on the host, in the double arithmetic fdgs_adam_step uses (it calls this function):
+ * for each of n <= FDGS_MAX_PACK tensors with enable[i] != 0 and its 1-based step count steps[i] (already advanced),
+ *   table[3i] = (float)((double)lrs[i] / (1 - beta1^steps[i])),  table[3i+1] = (float)sqrt(1 - beta2^steps[i]),
+ *   table[3i+2] = 1;
+ * a tensor with enable[i] == 0 gets {0, 1, 0} (its step count is not read).  All pointers are host arrays. */
+int fdgs_adam_scalars(int n, const float* lrs, const long long* steps, const int* enable, double beta1, double beta2,
+                      float* table);
+
+/* Dense fused Adam with the per-tensor scalars read on the device, for a step captured in a CUDA graph: the tensor
+ * table of fdgs_adam_step; scalars = device float[3n], a table as fdgs_adam_scalars fills it (a tensor whose enable
+ * entry is 0 keeps its parameter and both moments); status = NULL or the rasterizer's device int[4] {R, largest tile,
+ * overflow, wrap}: with overflow or wrap set nothing is written.  Tensors of different step counts share the launch. */
+int fdgs_adam_step_staged(int n, float* const* params, float* const* grads, float* const* exp_avg, float* const* exp_avg_sq,
+                          const int* widths, long long P, const float* scalars, const int* status, double beta1, double beta2,
+                          double eps, void* stream);
 
 /* k nearest neighbours (k <= 32) of every point among the same n points, squared distances ascending, the point
  * itself first (reference: pointops2 knnquery, pointops2/src/knnquery/knnquery_cuda_kernel.cu:65-107, as called by
