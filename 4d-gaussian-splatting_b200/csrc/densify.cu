@@ -204,12 +204,16 @@ __global__ void __launch_bounds__(THREADS) reset_opacity_kernel(long long P, flo
     if (v) v[i] = 0.f;
 }
 
-// Gaussian i's statistics, the body of both statistics kernels
-__device__ __forceinline__ void densify_stats_row(long long i, long long P, int B, const float* __restrict__ pgrad, int stride,
-                                                  const float* __restrict__ vis, const int* __restrict__ radii,
-                                                  const float* __restrict__ tgrad, float* __restrict__ accum,
-                                                  float* __restrict__ denom, float* __restrict__ taccum,
-                                                  float* __restrict__ max_radii2D) {
+// One thread per Gaussian.  With a status {R, largest tile, overflow, wrap} from the rasterizer, nothing is accumulated
+// when it reports an overflow or a wrap: a captured step whose forward overflowed is replayed after a re-capture
+__global__ void __launch_bounds__(THREADS) densify_stats_kernel(long long P, int B, const float* __restrict__ pgrad, int stride,
+                                                               const float* __restrict__ vis, const int* __restrict__ radii,
+                                                               const float* __restrict__ tgrad, float* __restrict__ accum,
+                                                               float* __restrict__ denom, float* __restrict__ taccum,
+                                                               float* __restrict__ max_radii2D,
+                                                               const int* __restrict__ status) {
+    if (status && (status[2] | status[3])) return;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P) return;
     const int r = radii[i];
     float g, tg = 0.f;
@@ -229,29 +233,6 @@ __device__ __forceinline__ void densify_stats_row(long long i, long long P, int 
     accum[i] = fadd(accum[i], g);
     denom[i] = fadd(denom[i], 1.0f);
     if (taccum) taccum[i] = fadd(taccum[i], tg);
-}
-
-__global__ void __launch_bounds__(THREADS) densify_stats_kernel(long long P, int B, const float* __restrict__ pgrad, int stride,
-                                                               const float* __restrict__ vis, const int* __restrict__ radii,
-                                                               const float* __restrict__ tgrad, float* __restrict__ accum,
-                                                               float* __restrict__ denom, float* __restrict__ taccum,
-                                                               float* __restrict__ max_radii2D) {
-    densify_stats_row((long long)blockIdx.x * blockDim.x + threadIdx.x, P, B, pgrad, stride, vis, radii, tgrad, accum, denom,
-                      taccum, max_radii2D);
-}
-
-// The same, skipped when the rasterizer's status {R, largest tile, overflow, wrap} reports an overflow or a wrap: a
-// captured step whose forward overflowed accumulates nothing and is replayed after a re-capture
-__global__ void __launch_bounds__(THREADS) densify_stats_status_kernel(long long P, int B, const float* __restrict__ pgrad,
-                                                                      int stride, const float* __restrict__ vis,
-                                                                      const int* __restrict__ radii,
-                                                                      const float* __restrict__ tgrad, float* __restrict__ accum,
-                                                                      float* __restrict__ denom, float* __restrict__ taccum,
-                                                                      float* __restrict__ max_radii2D,
-                                                                      const int* __restrict__ status) {
-    if (status[2] | status[3]) return;
-    densify_stats_row((long long)blockIdx.x * blockDim.x + threadIdx.x, P, B, pgrad, stride, vis, radii, tgrad, accum, denom,
-                      taccum, max_radii2D);
 }
 
 inline size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
@@ -336,12 +317,8 @@ cudaError_t launch_densify_stats(long long P, int B, const float* pgrad, int str
                                  const float* tgrad, float* accum, float* denom, float* taccum, float* max_radii2D,
                                  const int* status, cudaStream_t stream) {
     if (P == 0) return cudaSuccess;
-    if (status)
-        densify_stats_status_kernel<<<grid_for(P), THREADS, 0, stream>>>(P, B, pgrad, stride, vis, radii, tgrad, accum, denom,
-                                                                        taccum, max_radii2D, status);
-    else
-        densify_stats_kernel<<<grid_for(P), THREADS, 0, stream>>>(P, B, pgrad, stride, vis, radii, tgrad, accum, denom, taccum,
-                                                                 max_radii2D);
+    densify_stats_kernel<<<grid_for(P), THREADS, 0, stream>>>(P, B, pgrad, stride, vis, radii, tgrad, accum, denom, taccum,
+                                                             max_radii2D, status);
     return cudaGetLastError();
 }
 

@@ -9,7 +9,6 @@
 // The backward scatters dL/dsky to the four texels of every pixel.  Neighbouring pixels share texels (at 1352x1014
 // against a 500x500 map about a hundred pixels land on each), so the lanes of a warp that read the same 2x2 texel
 // block add their contributions first (__match_any_sync) and one lane issues the RED per texel and channel.
-#include <stdlib.h>
 #include "fdgs_internal.h"
 
 namespace fdgs {
@@ -92,8 +91,7 @@ __global__ void __launch_bounds__(SKY_THREADS) sky_fwd_kernel(const SkyParams p,
     out[2 * (size_t)HW + pix] = c2;
 }
 
-// AGGREGATE: sum the contributions of the lanes sharing a 2x2 texel block before the RED (see the file comment)
-template <bool AGGREGATE>
+// the lanes sharing a 2x2 texel block sum their contributions before the RED (see the file comment)
 __global__ void __launch_bounds__(SKY_THREADS) sky_bwd_kernel(const SkyParams p, const float* __restrict__ g,
                                                               float* __restrict__ denv) {
     const int pix = blockIdx.x * SKY_THREADS + threadIdx.x;
@@ -111,19 +109,6 @@ __global__ void __launch_bounds__(SKY_THREADS) sky_bwd_kernel(const SkyParams p,
         t.w[0] = t.w[1] = t.w[2] = t.w[3] = 0.f;
     }
     const int HWm = p.env_width * p.env_height;
-    if (!AGGREGATE) {
-        if (!live) return;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const int x = t.x0 + (k & 1), y = t.y0 + (k >> 1);
-            if (!texel_in(p, x, y)) continue;
-            float* e = denv + (size_t)y * p.env_width + x;
-            atomicAdd(e, t.w[k] * g0);
-            atomicAdd(e + HWm, t.w[k] * g1);
-            atomicAdd(e + 2 * (size_t)HWm, t.w[k] * g2);
-        }
-        return;
-    }
     // every lane of the warp takes part (dead lanes carry zero weights on a block no live lane can have)
     __shared__ float part[SKY_THREADS / 32][12][32];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -170,9 +155,7 @@ cudaError_t launch_sky_fwd(const SkyParams& p, float* out_sky, int* miss_flag, c
 cudaError_t launch_sky_bwd(const SkyParams& p, const float* dL_dsky, float* dL_denv, cudaStream_t stream) {
     const long long n = (long long)p.W * p.H;
     const unsigned int blocks = (unsigned int)((n + SKY_THREADS - 1) / SKY_THREADS);
-    // FDGS_SKY_BWD_PLAIN selects one RED per pixel, texel and channel (kept to measure the warp aggregation against)
-    if (getenv("FDGS_SKY_BWD_PLAIN") != nullptr) sky_bwd_kernel<false><<<blocks, SKY_THREADS, 0, stream>>>(p, dL_dsky, dL_denv);
-    else sky_bwd_kernel<true><<<blocks, SKY_THREADS, 0, stream>>>(p, dL_dsky, dL_denv);
+    sky_bwd_kernel<<<blocks, SKY_THREADS, 0, stream>>>(p, dL_dsky, dL_denv);
     return cudaGetLastError();
 }
 

@@ -10,7 +10,6 @@ CUDA library (fdgs) instead of diff-gaussian-rasterization.
 import the reference's `scene` or `utils` packages, so it also works stand-alone (tests, bench).
 """
 import math
-import os
 
 import torch
 from torch.nn import functional as F
@@ -31,9 +30,9 @@ def _fused_prologue_ok(pc, pipe, override_color):
     """Can this frame take the raw-parameter entry (GaussianRasterizer.forward_raw)?  Yes when the model is the
     reference's GaussianModel in its all-CUDA configuration: raw parameter tensors present, the standard activations
     (scene/gaussian_model.py:44-60: exp / sigmoid / F.normalize) and no python-side preprocessing or colour override.
-    Then exp, F.normalize x2, sigmoid and the torch.cat of get_features run inside the kernels.  FDGS_FUSED_PROLOGUE=0
-    (or pipe.fused_prologue = False) forces the getter path."""
-    if os.environ.get("FDGS_FUSED_PROLOGUE", "1") == "0" or not getattr(pipe, "fused_prologue", True):
+    Then exp, F.normalize x2, sigmoid and the torch.cat of get_features run inside the kernels.
+    pipe.fused_prologue = False forces the getter path."""
+    if not getattr(pipe, "fused_prologue", True):
         return False
     if override_color is not None or pipe.compute_cov3D_python or pipe.convert_SHs_python:
         return False

@@ -67,22 +67,6 @@ def test_sky_sampler_against_float64(camname, emap, img):
         assert l2n <= 2 * l2t + 1e-6
 
 
-def test_sky_backward_aggregation_matches_plain_reds(monkeypatch):
-    """the warp-aggregated scatter and one RED per pixel / texel / channel sum the same contributions"""
-    from fdgs.sky import sky_background
-    W, H = 1352, 1014
-    cam = _camera(CAMERAS["n3v"], W, H)
-    g = torch.randn(3, H, W, generator=torch.Generator().manual_seed(11)).to(DEV)
-    grads = []
-    for plain in (False, True):
-        if plain:
-            monkeypatch.setenv("FDGS_SKY_BWD_PLAIN", "1")
-        env = _env((500, 500)).requires_grad_(True)
-        (sky_background(env, cam) * g).sum().backward()
-        grads.append(env.grad)
-    assert helpers.l2_rel(helpers.to_np(grads[0]), helpers.to_np(grads[1])) < 1e-5
-
-
 # ---- render() with an environment map ---------------------------------------------------------------------------------
 class SkyModel(RawModel):
     """RawModel with an environment-map parameter and the python-side covariance helpers of the reference's model."""

@@ -5,7 +5,7 @@ backward per step.
 
 The two arms alternate inside one process (warm-up, then timed steps with CUDA events).  A separate torch.profiler run
 of each arm names the blend-backward instantiation it ran and the kernel times of the sky; a third run times the
-sky backward with and without warp aggregation.  Prints the card name and power limit with the numbers.
+sky sampler's kernels alone.  Prints the card name and power limit with the numbers.
 
     python tools/bench_sky.py --steps 50 --warmup 10 [--out DIR]
 """
@@ -113,24 +113,19 @@ def main():
             "ms_per_step": {n: round(v[0], 4) for n, v in per.items()
                             if any(s in n for s in ("blend_bwd", "blend_fwd", "sky_", "grid_sampler", "linalg", "atan2", "acos"))},
         }
-    # the sky backward alone, warp-aggregated against one RED per pixel / texel / channel
-    sky_bwd = {}
+    # the sky sampler alone, forward and backward
     from fdgs.sky import sky_background
     g = torch.randn(3, cfg["H"], cfg["W"], generator=torch.Generator().manual_seed(3)).to(DEV)
-    for mode in ("aggregated", "plain"):
-        if mode == "plain":
-            os.environ["FDGS_SKY_BWD_PLAIN"] = "1"
-        env = model.env_map.detach().clone().requires_grad_(True)
-        for _ in range(5):
+    env = model.env_map.detach().clone().requires_grad_(True)
+    for _ in range(5):
+        (sky_background(env, cam) * g).sum().backward()
+    torch.cuda.synchronize()
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        for _ in range(20):
             (sky_background(env, cam) * g).sum().backward()
         torch.cuda.synchronize()
-        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-            for _ in range(20):
-                (sky_background(env, cam) * g).sum().backward()
-            torch.cuda.synchronize()
-        sky_bwd[mode] = {e.key: round(getattr(e, "device_time_total", 0.0) / 20.0 / 1000.0, 4)
-                         for e in prof.key_averages() if "sky_" in e.key}
-    os.environ.pop("FDGS_SKY_BWD_PLAIN", None)
+    sky_bwd = {e.key: round(getattr(e, "device_time_total", 0.0) / 20.0 / 1000.0, 4)
+               for e in prof.key_averages() if "sky_" in e.key}
 
     name, limit = card()
     res = {"workload": "cfg5 + env_map 500x500, render + colour-only loss + backward", "card": name,
