@@ -721,6 +721,27 @@ fdgs::SkyParams sky_params(const fdgs_sky_args* a) {
     return p;
 }
 
+int check_sky_batch_args(const fdgs_sky_batch_args* a) {
+    if (!a) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    if (!a->env_map || !a->c2w || !a->campos || !a->intrinsics)
+        return fail(FDGS_ERR_INVALID_ARG, "env_map / c2w / campos / intrinsics required");
+    if (a->B < 1 || a->B > 65535) return fail(FDGS_ERR_INVALID_ARG, "view count B must be in 1..65535");
+    if (a->env_height <= 0 || a->env_width <= 0 || a->env_width > 65000 || a->width <= 0 || a->height <= 0)
+        return fail(FDGS_ERR_INVALID_ARG, "bad environment map / image size");
+    if ((long long)a->width * a->height * 3 * a->B > INT_MAX)
+        return fail(FDGS_ERR_INVALID_ARG, "bad environment map / image size: B x 3 x H x W exceeds 2^31 - 1");
+    if (!(a->radius > 0.0f)) return fail(FDGS_ERR_INVALID_ARG, "sky radius must be positive");
+    return FDGS_OK;
+}
+
+fdgs::SkyBatchParams sky_batch_params(const fdgs_sky_batch_args* a) {
+    fdgs::SkyBatchParams p;
+    p.env_map = a->env_map; p.env_height = a->env_height; p.env_width = a->env_width;
+    p.c2w = a->c2w; p.campos = a->campos; p.intrinsics = a->intrinsics; p.radius = a->radius;
+    p.W = a->width; p.H = a->height; p.B = a->B;
+    return p;
+}
+
 }  // namespace
 
 extern "C" {
@@ -785,6 +806,26 @@ int fdgs_sky_backward(const fdgs_sky_args* a, const float* dL_dsky, float* dL_de
     if (int rc = check_sky_args(a)) return rc;
     if (!dL_dsky || !dL_denv) return fail(FDGS_ERR_INVALID_ARG, "null argument");
     FDGS_CUDA(fdgs::launch_sky_bwd(sky_params(a), dL_dsky, dL_denv, reinterpret_cast<cudaStream_t>(stream_v)), "sky_backward");
+    g_kernel_launches += 1;
+    return FDGS_OK;
+}
+
+int fdgs_sky_forward_batch(const fdgs_sky_batch_args* a, float* out_sky, int* miss_flag, void* stream_v) {
+    g_last_error.clear();
+    if (int rc = check_sky_batch_args(a)) return rc;
+    if (!out_sky) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    FDGS_CUDA(fdgs::launch_sky_fwd_batch(sky_batch_params(a), out_sky, miss_flag, reinterpret_cast<cudaStream_t>(stream_v)),
+              "sky_forward_batch");
+    g_kernel_launches += 1;
+    return FDGS_OK;
+}
+
+int fdgs_sky_backward_batch(const fdgs_sky_batch_args* a, const float* dL_dsky, float* dL_denv, void* stream_v) {
+    g_last_error.clear();
+    if (int rc = check_sky_batch_args(a)) return rc;
+    if (!dL_dsky || !dL_denv) return fail(FDGS_ERR_INVALID_ARG, "null argument");
+    FDGS_CUDA(fdgs::launch_sky_bwd_batch(sky_batch_params(a), dL_dsky, dL_denv, reinterpret_cast<cudaStream_t>(stream_v)),
+              "sky_backward_batch");
     g_kernel_launches += 1;
     return FDGS_OK;
 }

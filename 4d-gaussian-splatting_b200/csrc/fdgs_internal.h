@@ -343,5 +343,19 @@ struct SkyParams {
 cudaError_t launch_sky_fwd(const SkyParams& p, float* out_sky, int* miss_flag, cudaStream_t stream);
 // dL_denv [3,Hm,Wm] += the bilinear taps' share of dL_dsky [3,H,W]
 cudaError_t launch_sky_bwd(const SkyParams& p, const float* dL_dsky, float* dL_denv, cudaStream_t stream);
+// B views of one image size, each camera from device tables (include/fdgs.h: fdgs_sky_batch_args)
+struct SkyBatchParams {
+    const float* env_map;     // [3,Hm,Wm]
+    int env_height, env_width;
+    const float* c2w;         // [B,16] row-major camera-to-world
+    const float* campos;      // [B,3]
+    const float* intrinsics;  // [B,4] fl_x, fl_y, cx, cy
+    float radius;
+    int W, H, B;
+};
+// out_sky [B,3,H,W]; miss_flag[0] = 1 if a ray of any view misses the sphere (may be NULL)
+cudaError_t launch_sky_fwd_batch(const SkyBatchParams& b, float* out_sky, int* miss_flag, cudaStream_t stream);
+// dL_denv [3,Hm,Wm] += every view's bilinear taps' share of dL_dsky [B,3,H,W]
+cudaError_t launch_sky_bwd_batch(const SkyBatchParams& b, const float* dL_dsky, float* dL_denv, cudaStream_t stream);
 
 }  // namespace fdgs

@@ -69,10 +69,9 @@ __device__ __forceinline__ bool texel_in(const SkyParams& p, int x, int y) {
     return x >= 0 && x < p.env_width && y >= 0 && y < p.env_height;
 }
 
-__global__ void __launch_bounds__(SKY_THREADS) sky_fwd_kernel(const SkyParams p, float* __restrict__ out, int* miss_flag) {
-    const int pix = blockIdx.x * SKY_THREADS + threadIdx.x;
+// one pixel of the forward: the sky colour of pixel `pix` of the camera in p into out [3,H,W]
+__device__ __forceinline__ void sky_fwd_pixel(const SkyParams& p, int pix, float* __restrict__ out, int* miss_flag) {
     const int HW = p.W * p.H;
-    if (pix >= HW) return;
     const SkyTap t = sky_tap(p, pix % p.W, pix / p.W);
     if (t.miss && miss_flag) atomicOr(miss_flag, 1);
     const int HWm = p.env_width * p.env_height;
@@ -91,9 +90,9 @@ __global__ void __launch_bounds__(SKY_THREADS) sky_fwd_kernel(const SkyParams p,
     out[2 * (size_t)HW + pix] = c2;
 }
 
-// the lanes sharing a 2x2 texel block sum their contributions before the RED (see the file comment)
-__global__ void __launch_bounds__(SKY_THREADS) sky_bwd_kernel(const SkyParams p, const float* __restrict__ g,
-                                                              float* __restrict__ denv) {
+// the backward of the block's pixels (blockIdx.x) of the camera in p, called by every thread of the block; the lanes
+// sharing a 2x2 texel block sum their contributions before the RED (see the file comment)
+__device__ __forceinline__ void sky_bwd_pixels(const SkyParams& p, const float* __restrict__ g, float* __restrict__ denv) {
     const int pix = blockIdx.x * SKY_THREADS + threadIdx.x;
     const int HW = p.W * p.H;
     const bool live = pix < HW;
@@ -143,6 +142,46 @@ __global__ void __launch_bounds__(SKY_THREADS) sky_bwd_kernel(const SkyParams p,
     }
 }
 
+__global__ void __launch_bounds__(SKY_THREADS) sky_fwd_kernel(const SkyParams p, float* __restrict__ out, int* miss_flag) {
+    const int pix = blockIdx.x * SKY_THREADS + threadIdx.x;
+    if (pix >= p.W * p.H) return;
+    sky_fwd_pixel(p, pix, out, miss_flag);
+}
+
+__global__ void __launch_bounds__(SKY_THREADS) sky_bwd_kernel(const SkyParams p, const float* __restrict__ g,
+                                                              float* __restrict__ denv) {
+    sky_bwd_pixels(p, g, denv);
+}
+
+// view v's camera from the device tables: the single-view kernels' SkyParams, so the per-pixel arithmetic is theirs
+__device__ __forceinline__ SkyParams batch_view(const SkyBatchParams& b, int v) {
+    SkyParams p;
+    p.env_map = b.env_map; p.env_height = b.env_height; p.env_width = b.env_width;
+    p.c2w = b.c2w + 16 * (size_t)v;
+    p.campos = b.campos + 3 * (size_t)v;
+    const float* k = b.intrinsics + 4 * (size_t)v;
+    p.fl_x = k[0]; p.fl_y = k[1]; p.cx = k[2]; p.cy = k[3];
+    p.radius = b.radius;
+    p.W = b.W; p.H = b.H;
+    return p;
+}
+
+// blockIdx.y = view: sky [B,3,H,W], every view's misses ORed into one flag
+__global__ void __launch_bounds__(SKY_THREADS) sky_fwd_batch_kernel(const SkyBatchParams b, float* __restrict__ out,
+                                                                    int* miss_flag) {
+    const int pix = blockIdx.x * SKY_THREADS + threadIdx.x;
+    if (pix >= b.W * b.H) return;
+    const int v = blockIdx.y;
+    sky_fwd_pixel(batch_view(b, v), pix, out + (size_t)v * 3 * b.W * b.H, miss_flag);
+}
+
+// blockIdx.y = view: every view's dL_dsky [B,3,H,W] accumulated into the one dL_denv [3,Hm,Wm]
+__global__ void __launch_bounds__(SKY_THREADS) sky_bwd_batch_kernel(const SkyBatchParams b, const float* __restrict__ g,
+                                                                    float* __restrict__ denv) {
+    const int v = blockIdx.y;
+    sky_bwd_pixels(batch_view(b, v), g + (size_t)v * 3 * b.W * b.H, denv);
+}
+
 }  // namespace
 
 cudaError_t launch_sky_fwd(const SkyParams& p, float* out_sky, int* miss_flag, cudaStream_t stream) {
@@ -156,6 +195,20 @@ cudaError_t launch_sky_bwd(const SkyParams& p, const float* dL_dsky, float* dL_d
     const long long n = (long long)p.W * p.H;
     const unsigned int blocks = (unsigned int)((n + SKY_THREADS - 1) / SKY_THREADS);
     sky_bwd_kernel<<<blocks, SKY_THREADS, 0, stream>>>(p, dL_dsky, dL_denv);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_sky_fwd_batch(const SkyBatchParams& b, float* out_sky, int* miss_flag, cudaStream_t stream) {
+    const long long n = (long long)b.W * b.H;
+    const dim3 grid((unsigned int)((n + SKY_THREADS - 1) / SKY_THREADS), (unsigned int)b.B);
+    sky_fwd_batch_kernel<<<grid, SKY_THREADS, 0, stream>>>(b, out_sky, miss_flag);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_sky_bwd_batch(const SkyBatchParams& b, const float* dL_dsky, float* dL_denv, cudaStream_t stream) {
+    const long long n = (long long)b.W * b.H;
+    const dim3 grid((unsigned int)((n + SKY_THREADS - 1) / SKY_THREADS), (unsigned int)b.B);
+    sky_bwd_batch_kernel<<<grid, SKY_THREADS, 0, stream>>>(b, dL_dsky, dL_denv);
     return cudaGetLastError();
 }
 

@@ -733,6 +733,52 @@ torch::Tensor SkyBackward(const torch::Tensor& env_map, const torch::Tensor& c2w
     return denv;
 }
 
+// ---- the sky of B views, cameras from device tables (include/fdgs.h: fdgs_sky_forward_batch / _backward_batch) -------
+static fdgs_sky_batch_args sky_batch_args(const torch::Tensor& env_map, const torch::Tensor& c2w, const torch::Tensor& campos,
+                                          const torch::Tensor& intrinsics, const double radius, const int64_t H,
+                                          const int64_t W) {
+    fdgs_sky_batch_args a;
+    memset(&a, 0, sizeof(a));
+    a.env_map = arg<float>(env_map, "env_map", 3, -1, REQUIRED);
+    TORCH_CHECK(env_map.dim() == 3, "fdgs: env_map must be [3,Hm,Wm]");
+    TORCH_CHECK(c2w.dim() == 3 && c2w.size(1) == 4 && c2w.size(2) == 4, "fdgs: c2w must be [B,4,4]");
+    const int64_t B = c2w.size(0);
+    a.c2w = arg<float>(c2w, "c2w", B, 16 * B, REQUIRED);
+    a.campos = arg<float>(campos, "campos", B, 3 * B, REQUIRED);
+    a.intrinsics = arg<float>(intrinsics, "intrinsics", B, 4 * B, REQUIRED);
+    same_cuda_device("sky", {env_map, c2w, campos, intrinsics});
+    a.env_height = (int)env_map.size(1); a.env_width = (int)env_map.size(2);
+    a.radius = (float)radius;
+    a.width = (int)W; a.height = (int)H; a.B = (int)B;
+    return a;
+}
+
+// (sky [B,3,H,W], miss flag int32 [1]: 1 if a ray of any view missed the sphere)
+std::tuple<torch::Tensor, torch::Tensor> SkyForwardBatch(const torch::Tensor& env_map, const torch::Tensor& c2w,
+                                                         const torch::Tensor& campos, const torch::Tensor& intrinsics,
+                                                         const double radius, const int64_t H, const int64_t W) {
+    const fdgs_sky_batch_args a = sky_batch_args(env_map, c2w, campos, intrinsics, radius, H, W);
+    const DeviceStream on(env_map);
+    torch::Tensor sky = torch::empty({(int64_t)a.B, 3, H, W}, env_map.options());
+    torch::Tensor miss = torch::zeros({1}, env_map.options().dtype(torch::kInt32));
+    check(fdgs_sky_forward_batch(&a, sky.data_ptr<float>(), miss.data_ptr<int>(), (void*)on.stream), "sky_forward_batch");
+    return std::make_tuple(sky, miss);
+}
+
+// dL/d env_map [3,Hm,Wm] of dL_dsky [B,3,H,W], summed over the views
+torch::Tensor SkyBackwardBatch(const torch::Tensor& env_map, const torch::Tensor& c2w, const torch::Tensor& campos,
+                               const torch::Tensor& intrinsics, const double radius, const torch::Tensor& dL_dsky) {
+    TORCH_CHECK(dL_dsky.is_cuda() && dL_dsky.scalar_type() == torch::kFloat32 && dL_dsky.dim() == 4 && dL_dsky.size(1) == 3 &&
+                    dL_dsky.size(0) == c2w.size(0),
+                "fdgs: dL_dsky must be a float32 CUDA tensor [B,3,H,W]");
+    const fdgs_sky_batch_args a = sky_batch_args(env_map, c2w, campos, intrinsics, radius, dL_dsky.size(2), dL_dsky.size(3));
+    const DeviceStream on(env_map);
+    const auto g = dL_dsky.contiguous();
+    torch::Tensor denv = torch::zeros_like(env_map);
+    check(fdgs_sky_backward_batch(&a, g.data_ptr<float>(), denv.data_ptr<float>(), (void*)on.stream), "sky_backward_batch");
+    return denv;
+}
+
 // rebuild + sum the dL_dsh rows of all views from the gathered colour factors (include/fdgs.h: fdgs_sh_outer_sum)
 void ShOuterSum(const torch::Tensor& table, const int64_t view_stride, const int64_t meta_off, const int64_t V,
                 const int64_t K, const torch::Tensor& slot_of, const torch::Tensor& union_idx, const torch::Tensor& means3D,
@@ -1339,6 +1385,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("debug_export_binning_view", &DebugExportBinningView);
     m.def("sky_forward", &SkyForward);
     m.def("sky_backward", &SkyBackward);
+    m.def("sky_forward_batch", &SkyForwardBatch);
+    m.def("sky_backward_batch", &SkyBackwardBatch);
     m.def("sh_outer_sum", &ShOuterSum);
     m.def("check_rows_zero", &CheckRowsZero);
     m.def("union_maps", &UnionMaps);

@@ -11,7 +11,8 @@ moments instead of coasting on decaying momentum) and is opt-in.  CUDA only.
 Step counts are per parameter, as in torch: `state[p]["step"]` (a CPU float32 scalar tensor, torch's format, so
 `fdgs.densify` and state copied from `torch.optim.Adam` carry it) counts the steps in which `p` had a gradient, and
 that count sets `p`'s bias correction.  A parameter whose `.grad` is None is skipped without advancing its count; a
-parameter group added later starts at step 1.  Tensors of equal step share a launch.
+parameter group added later starts at step 1.  Tensors of equal step and row count share a launch (a tensor of another
+row count, such as an environment map [3,Hm,Wm] beside the per-Gaussian rows, gets its own).
 
 For a step captured in a CUDA graph (fdgs.graph.GraphedStep(..., optimizer=)), the learning rates and step counts
 cannot be kernel arguments: the graph would freeze them.  `init_state()` allocates every leaf's state outside the
@@ -26,6 +27,18 @@ from typing import Iterable, Optional
 import torch
 
 import fdgs
+
+
+def _launches(params):
+    """[i, j) runs of consecutive tensors that one launch can take: at most 16 (FDGS_MAX_PACK), all of one row count."""
+    out, i = [], 0
+    while i < len(params):
+        j = i + 1
+        while j < len(params) and j - i < 16 and params[j].shape[0] == params[i].shape[0]:
+            j += 1
+        out.append((i, j))
+        i = j
+    return out
 
 
 class FusedAdam:
@@ -65,7 +78,7 @@ class FusedAdam:
     @torch.no_grad()
     def step(self, rows: Optional[torch.Tensor] = None, zero_grad: bool = False):
         """One Adam step over every parameter that has a gradient.  rows: int64 CUDA index tensor or None (dense)."""
-        by_step = {}   # step count -> (params, grads, exp_avg, exp_avg_sq, lrs): one bias correction per launch
+        by_step = {}   # (step count, rows) -> (params, grads, exp_avg, exp_avg_sq, lrs): one bias correction per launch
         for g in self.param_groups:
             for p in g["params"]:
                 if p.grad is None:
@@ -74,13 +87,13 @@ class FusedAdam:
                 st["step"] += 1
                 if not p.grad.is_contiguous():
                     p.grad = p.grad.contiguous()
-                t = by_step.setdefault(int(st["step"]), ([], [], [], [], []))
+                t = by_step.setdefault((int(st["step"]), p.shape[0]), ([], [], [], [], []))
                 for lst, x in zip(t, (p.data, p.grad, st["exp_avg"], st["exp_avg_sq"], float(g["lr"]))):
                     lst.append(x)
         C = fdgs.ext()
         sparse = rows is not None
         rows_t = rows if sparse else torch.empty(0, dtype=torch.int64)
-        for step, (ps, gs, ms, vs, lrs) in by_step.items():
+        for (step, _), (ps, gs, ms, vs, lrs) in by_step.items():
             for i in range(0, len(ps), 16):
                 C.adam_step(ps[i:i + 16], gs[i:i + 16], ms[i:i + 16], vs[i:i + 16], lrs[i:i + 16], rows_t, sparse,
                             step, self.betas[0], self.betas[1], self.eps, zero_grad)
@@ -128,8 +141,8 @@ class FusedAdam:
             raise RuntimeError("FusedAdam.step_staged: call init_state() first (outside any graph capture)")
         C = fdgs.ext()
         st = status if status is not None else torch.empty(0, dtype=torch.int32)
-        for i in range(0, len(params), 16):
-            ps = params[i:i + 16]
+        for i, j in _launches(params):
+            ps = params[i:j]
             sts = [self.state[p] for p in ps]
             C.adam_step_staged([p.data for p in ps], [p.grad.contiguous() for p in ps], [s["exp_avg"] for s in sts],
                                [s["exp_avg_sq"] for s in sts], self._table[i:i + len(ps)].view(-1), st,

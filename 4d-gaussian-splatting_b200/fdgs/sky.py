@@ -7,6 +7,10 @@ the sampling is one CUDA kernel each way and the composition happens inside the 
 
     sky = sky_background(pc.env_map, camera)                  # [3,H,W], differentiable w.r.t. env_map
     color, radii, depth, alpha, flow, covs = rasterizer(..., bg_image=sky)
+
+sample_sky_batch(env_map, views) samples the B cameras of an fdgs.graph.StaticViews(..., sky=True) in one launch each
+way from the views' device tables: it neither synchronises nor reads the miss flag on the host, so a CUDA graph can
+capture it.
 """
 import torch
 
@@ -39,6 +43,28 @@ class _SkyBackground(torch.autograd.Function):
         return (denv,) + (None,) * 9
 
 
+MISS_MESSAGE = "a camera ray does not intersect the sky sphere (camera outside the radius-%g sphere)" % RADIUS
+
+
+class _SkyBatch(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, env_map, c2w, campos, intrinsics, radius, H, W):
+        import fdgs
+        env = env_map.detach().contiguous()
+        sky, miss = fdgs.ext().sky_forward_batch(env, c2w, campos, intrinsics, radius, H, W)
+        ctx.save_for_backward(env, c2w, campos, intrinsics)
+        ctx.radius = radius
+        ctx.mark_non_differentiable(miss)
+        return sky, miss
+
+    @staticmethod
+    def backward(ctx, grad_sky, _grad_miss):
+        import fdgs
+        env, c2w, campos, intrinsics = ctx.saved_tensors
+        denv = fdgs.ext().sky_backward_batch(env, c2w, campos, intrinsics, ctx.radius, grad_sky.contiguous())
+        return (denv,) + (None,) * 6
+
+
 class MissFlag:
     """Whether any ray of a sky_background() call missed the sphere (a camera outside it looking away).  The device flag
     travels to pinned host memory right behind the sky kernel; check() waits only for that copy, so called after the
@@ -53,7 +79,7 @@ class MissFlag:
     def check(self):
         self.ready.synchronize()
         # the reference asserts the same condition on its ray / sphere discriminant
-        assert int(self.host[0]) == 0, "a camera ray does not intersect the sky sphere (camera outside the radius-%g sphere)" % RADIUS
+        assert int(self.host[0]) == 0, MISS_MESSAGE
 
 
 def sample_sky(env_map, camera, radius=RADIUS):
@@ -76,3 +102,16 @@ def sky_background(env_map, camera, radius=RADIUS):
     sky, miss = sample_sky(env_map, camera, radius)
     miss.check()
     return sky
+
+
+def sample_sky_batch(env_map, views, radius=RADIUS):
+    """(sky [B,3,H,W], miss int32 [1] on the device) -- the sky of every camera of `views`, an fdgs.graph.StaticViews
+    built with sky=True; gradients flow to env_map, summed over the views.  View b's sky equals sample_sky(env_map,
+    camera b) bit for bit.  miss is 1 if a ray of any view missed the sphere; nothing here reads it (the reference
+    asserts on it: raise AssertionError(MISS_MESSAGE) once it is read)."""
+    if env_map.dim() != 3 or env_map.shape[0] != 3 or env_map.dtype != torch.float32 or not env_map.is_cuda:
+        raise ValueError("env_map must be a float32 CUDA tensor [3,Hm,Wm], got %s %s on %s"
+                         % (tuple(env_map.shape), env_map.dtype, env_map.device))
+    if getattr(views, "c2w", None) is None:
+        raise ValueError("sample_sky_batch needs StaticViews(..., sky=True) (camera-to-world and intrinsics tables)")
+    return _SkyBatch.apply(env_map, views.c2w, views.campos, views.intrinsics, float(radius), views.H, views.W)

@@ -17,7 +17,7 @@ from torch.nn import functional as F
 from .diff_gaussian_rasterization import (BatchRasterizationSettings, GaussianRasterizationSettings, GaussianRasterizer,
                                           rasterize_gaussians_batch)
 from . import pyprep
-from fdgs.sky import sample_sky
+from fdgs.sky import sample_sky, sample_sky_batch
 
 __all__ = ["render", "render_batch", "GaussianRasterizationSettings", "GaussianRasterizer"]
 
@@ -211,9 +211,11 @@ def render_batch(viewpoint_cameras, pc, pipe, bg_color: torch.Tensor, scaling_mo
     `viewpoint_cameras` may also be an fdgs.graph.StaticViews: the cameras then come from its device tensors, the
     rasterizer is sized by its instance capacity and never synchronises with the host (the call can be captured in a CUDA
     graph), and the result has an eighth key, "status" (int32 [4] on the device: instances R, largest tile, overflow,
-    wrap; on overflow every view renders as if no Gaussian were listed).  An environment map and pipe.debug are not
-    supported then (ValueError): the sky sampler inverts the cameras and checks its miss flag on the host, and debug
-    synchronises after every stage."""
+    wrap; on overflow every view renders as if no Gaussian were listed).  pipe.debug is not supported then (ValueError:
+    it synchronises after every stage).  An environment map needs StaticViews(..., sky=True) (ValueError otherwise): the
+    sky of every view is then sampled by one batched call on the views' device cameras (fdgs.sky.sample_sky_batch), and
+    the result has a ninth key, "sky_miss" (int32 [1] on the device: 1 if a ray missed the sky sphere), which nothing
+    here reads -- the caller asserts on it, as fdgs.graph.GraphedStep does."""
     from fdgs.graph import StaticViews
     views = viewpoint_cameras if isinstance(viewpoint_cameras, StaticViews) else None
     cams = None if views is not None else list(viewpoint_cameras)
@@ -230,8 +232,9 @@ def render_batch(viewpoint_cameras, pc, pipe, bg_color: torch.Tensor, scaling_mo
         raise ValueError("render_batch cannot run inside an active ViewParallelStep; render its views with render()")
     env_map_res = getattr(pipe, "env_map_res", 0)
     if views is not None:
-        if env_map_res:
-            raise ValueError("render_batch with StaticViews does not support an environment map (its sampler synchronises)")
+        if env_map_res and getattr(views, "c2w", None) is None:
+            raise ValueError("render_batch with an environment map needs StaticViews(..., sky=True): these views carry no "
+                             "sky tables")
         if pipe.debug:
             raise ValueError("render_batch with StaticViews does not support pipe.debug (it synchronises after every stage)")
         B, H, W = views.B, views.H, views.W
@@ -268,9 +271,12 @@ def render_batch(viewpoint_cameras, pc, pipe, bg_color: torch.Tensor, scaling_mo
         prefiltered=False, debug=pipe.debug, **cameras)
     capacity = None if views is None else views.capacity
 
-    sky = None
+    sky = sky_miss = None
     misses = []
-    if env_map_res:
+    if env_map_res and views is not None:
+        assert pc.env_map is not None
+        sky, sky_miss = sample_sky_batch(pc.env_map, views)
+    elif env_map_res:
         assert pc.env_map is not None
         skies = []
         for c in cams:
@@ -302,4 +308,6 @@ def render_batch(viewpoint_cameras, pc, pipe, bg_color: torch.Tensor, scaling_mo
            "depth": depth, "alpha": alpha, "flow": flow}
     if views is not None:
         pkg["status"] = out[5]
+        if sky_miss is not None:
+            pkg["sky_miss"] = sky_miss
     return pkg

@@ -337,6 +337,24 @@ typedef struct fdgs_sky_args {
 int fdgs_sky_forward(const fdgs_sky_args* args, float* out_sky, int* miss_flag, void* stream);
 /* dL_denv [3,Hm,Wm] += the share of dL_dsky [3,H,W] of every texel (accumulated: zero it for a fresh gradient). */
 int fdgs_sky_backward(const fdgs_sky_args* args, const float* dL_dsky, float* dL_denv, void* stream);
+/* The sky of B views of one image size in one launch each way, every camera read from device tables, so that neither
+ * entry synchronises or reads device memory on the host (a CUDA graph can capture both).  View b's sky is
+ * fdgs_sky_forward's with c2w = c2w[b], campos = campos[b] and (fl_x, fl_y, cx, cy) = intrinsics[b], bit for bit. */
+typedef struct fdgs_sky_batch_args {
+    const float* env_map;         /* [3,Hm,Wm]                                 */
+    int env_height, env_width;    /* Hm, Wm                                    */
+    const float* c2w;             /* device [B,16] row-major camera-to-world, as fdgs_sky_args.c2w */
+    const float* campos;          /* device [B,3] ray origins (camera centres) */
+    const float* intrinsics;      /* device [B,4] fl_x, fl_y, cx, cy in pixels */
+    float radius;                 /* sky sphere radius (60 in the reference)   */
+    int width, height;            /* image size W, H                           */
+    int B;                        /* views, >= 1                               */
+} fdgs_sky_batch_args;
+/* out_sky [B,3,H,W] overwritten; miss_flag (device int, or NULL) is set to 1 if any ray of any view does not cross the
+ * sphere, and never cleared. */
+int fdgs_sky_forward_batch(const fdgs_sky_batch_args* args, float* out_sky, int* miss_flag, void* stream);
+/* dL_denv [3,Hm,Wm] += the share of every view's dL_dsky [B,3,H,W] of every texel (accumulated: zero it first). */
+int fdgs_sky_backward_batch(const fdgs_sky_batch_args* args, const float* dL_dsky, float* dL_denv, void* stream);
 
 /* present[i] = (view-space z of means3D[i] > 0.2)
  * (reference: rasterizer_impl.cu:54-67, auxiliary.h:140-163). */

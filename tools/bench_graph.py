@@ -2,9 +2,9 @@
 
     python tools/bench_graph.py [--steps 30] [--warmup 5] [--only lego-400,trex]
 
-For each workload (lego-800, lego-400, hook, trex, dynerf; the sky variant is left out, the graph does not take an
-environment map) the same seeded scene and cameras run two arms, alternating step by step:
-  eager  render_batch(cams) -> the B fused L1/SSIM losses -> one backward()
+For each workload (lego-800, lego-400, hook, trex, dynerf, dynerf-sky: dynerf with a 500^2 environment map) the same
+seeded scene and cameras run two arms, alternating step by step:
+  eager  render_batch(cams) -> the B fused L1/SSIM losses -> one backward() (with a map: the per-view sky sampler)
   graph  fdgs.graph.GraphedStep around the same step over StaticViews: one graph replay + one status read
 Reported per workload: the median CUDA-event step time of each arm, the median host time to enqueue a step (the host
 clock from the call until it returns, without the graph's final status read, i.e. the time the host needs before the
@@ -31,7 +31,7 @@ for p in (os.path.join(ROOT, "4d-gaussian-splatting_b200"), os.path.join(ROOT, "
 
 from bench_batch import DEV, WORKLOADS as BATCH_WORKLOADS, _Pipe, _setup, gpu_info  # noqa: E402
 
-WORKLOADS = {n: BATCH_WORKLOADS[n] for n in ("lego-800", "lego-400", "hook", "trex", "dynerf")}
+WORKLOADS = {n: BATCH_WORKLOADS[n] for n in ("lego-800", "lego-400", "hook", "trex", "dynerf", "dynerf-sky")}
 
 
 def _step_fn(pc, pipe, bg):
@@ -47,9 +47,9 @@ def _step_fn(pc, pipe, bg):
 
 
 def bench(name, w, steps, warmup):
-    from fdgs.graph import GraphedStep
+    from fdgs.graph import GraphedStep, _leaves
     pc, cams, gts = _setup(w)
-    pipe, bg = _Pipe(False), torch.zeros(3, device=DEV)
+    pipe, bg = _Pipe(w.get("sky")), torch.zeros(3, device=DEV)
     gt = torch.stack(gts)
     fn = _step_fn(pc, pipe, bg)
     out = {"workload": name, "P": w["P"], "W": w["W"], "H": w["H"], "B": w["B"]}
@@ -73,7 +73,15 @@ def bench(name, w, steps, warmup):
     torch.cuda.synchronize()
 
     # graph arm: the first call warms up, sizes the capacity and captures
-    step = GraphedStep(fn, pc.leaves)
+    if w.get("sky"):
+        # the graph steps a learned map only as the "env_map" group of the model's FusedAdam (its gradient must be
+        # one of the step's leaves)
+        from bench_graph_iteration import _model
+        params = _model(pc)
+    else:
+        params = pc.leaves
+    leaves = lambda: _leaves(params)     # noqa: E731  (the order GraphedStep's calls use)
+    step = GraphedStep(fn, params)
     base = torch.cuda.memory_allocated()
     torch.cuda.reset_peak_memory_stats()
     t0 = time.perf_counter()
@@ -82,10 +90,10 @@ def bench(name, w, steps, warmup):
     out["first_call_ms"] = round(1e3 * (time.perf_counter() - t0), 1)
     out["graph_peak_extra_MB"] = round((torch.cuda.max_memory_allocated() - base) / 2 ** 20, 1)
     t0 = time.perf_counter()
-    step._capture(pc.leaves())     # a capture alone (the graph is rebuilt in place; the next call replays it)
+    step._capture(leaves())     # a capture alone (the graph is rebuilt in place; the next call replays it)
     torch.cuda.synchronize()
     out["capture_ms"] = round(1e3 * (time.perf_counter() - t0), 1)
-    step._replay(pc.leaves())
+    step._replay(leaves())
     for _ in range(warmup):
         step(cams, gt)
 

@@ -3,17 +3,21 @@ workloads.
 
     python tools/bench_graph_iteration.py [--iters 20] [--rounds 15] [--warmup 5] [--only lego-400,trex]
 
-For each workload (lego-800, lego-400, hook, trex, dynerf, and lego-400-rigid: lego-400 with the rigidity loss, k = 20,
-its neighbour list rebuilt inside the step) two copies of the same seeded scene, each with a FusedAdam over nine named
-groups and the densification accumulators, run two arms in alternating blocks of iterations:
+For each workload (lego-800, lego-400, hook, trex, dynerf, lego-400-rigid: lego-400 with the rigidity loss, k = 20,
+its neighbour list rebuilt inside the step, and dynerf-sky: dynerf with a learned 500^2 environment map) two copies of
+the same seeded scene, each with a FusedAdam over nine named groups (with a map, a tenth, "env_map", at the features'
+learning rate) and the densification accumulators, run two arms in alternating blocks of iterations:
   eager-tail  GraphedStep(fn) -> ViewBatchStats + B add_view + add_densification_stats -> FusedAdam.step() -> zero_grad
               (the INTEGRATION loop before the optimiser joined the graph)
+  eager       (dynerf-sky, in place of eager-tail: before this graph took a map) fn(cams, gt) eagerly, render_batch
+              over the camera list with the per-view sky sampler, then the same tail; the one FusedAdam step is both
+              the Gaussians' and the map's Adam step
   graph       GraphedStep(fn, optimizer=FusedAdam)(cams, gt, densify_stats=True): statistics and Adam in the capture
 Both set the xyz learning rate every iteration.  fn = render_batch + B fused L1/SSIM losses (+ the rigidity loss) +
 backward.  Reported per workload: the median iteration time of each arm (host clock over a block of iterations ending in
 a device synchronise, divided by the block length) with its inter-quartile range over the blocks, the median host time
 to enqueue one iteration (inputs, staging and replay, plus for eager-tail the statistics and optimiser launches; the
-status read is excluded), captures and overflows, and the peak memory of the first iteration above the resident scene.
+status read is excluded; not given for the eager arm, which synchronises inside its forward), captures and overflows, and the peak memory of the first iteration above the resident scene.
 Then, in a separate profiled run, the fused Adam kernel's time per step, eager (adam_kernel) against staged
 (adam_staged_kernel), from torch.profiler.  One JSON line each, with the GPU's name, power limit and max SM clock read in
 the same process.  Writes nothing into the tree.
@@ -37,6 +41,7 @@ from bench_batch import DEV, WORKLOADS as BATCH_WORKLOADS, _Pipe, _setup, gpu_in
 
 WORKLOADS = {n: BATCH_WORKLOADS[n] for n in ("lego-800", "lego-400", "hook", "trex", "dynerf")}
 WORKLOADS["lego-400-rigid"] = dict(BATCH_WORKLOADS["lego-400"], rigid=20)
+WORKLOADS["dynerf-sky"] = BATCH_WORKLOADS["dynerf-sky"]
 GROUPS = [("xyz", "_xyz", 1.6e-4), ("t", "_t", 1.6e-4), ("f_dc", "_features_dc", 2.5e-3),
           ("f_rest", "_features_rest", 2.5e-3 / 20), ("opacity", "_opacity", 5e-2), ("scaling", "_scaling", 5e-3),
           ("scaling_t", "_scaling_t", 5e-3), ("rotation", "_rotation", 1e-3), ("rotation_r", "_rotation_r", 1e-3)]
@@ -47,6 +52,8 @@ def _model(m):
     densification accumulators."""
     from fdgs.optim import FusedAdam
     m.optimizer = FusedAdam([{"params": [getattr(m, a)], "lr": lr, "name": n} for n, a, lr in GROUPS], lr=0.0, eps=1e-15)
+    if m.env_map is not None:      # the reference's Adam([env_map], lr=feature_lr, eps=1e-15)
+        m.optimizer.add_param_group({"params": [m.env_map], "lr": 2.5e-3, "name": "env_map"})
     P = m._xyz.shape[0]
     m.xyz_gradient_accum, m.t_gradient_accum = torch.zeros(P, 1, device=DEV), torch.zeros(P, 1, device=DEV)
     m.denom, m.max_radii2D = torch.zeros(P, 1, device=DEV), torch.zeros(P, device=DEV)
@@ -86,10 +93,10 @@ def _tail(m, pkg, B):
 
 def bench(name, w, iters, rounds, warmup):
     from fdgs.graph import GraphedStep
-    pipe, bg = _Pipe(False), torch.zeros(3, device=DEV)
+    pipe, bg = _Pipe(w.get("sky")), torch.zeros(3, device=DEV)
     out = {"workload": name, "P": w["P"], "W": w["W"], "H": w["H"], "B": w["B"], "rigid_k": w.get("rigid", 0)}
     arms = {}
-    for arm in ("eager_tail", "graph"):
+    for arm in ("eager" if w.get("sky") else "eager_tail", "graph"):
         pc, cams, gts = _setup(w)
         m = _model(pc)
         gt = torch.stack(gts)
@@ -100,6 +107,9 @@ def bench(name, w, iters, rounds, warmup):
         if arm == "graph":
             step = GraphedStep(fn, m, optimizer=m.optimizer)
             call = lambda it, s=step, m=m: (_set_lr(m, it), s(cams, gt, densify_stats=True))   # noqa: E731
+        elif arm == "eager":
+            step = None
+            call = lambda it, fn=fn, m=m: (_set_lr(m, it), _tail(m, fn(cams, gt)[1], w["B"]))  # noqa: E731
         else:
             step = GraphedStep(fn, m)
             call = lambda it, s=step, m=m: (_set_lr(m, it), _tail(m, s(cams, gt)[1], w["B"]))  # noqa: E731
@@ -123,9 +133,12 @@ def bench(name, w, iters, rounds, warmup):
         q = sorted(a["times"])
         out[arm + "_ms"] = round(statistics.median(q), 3)
         out[arm + "_ms_iqr"] = [round(q[len(q) // 4], 3), round(q[(3 * len(q)) // 4], 3)]
+        if a["step"] is None:
+            out[arm + "_enqueue_ms"] = None
+            continue
         out[arm + "_enqueue_ms"] = round(_enqueue(arm, a), 3)
         out[arm + "_captures"], out[arm + "_overflows"] = a["step"].info["captures"], a["step"].info["overflows"]
-    out["speedup"] = round(out["eager_tail_ms"] / out["graph_ms"], 3)
+    out["speedup"] = round(out[("eager" if w.get("sky") else "eager_tail") + "_ms"] / out["graph_ms"], 3)
     out.update(_adam_kernels(arms["graph"]["m"]))
     return out
 
