@@ -266,6 +266,9 @@ size_t fdgs_image_batch_bytes(int width, int height, int B) {
     return ImageState::carve(nullptr, width, height, B > 0 ? B : 0).bytes + 128;
 }
 size_t fdgs_backward_batch_scratch_bytes(int P, int B) { return BatchBwdScratch::carve(nullptr, P, B).bytes + 128; }
+size_t fdgs_camera_grad_scratch_bytes(int P, int B) {
+    return (size_t)fdgs::CAM_TERMS * fdgs::camera_grad_blocks(P) * (size_t)(B > 0 ? B : 0) * sizeof(float) + 128;
+}
 
 }  // extern "C"
 
@@ -458,12 +461,29 @@ int forward_impl(const fdgs_forward_args* a, const float* bg_image, float* zero_
                           reinterpret_cast<cudaStream_t>(stream_v), res);
 }
 
+// The camera gradient of `views` views with no Gaussian: zeros (fdgs_backward_camera)
+int camera_grad_zero(const fdgs::CameraGradParams& cam, int views, bool debug, cudaStream_t stream) {
+    FDGS_STAGE(7, 1, fdgs::launch_camera_grad_finish(cam, 0, views, stream), "camera_grad (no Gaussian)");
+    return FDGS_OK;
+}
+
+// The camera outputs of fdgs_backward_camera / fdgs_backward_batch_camera, checked before anything is launched
+int camera_grad_params(const fdgs_camera_grad_out* c, fdgs::CameraGradParams* p) {
+    if (!c || !c->dL_dviewmatrix || !c->dL_dprojmatrix || !c->dL_dcampos || !c->scratch)
+        return fail(FDGS_ERR_INVALID_ARG, "camera gradient outputs (dL_dviewmatrix / dL_dprojmatrix / dL_dcampos) and scratch required");
+    p->partials = reinterpret_cast<float*>(align128(c->scratch));
+    p->dL_dviewmatrix = c->dL_dviewmatrix; p->dL_dprojmatrix = c->dL_dprojmatrix; p->dL_dcampos = c->dL_dcampos;
+    return FDGS_OK;
+}
+
 // The backward's stages on the forward's buffers: the blend backward (when there is an instance or dL_dbg_image to
 // write), then the per-Gaussian backward (when there is a Gaussian).  vb as in forward_stages; for a batch, a's
 // gradient outputs are the per-view stacks of BatchBwdScratch.  sh_rows_zeroed: the forward zeroed the non-rendered
-// dL_dsh rows (fdgs_backward_zero_sh).  The arguments have been checked by the entry.
+// dL_dsh rows (fdgs_backward_zero_sh).  cam: also the camera gradient (fdgs_backward_camera), or NULL.  The arguments
+// have been checked by the entry.
 int backward_stages(const fdgs_backward_args* a, const float* bg_image, float* dL_dbg_image, int sh_rows_zeroed,
-                    const fdgs::ViewBatch& vb, const GeomState& geom, const ImageState& img, cudaStream_t stream) {
+                    const fdgs::ViewBatch& vb, const GeomState& geom, const ImageState& img, cudaStream_t stream,
+                    const fdgs::CameraGradParams* cam = nullptr) {
     const bool debug = a->debug != 0, batch = vb.scalars != nullptr;
     const int P = a->P, W = a->width, H = a->height, R = a->R;
     BinningState bin = BinningState::carve(a->binning_buffer ? align128(const_cast<char*>(a->binning_buffer)) : nullptr, R);
@@ -482,7 +502,7 @@ int backward_stages(const fdgs_backward_args* a, const float* bg_image, float* d
         bp.views = batch ? vb.B : 0; bp.P = P;
         FDGS_STAGE(6, 1, fdgs::launch_blend_bwd(bp, stream), batch ? "blend_bwd (batch)" : "blend_bwd");
     }
-    if (P <= 0) return FDGS_OK;
+    if (P <= 0) return cam ? camera_grad_zero(*cam, batch ? vb.B : 1, debug, stream) : FDGS_OK;
     fdgs::PreprocessBwdParams pb;
     memset(&pb, 0, sizeof(pb));
     pb.P = P; pb.D = a->D; pb.D_t = a->D_t; pb.M = a->M;
@@ -509,17 +529,18 @@ int backward_stages(const fdgs_backward_args* a, const float* bg_image, float* d
     pb.dL_dts = a->dL_dts;
     pb.dL_dscale = a->dL_dscale; pb.dL_dscale_t = a->dL_dscale_t; pb.dL_drot = a->dL_drot; pb.dL_drot_r = a->dL_drot_r;
     pb.vb = vb; pb.factor_stride = BatchBwdScratch::factor_stride(P);
-    FDGS_STAGE(7, fdgs::preprocess_bwd_kernel_count(pb), fdgs::launch_preprocess_bwd(pb, stream),
+    FDGS_STAGE(7, fdgs::preprocess_bwd_kernel_count(pb) + (cam ? 1 : 0), fdgs::launch_preprocess_bwd(pb, stream, cam),
                batch ? "preprocess_bwd (batch)" : "preprocess_bwd");
     return FDGS_OK;
 }
 
 int backward_impl(const fdgs_backward_args* a, const float* bg_image, float* dL_dbg_image, int sh_rows_zeroed,
-                  void* stream_v) {
+                  void* stream_v, const fdgs::CameraGradParams* cam = nullptr) {
     g_last_error.clear();
     if (!a) return fail(FDGS_ERR_INVALID_ARG, "null argument");
     const int P = a->P, W = a->width, H = a->height, R = a->R;
-    if (P <= 0 && !dL_dbg_image) return FDGS_OK;
+    if (P <= 0 && !dL_dbg_image)
+        return cam ? camera_grad_zero(*cam, 1, a->debug != 0, reinterpret_cast<cudaStream_t>(stream_v)) : FDGS_OK;
     if (W <= 0 || H <= 0 || R < 0) return fail(FDGS_ERR_INVALID_ARG, "bad width / height / R");
     if (P <= 0) {
         if (!a->image_buffer || !a->dL_dpix || !a->background)
@@ -544,7 +565,7 @@ int backward_impl(const fdgs_backward_args* a, const float* bg_image, float* dL_
     GeomState geom = GeomState::carve(align128(const_cast<char*>(a->geom_buffer)), P);
     ImageState img = ImageState::carve(align128(const_cast<char*>(a->image_buffer)), W, H);
     return backward_stages(a, bg_image, dL_dbg_image, sh_rows_zeroed, {1, nullptr}, geom, img,
-                           reinterpret_cast<cudaStream_t>(stream_v));
+                           reinterpret_cast<cudaStream_t>(stream_v), cam);
 }
 
 // ---- batched views: B cameras of the same Gaussians in one pass per stage (include/fdgs.h: fdgs_forward_batch) -------
@@ -629,7 +650,7 @@ int forward_batch_impl(const fdgs_forward_batch_args* b, const fdgs_forward_capa
                           res);
 }
 
-int backward_batch_impl(const fdgs_backward_batch_args* b, void* stream_v) {
+int backward_batch_impl(const fdgs_backward_batch_args* b, void* stream_v, const fdgs::CameraGradParams* cam = nullptr) {
     g_last_error.clear();
     if (!b) return fail(FDGS_ERR_INVALID_ARG, "null argument");
     const fdgs_backward_args* a = &b->view;
@@ -647,7 +668,7 @@ int backward_batch_impl(const fdgs_backward_batch_args* b, void* stream_v) {
     GeomState geom = GeomState::carve(align128(const_cast<char*>(a->geom_buffer)), P, true, B);
     ImageState img = ImageState::carve(align128(const_cast<char*>(a->image_buffer)), W, H, B);
     const fdgs::ViewBatch vb = {B, geom.scalars};
-    if (P == 0) return backward_stages(a, b->bg_image, b->dL_dbg_image, 0, vb, geom, img, stream);
+    if (P == 0) return backward_stages(a, b->bg_image, b->dL_dbg_image, 0, vb, geom, img, stream, cam);
     if (R > 0 && !a->binning_buffer) return fail(FDGS_ERR_INVALID_ARG, "scratch buffers of the forward pass required");
     if (!a->radii || !a->out_means3D || !a->viewmatrix || !a->projmatrix || !a->campos)
         return fail(FDGS_ERR_INVALID_ARG, "radii / out_means3D / viewmatrix / projmatrix / campos required");
@@ -671,7 +692,7 @@ int backward_batch_impl(const fdgs_backward_batch_args* b, void* stream_v) {
     views.dL_dsh = nullptr; views.sh_factors = sc.table; views.dL_dsh_rest = nullptr; views.dL_dts = sc.dL_dts;
     views.dL_dscale = sc.dL_dscale; views.dL_dscale_t = sc.dL_dscale_t; views.dL_drot = sc.dL_drot;
     views.dL_drot_r = sc.dL_drot_r;
-    if (int rc = backward_stages(&views, b->bg_image, b->dL_dbg_image, 0, vb, geom, img, stream)) return rc;
+    if (int rc = backward_stages(&views, b->bg_image, b->dL_dbg_image, 0, vb, geom, img, stream, cam)) return rc;
 
     // every per-Gaussian gradient but the SH rows: summed over the views in view order
     fdgs::ViewSumParams vsum;
@@ -791,6 +812,21 @@ int fdgs_forward_batch_capacity(const fdgs_forward_capacity_args* args, fdgs_all
 }
 
 int fdgs_backward_batch(const fdgs_backward_batch_args* args, void* stream) { return backward_batch_impl(args, stream); }
+
+int fdgs_backward_camera(const fdgs_backward_args* a, const float* bg_image, float* dL_dbg_image, int sh_rows_zeroed,
+                         const fdgs_camera_grad_out* cam, void* stream) {
+    g_last_error.clear();
+    fdgs::CameraGradParams c;
+    if (int rc = camera_grad_params(cam, &c)) return rc;
+    return backward_impl(a, bg_image, dL_dbg_image, sh_rows_zeroed, stream, &c);
+}
+
+int fdgs_backward_batch_camera(const fdgs_backward_batch_args* args, const fdgs_camera_grad_out* cam, void* stream) {
+    g_last_error.clear();
+    fdgs::CameraGradParams c;
+    if (int rc = camera_grad_params(cam, &c)) return rc;
+    return backward_batch_impl(args, stream, &c);
+}
 
 int fdgs_sky_forward(const fdgs_sky_args* a, float* out_sky, int* miss_flag, void* stream_v) {
     g_last_error.clear();

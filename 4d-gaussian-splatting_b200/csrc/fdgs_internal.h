@@ -224,7 +224,24 @@ struct PreprocessBwdParams {
     ViewBatch vb;
     long long factor_stride;
 };
-cudaError_t launch_preprocess_bwd(const PreprocessBwdParams& p, cudaStream_t stream);
+// The camera gradient (fdgs_backward_camera): geom_bwd reduces each rendered row's CAM_TERMS terms per block into
+// `partials`, a [views][CAM_TERMS][camera_grad_blocks(P)] scratch, and one small kernel sums the blocks.  Term slots, in
+// the torch tensors' [4,4] layout (element [c][r] = V[4c + r]):
+//   0..11   dL/dviewmatrix[c][r], c = 0..3, r = 0..2   (column 3, the view-space w, is not used: 0)
+//   12..23  dL/dprojmatrix[c][r], c = 0..3, r = 0, 1, 3 (column 2, clip z, is not used: 0)
+//   24..26  dL/dcampos
+constexpr int CAM_TERMS = 27;
+struct CameraGradParams {
+    float* partials;
+    float* dL_dviewmatrix;   // [views,16] overwritten
+    float* dL_dprojmatrix;   // [views,16] overwritten
+    float* dL_dcampos;       // [views,3]  overwritten
+};
+int camera_grad_blocks(int P);
+// the views' outputs from `blocks` partials per term (blocks == 0: zeros)
+cudaError_t launch_camera_grad_finish(const CameraGradParams& c, int blocks, int views, cudaStream_t stream);
+// cam != NULL: geom_bwd also reduces the camera gradient (one more launch)
+cudaError_t launch_preprocess_bwd(const PreprocessBwdParams& p, cudaStream_t stream, const CameraGradParams* cam = nullptr);
 int preprocess_bwd_kernel_count(const PreprocessBwdParams& p);
 // dst_i[e] = ((src_i[0][e] + src_i[1][e]) + src_i[2][e]) + ... in fp32, view order: the order in which autograd's
 // AccumulateGrad builds .grad over a sequential loop of views.  src_i is a [B][n_i] stack.

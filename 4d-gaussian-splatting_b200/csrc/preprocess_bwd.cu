@@ -633,8 +633,10 @@ __device__ __forceinline__ void mat3_mul(const float A[3][3], const float B[3][3
 }
 
 // ---- geometry backward ---------------------------------------------------------------------------
-template <bool BATCH>
-__device__ __forceinline__ void geom_bwd_body(const PreprocessBwdParams& a_, const int has_sh_part) {
+// CAM: also write the rendered row's CAM_TERMS camera terms to cam[s * GB_THREADS] (s = the slot, see
+// CameraGradParams); the caller zeroes the slots, so rows that are not rendered contribute 0
+template <bool BATCH, bool CAM = false>
+__device__ __forceinline__ void geom_bwd_body(const PreprocessBwdParams& a_, const int has_sh_part, float* cam = nullptr) {
     // an lvalue on both sides: the single-view instantiation reads its parameters in place, no copy
     PreprocessBwdParams view_;
     if (BATCH) view_ = preprocess_bwd_view(a_, blockIdx.y);
@@ -727,6 +729,24 @@ __device__ __forceinline__ void geom_bwd_body(const PreprocessBwdParams& a_, con
             g_mean[0] = V[0] * vx + V[1] * vy + V[2] * vz;
             g_mean[1] = V[4] * vx + V[5] * vy + V[6] * vz;
             g_mean[2] = V[8] * vx + V[9] * vy + V[10] * vz;
+            if (CAM) {
+                // view-space point t = W m + V[12..14]: dL/dV[4c + r] = m_c g_r with m_3 = 1, g = (vx, vy, vz); plus,
+                // on c < 3, the W part of T = J W (build_T): dL/dW[r][c] = sum_i J[i][r] dL/dT[i][c], W[r][c] = V[4c + r]
+                const float j00 = fdiv(h_x, Pj.tz), j11 = fdiv(h_y, Pj.tz);
+                const float j02 = fdiv(fmul(h_x, -Pj.tx), fmul(Pj.tz, Pj.tz));
+                const float j12 = fdiv(fmul(h_y, -Pj.ty), fmul(Pj.tz, Pj.tz));
+                const float m[3] = {mx, my, mz};
+                const float dT0[3] = {dL_dT00, dL_dT01, dL_dT02}, dT1[3] = {dL_dT10, dL_dT11, dL_dT12};
+#pragma unroll
+                for (int c = 0; c < 3; ++c) {
+                    cam[(3 * c + 0) * GB_THREADS] = m[c] * vx + j00 * dT0[c];
+                    cam[(3 * c + 1) * GB_THREADS] = m[c] * vy + j11 * dT1[c];
+                    cam[(3 * c + 2) * GB_THREADS] = m[c] * vz + (j02 * dT0[c] + j12 * dT1[c]);
+                }
+                cam[9 * GB_THREADS] = vx;
+                cam[10 * GB_THREADS] = vy;
+                cam[11 * GB_THREADS] = vz;
+            }
         }
 
         // ---------------- preprocessCUDA (backward), backward.cu:877-894 ----------------
@@ -739,6 +759,16 @@ __device__ __forceinline__ void geom_bwd_body(const PreprocessBwdParams& a_, con
             g_mean[0] += (Pm[0] * m_w - Pm[3] * mul1) * d2x + (Pm[1] * m_w - Pm[3] * mul2) * d2y;
             g_mean[1] += (Pm[4] * m_w - Pm[7] * mul1) * d2x + (Pm[5] * m_w - Pm[7] * mul2) * d2y;
             g_mean[2] += (Pm[8] * m_w - Pm[11] * mul1) * d2x + (Pm[9] * m_w - Pm[11] * mul2) * d2y;
+            if (CAM) {
+                // homogeneous projection p = P [m, 1]: dL/dPm[4c + r] = m_c gp_r, gp = (d2x m_w, d2y m_w, 0 (clip z is
+                // not used), -(mul1 d2x + mul2 d2y)); the zero column is not reduced
+                const float gp[3] = {d2x * m_w, d2y * m_w, -(mul1 * d2x + mul2 * d2y)};
+                const float m[4] = {mx, my, mz, 1.f};
+#pragma unroll
+                for (int c = 0; c < 4; ++c)
+#pragma unroll
+                    for (int j = 0; j < 3; ++j) cam[(12 + 3 * c + j) * GB_THREADS] = m[c] * gp[j];
+            }
         }
 
         // SH view-direction / time terms left by sh_bwd_kernel (backward.cu:896-906)
@@ -747,6 +777,11 @@ __device__ __forceinline__ void geom_bwd_body(const PreprocessBwdParams& a_, con
             g_mean[1] += a.dL_dmean3D[3 * idx + 1];
             g_mean[2] += a.dL_dmean3D[3 * idx + 2];
             g_ts += a.dL_dts[idx];
+            if (CAM) {
+                // the view direction is m - campos: its gradient w.r.t. campos is minus the term w.r.t. the mean
+#pragma unroll
+                for (int k = 0; k < 3; ++k) cam[(24 + k) * GB_THREADS] = -a.dL_dmean3D[3 * idx + k];
+            }
         }
 
         // ---------------- covariance backward ----------------
@@ -887,6 +922,56 @@ __global__ void __launch_bounds__(GB_THREADS, 8) geom_bwd_batch_kernel(const Pre
     geom_bwd_body<true>(a_, has_sh_part);
 }
 
+// geom_bwd with the camera gradient: each block sums its rows' CAM_TERMS camera terms and writes one partial per term,
+// partials[(view * CAM_TERMS + term) * gridDim.x + blockIdx.x].  The terms wait in shared memory, not registers, while
+// the covariance chain runs (the kernel keeps geom_bwd's 8 CTAs per SM); then per term a butterfly over each warp and
+// the four warps in order.  No floating-point atomics: the result does not depend on scheduling.
+template <bool BATCH>
+__global__ void __launch_bounds__(GB_THREADS, 8) geom_bwd_cam_kernel(const PreprocessBwdParams a_, const int has_sh_part,
+                                                                     float* __restrict__ partials) {
+    __shared__ float terms[CAM_TERMS][GB_THREADS];
+    __shared__ float warp_sum[GB_THREADS / 32][CAM_TERMS];
+#pragma unroll
+    for (int s = 0; s < CAM_TERMS; ++s) terms[s][threadIdx.x] = 0.f;
+    geom_bwd_body<BATCH, true>(a_, has_sh_part, &terms[0][threadIdx.x]);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int s = 0; s < CAM_TERMS; ++s) {   // every slot is read back by the thread that wrote it
+        float v = terms[s][threadIdx.x];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == 0) warp_sum[warp][s] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < CAM_TERMS) {
+        float v = warp_sum[0][threadIdx.x];
+#pragma unroll
+        for (int w = 1; w < GB_THREADS / 32; ++w) v += warp_sum[w][threadIdx.x];
+        partials[((size_t)blockIdx.y * CAM_TERMS + threadIdx.x) * gridDim.x + blockIdx.x] = v;
+    }
+}
+
+// one block per view, one warp per term: the view's block partials summed in fp64 in a fixed order (lane l takes blocks
+// l, l + 32, ...; then a butterfly), rounded once, and scattered to the [16] / [16] / [3] outputs in the tensors'
+// layout, with exact zeros in the entries the forward does not use (see CameraGradParams)
+__global__ void __launch_bounds__(CAM_TERMS * 32) camera_grad_finish_kernel(const CameraGradParams c, const int blocks) {
+    const int view = blockIdx.x, s = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const float* src = c.partials + ((size_t)view * CAM_TERMS + s) * (size_t)blocks;
+    double acc = 0.0;
+    for (int b = lane; b < blocks; b += 32) acc += (double)src[b];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    if (lane == 0) {
+        const float v = (float)acc;
+        if (s < 12) c.dL_dviewmatrix[16 * view + 4 * (s / 3) + s % 3] = v;
+        else if (s < 24) c.dL_dprojmatrix[16 * view + 4 * ((s - 12) / 3) + ((s - 12) % 3 == 2 ? 3 : (s - 12) % 3)] = v;
+        else c.dL_dcampos[3 * view + s - 24] = v;
+    }
+    if (threadIdx.x < 4) {
+        c.dL_dviewmatrix[16 * view + 4 * threadIdx.x + 3] = 0.f;
+        c.dL_dprojmatrix[16 * view + 4 * threadIdx.x + 2] = 0.f;
+    }
+}
+
 // one thread per element of a tensor (blockIdx.y), its B view rows added in view order with round-to-nearest adds
 __global__ void __launch_bounds__(256) view_sum_kernel(const ViewSumParams p) {
     const int i = blockIdx.y;
@@ -925,7 +1010,7 @@ static PreprocessBwdKernel sh_bwd_for(bool factors) {
 }
 
 template <bool BATCH>
-static cudaError_t preprocess_bwd(const PreprocessBwdParams& p, cudaStream_t stream) {
+static cudaError_t preprocess_bwd(const PreprocessBwdParams& p, cudaStream_t stream, const CameraGradParams* cam) {
     const bool factors = p.sh_factors != nullptr;
     const bool has_sh = p.shs != nullptr && p.M > 0 && (p.dL_dsh != nullptr || factors);
     const unsigned views = BATCH ? (unsigned)p.vb.B : 1u;
@@ -945,14 +1030,28 @@ static cudaError_t preprocess_bwd(const PreprocessBwdParams& p, cudaStream_t str
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
+    const unsigned blocks = (unsigned)camera_grad_blocks(p.P);
+    if (cam) {
+        geom_bwd_cam_kernel<BATCH><<<dim3(blocks, views), GB_THREADS, 0, stream>>>(p, has_sh ? 1 : 0, cam->partials);
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+        return launch_camera_grad_finish(*cam, (int)blocks, (int)views, stream);
+    }
     const PreprocessBwdKernelG g = BATCH ? geom_bwd_batch_kernel : geom_bwd_kernel;
-    g<<<dim3((p.P + GB_THREADS - 1) / GB_THREADS, views), GB_THREADS, 0, stream>>>(p, has_sh ? 1 : 0);
+    g<<<dim3(blocks, views), GB_THREADS, 0, stream>>>(p, has_sh ? 1 : 0);
     return cudaGetLastError();
 }
 
-cudaError_t launch_preprocess_bwd(const PreprocessBwdParams& p, cudaStream_t stream) {
+cudaError_t launch_preprocess_bwd(const PreprocessBwdParams& p, cudaStream_t stream, const CameraGradParams* cam) {
     if (p.P <= 0) return cudaSuccess;
-    return p.vb.scalars ? preprocess_bwd<true>(p, stream) : preprocess_bwd<false>(p, stream);
+    return p.vb.scalars ? preprocess_bwd<true>(p, stream, cam) : preprocess_bwd<false>(p, stream, cam);
+}
+
+int camera_grad_blocks(int P) { return P > 0 ? (P + GB_THREADS - 1) / GB_THREADS : 0; }
+
+cudaError_t launch_camera_grad_finish(const CameraGradParams& c, int blocks, int views, cudaStream_t stream) {
+    camera_grad_finish_kernel<<<(unsigned)views, CAM_TERMS * 32, 0, stream>>>(c, blocks);
+    return cudaGetLastError();
 }
 
 cudaError_t launch_view_sum(const ViewSumParams& p, cudaStream_t stream) {

@@ -20,6 +20,10 @@
 //
 //   rasterize_gaussians_batch / rasterize_gaussians_backward_batch
 //
+// and the backward with the camera gradients (include/fdgs.h: fdgs_backward_camera), single-view and batched:
+//
+//   rasterize_gaussians_backward_camera / rasterize_gaussians_backward_batch_camera
+//
 // and the batched forward sized by an instance capacity, which never synchronises (include/fdgs.h:
 // fdgs_forward_batch_capacity): rasterize_gaussians_batch_capacity
 //
@@ -34,6 +38,7 @@
 #include <torch/extension.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <c10/cuda/CUDAStream.h>
+#include <memory>
 #include <string>
 #include <tuple>
 #include <vector>
@@ -311,8 +316,31 @@ ForwardOut RasterizeGaussiansCUDA(const torch::Tensor& background, const torch::
 //                   as the SH gradient with their rendered rows written (fdgs_backward_zero_sh); empty: allocated here
 // Returns 15 tensors: the 12 gradients (w.r.t. the raw parameters under raw_params; dL_dsh is [P,1,3] when sh_rest is
 // given), sh_factors [P,3], dL_dsh_rest [P,M-1,3] and dL_dbg_image [3,H,W]; a tensor not asked for comes back empty.
+namespace {
+// The camera gradients of a backward (include/fdgs.h: fdgs_backward_camera): viewmatrix-, projmatrix- and campos-shaped
+// float32 tensors, and the scratch of the reduction
+struct CameraGrads {
+    torch::Tensor view, proj, campos, scratch;
+    fdgs_camera_grad_out out;
+    CameraGrads(const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const torch::Tensor& cam_pos,
+                const torch::Tensor& like, int P, int B) {
+        auto opts = like.options().dtype(torch::kFloat32);
+        TORCH_CHECK(viewmatrix.numel() == 16ll * B && projmatrix.numel() == 16ll * B && cam_pos.numel() == 3ll * B,
+                    "fdgs: the camera gradient needs viewmatrix / projmatrix of 16 and campos of 3 elements per view");
+        view = torch::empty(viewmatrix.sizes(), opts);
+        proj = torch::empty(projmatrix.sizes(), opts);
+        campos = torch::empty(cam_pos.sizes(), opts);
+        scratch = torch::empty({(int64_t)fdgs_camera_grad_scratch_bytes(P, B)}, like.options().dtype(torch::kByte));
+        out.dL_dviewmatrix = view.data_ptr<float>();
+        out.dL_dprojmatrix = proj.data_ptr<float>();
+        out.dL_dcampos = campos.data_ptr<float>();
+        out.scratch = reinterpret_cast<char*>(scratch.data_ptr());
+    }
+};
+
+// rasterize_gaussians_backward_ext, and with `camera` rasterize_gaussians_backward_camera
 std::vector<torch::Tensor>
-RasterizeGaussiansBackwardExtZeroSh(const torch::Tensor& background, const torch::Tensor& means3D,
+backward_ext(const torch::Tensor& background, const torch::Tensor& means3D,
                               const torch::Tensor& out_means3D, const torch::Tensor& radii, const torch::Tensor& colors,
                               const torch::Tensor& flows_2d, const torch::Tensor& opacities, const torch::Tensor& ts,
                               const torch::Tensor& scales, const torch::Tensor& scales_t, const torch::Tensor& rotations,
@@ -327,7 +355,7 @@ RasterizeGaussiansBackwardExtZeroSh(const torch::Tensor& background, const torch
                               const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer, const bool debug,
                               const torch::Tensor& sh_rest, const bool raw_params, const torch::Tensor& bg_image,
                               const bool sh_factor_mode, const bool want_dbg, const torch::Tensor& sh_grad,
-                              const torch::Tensor& sh_rest_grad) {
+                              const torch::Tensor& sh_rest_grad, const bool camera) {
     TORCH_CHECK(means3D.is_cuda(), "means3D must be a CUDA tensor");
     const DeviceStream on(means3D);
     const int P = means3D.size(0);
@@ -365,8 +393,10 @@ RasterizeGaussiansBackwardExtZeroSh(const torch::Tensor& background, const torch
     // overwritten for every pixel by the blend backward
     torch::Tensor dL_dbg_image = want_dbg ? torch::empty({3, H, W}, opts) : torch::empty({0}, opts);
     const auto bgi_c = background_image(bg_image, means3D, H, W);
+    std::unique_ptr<CameraGrads> cam;
+    if (camera) cam.reset(new CameraGrads(viewmatrix, projmatrix, campos, means3D, P, 1));
 
-    if (P != 0 || want_dbg) {
+    if (P != 0 || want_dbg || camera) {
         fdgs_backward_args a;
         memset(&a, 0, sizeof(a));
         Inputs in;
@@ -388,12 +418,71 @@ RasterizeGaussiansBackwardExtZeroSh(const torch::Tensor& background, const torch
         a.dL_dts = dL_dts.data_ptr<float>(); a.dL_dscale = dL_dscales.data_ptr<float>();
         a.dL_dscale_t = dL_dscales_t.data_ptr<float>(); a.dL_drot = dL_drotations.data_ptr<float>();
         a.dL_drot_r = dL_drotations_r.data_ptr<float>();
-        check(fdgs_backward_zero_sh(&a, fptr(bgi_c), want_dbg ? dL_dbg_image.data_ptr<float>() : nullptr, zeroed ? 1 : 0,
-                                    (void*)on.stream),
-              "backward");
+        float* dbg = want_dbg ? dL_dbg_image.data_ptr<float>() : nullptr;
+        if (cam)
+            check(fdgs_backward_camera(&a, fptr(bgi_c), dbg, zeroed ? 1 : 0, &cam->out, (void*)on.stream), "backward_camera");
+        else
+            check(fdgs_backward_zero_sh(&a, fptr(bgi_c), dbg, zeroed ? 1 : 0, (void*)on.stream), "backward");
     }
-    return {dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dflows, dL_dts, dL_dscales,
-            dL_dscales_t, dL_drotations, dL_drotations_r, sh_factors, dL_dsh_rest, dL_dbg_image};
+    std::vector<torch::Tensor> out = {dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dflows,
+                                      dL_dts, dL_dscales, dL_dscales_t, dL_drotations, dL_drotations_r, sh_factors,
+                                      dL_dsh_rest, dL_dbg_image};
+    if (cam) out.insert(out.end(), {cam->view, cam->proj, cam->campos});
+    return out;
+}
+}  // namespace
+
+std::vector<torch::Tensor>
+RasterizeGaussiansBackwardExtZeroSh(const torch::Tensor& background, const torch::Tensor& means3D,
+                              const torch::Tensor& out_means3D, const torch::Tensor& radii, const torch::Tensor& colors,
+                              const torch::Tensor& flows_2d, const torch::Tensor& opacities, const torch::Tensor& ts,
+                              const torch::Tensor& scales, const torch::Tensor& scales_t, const torch::Tensor& rotations,
+                              const torch::Tensor& rotations_r, const float scale_modifier,
+                              const torch::Tensor& cov3D_precomp, const float prefilter_var,
+                              const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx,
+                              const float tan_fovy, const torch::Tensor& dL_dout_color, const torch::Tensor& dL_dout_depth,
+                              const torch::Tensor& dL_dout_mask, const torch::Tensor& dL_dout_flow, const torch::Tensor& sh,
+                              const int degree, const int degree_t, const torch::Tensor& campos, const float timestamp,
+                              const float time_duration, const bool rot_4d, const int gaussian_dim,
+                              const bool force_sh_3d, const torch::Tensor& geomBuffer, const int R,
+                              const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer, const bool debug,
+                              const torch::Tensor& sh_rest, const bool raw_params, const torch::Tensor& bg_image,
+                              const bool sh_factor_mode, const bool want_dbg, const torch::Tensor& sh_grad,
+                              const torch::Tensor& sh_rest_grad) {
+    return backward_ext(background, means3D, out_means3D, radii, colors, flows_2d, opacities, ts, scales, scales_t,
+                        rotations, rotations_r, scale_modifier, cov3D_precomp, prefilter_var, viewmatrix, projmatrix,
+                        tan_fovx, tan_fovy, dL_dout_color, dL_dout_depth, dL_dout_mask, dL_dout_flow, sh, degree, degree_t,
+                        campos, timestamp, time_duration, rot_4d, gaussian_dim, force_sh_3d, geomBuffer, R, binningBuffer,
+                        imageBuffer, debug, sh_rest, raw_params, bg_image, sh_factor_mode, want_dbg, sh_grad, sh_rest_grad,
+                        false);
+}
+
+// rasterize_gaussians_backward_ext's arguments (with the zeroed SH gradient tensors, empty when none); returns its 15
+// tensors and then dL_dviewmatrix, dL_dprojmatrix and dL_dcampos, shaped like viewmatrix, projmatrix and campos
+// (include/fdgs.h: fdgs_backward_camera)
+std::vector<torch::Tensor>
+RasterizeGaussiansBackwardCamera(const torch::Tensor& background, const torch::Tensor& means3D,
+                              const torch::Tensor& out_means3D, const torch::Tensor& radii, const torch::Tensor& colors,
+                              const torch::Tensor& flows_2d, const torch::Tensor& opacities, const torch::Tensor& ts,
+                              const torch::Tensor& scales, const torch::Tensor& scales_t, const torch::Tensor& rotations,
+                              const torch::Tensor& rotations_r, const float scale_modifier,
+                              const torch::Tensor& cov3D_precomp, const float prefilter_var,
+                              const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix, const float tan_fovx,
+                              const float tan_fovy, const torch::Tensor& dL_dout_color, const torch::Tensor& dL_dout_depth,
+                              const torch::Tensor& dL_dout_mask, const torch::Tensor& dL_dout_flow, const torch::Tensor& sh,
+                              const int degree, const int degree_t, const torch::Tensor& campos, const float timestamp,
+                              const float time_duration, const bool rot_4d, const int gaussian_dim,
+                              const bool force_sh_3d, const torch::Tensor& geomBuffer, const int R,
+                              const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer, const bool debug,
+                              const torch::Tensor& sh_rest, const bool raw_params, const torch::Tensor& bg_image,
+                              const bool sh_factor_mode, const bool want_dbg, const torch::Tensor& sh_grad,
+                              const torch::Tensor& sh_rest_grad) {
+    return backward_ext(background, means3D, out_means3D, radii, colors, flows_2d, opacities, ts, scales, scales_t,
+                        rotations, rotations_r, scale_modifier, cov3D_precomp, prefilter_var, viewmatrix, projmatrix,
+                        tan_fovx, tan_fovy, dL_dout_color, dL_dout_depth, dL_dout_mask, dL_dout_flow, sh, degree, degree_t,
+                        campos, timestamp, time_duration, rot_4d, gaussian_dim, force_sh_3d, geomBuffer, R, binningBuffer,
+                        imageBuffer, debug, sh_rest, raw_params, bg_image, sh_factor_mode, want_dbg, sh_grad, sh_rest_grad,
+                        true);
 }
 
 std::vector<torch::Tensor>
@@ -612,8 +701,10 @@ RasterizeGaussiansBatchCapacity(const torch::Tensor& background, const torch::Te
 // dL_dopacity [P,1], dL_dmeans3D [P,3], dL_dsh ([P,M,3], or [P,1,3] with sh_rest), dL_dsh_rest, dL_dts [P,1],
 // dL_dscales [P,3], dL_dscales_t [P,1], dL_drotations [P,4], dL_drotations_r [P,4], and dL_dbg_image [B,3,H,W] (empty
 // unless want_dbg).
+namespace {
+// rasterize_gaussians_backward_batch, and with `camera` rasterize_gaussians_backward_batch_camera
 std::vector<torch::Tensor>
-RasterizeGaussiansBackwardBatch(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& out_means3D,
+backward_batch(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& out_means3D,
                                 const torch::Tensor& radii, const torch::Tensor& flows, const torch::Tensor& opacities,
                                 const torch::Tensor& ts, const torch::Tensor& scales, const torch::Tensor& scales_t,
                                 const torch::Tensor& rotations, const torch::Tensor& rotations_r, const float scale_modifier,
@@ -625,7 +716,7 @@ RasterizeGaussiansBackwardBatch(const torch::Tensor& background, const torch::Te
                                 const int degree, const int degree_t, const float time_duration, const bool rot_4d,
                                 const int gaussian_dim, const bool force_sh_3d, const torch::Tensor& geomBuffer, const int R,
                                 const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer, const bool debug,
-                                const bool raw_params, const torch::Tensor& bg_image, const bool want_dbg) {
+                                const bool raw_params, const torch::Tensor& bg_image, const bool want_dbg, const bool camera) {
     TORCH_CHECK(means3D.dim() == 2 && means3D.size(1) == 3, "means3D must have dimensions (num_points, 3)");
     const BatchCams cams = batch_cameras(means3D, viewmatrix, projmatrix, campos, timestamps, tanfovx, tanfovy);
     const int B = cams.B, P = means3D.size(0);
@@ -671,9 +762,61 @@ RasterizeGaussiansBackwardBatch(const torch::Tensor& background, const torch::Te
     b.B = B; b.bg_image = bgi; b.bg_views = bgi ? B : 0;
     b.dL_dbg_image = want_dbg ? dL_dbg_image.data_ptr<float>() : nullptr;
     b.scratch = reinterpret_cast<char*>(scratch.data_ptr());
-    check(fdgs_backward_batch(&b, (void*)on.stream), "backward_batch");
-    return {dL_dmeans2D, dL_dopacity, dL_dmeans3D, dL_dsh, dL_dsh_rest, dL_dts, dL_dscales, dL_dscales_t, dL_drot, dL_drot_r,
-            dL_dbg_image};
+    if (!camera) {
+        check(fdgs_backward_batch(&b, (void*)on.stream), "backward_batch");
+        return {dL_dmeans2D, dL_dopacity, dL_dmeans3D, dL_dsh, dL_dsh_rest, dL_dts, dL_dscales, dL_dscales_t, dL_drot,
+                dL_drot_r, dL_dbg_image};
+    }
+    CameraGrads cam(viewmatrix, projmatrix, campos, means3D, P, B);
+    check(fdgs_backward_batch_camera(&b, &cam.out, (void*)on.stream), "backward_batch_camera");
+    return {dL_dmeans2D, dL_dopacity, dL_dmeans3D, dL_dsh, dL_dsh_rest, dL_dts, dL_dscales, dL_dscales_t, dL_drot,
+            dL_drot_r, dL_dbg_image, cam.view, cam.proj, cam.campos};
+}
+}  // namespace
+
+std::vector<torch::Tensor>
+RasterizeGaussiansBackwardBatch(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& out_means3D,
+                                const torch::Tensor& radii, const torch::Tensor& flows, const torch::Tensor& opacities,
+                                const torch::Tensor& ts, const torch::Tensor& scales, const torch::Tensor& scales_t,
+                                const torch::Tensor& rotations, const torch::Tensor& rotations_r, const float scale_modifier,
+                                const float prefilter_var, const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix,
+                                const torch::Tensor& campos, const torch::Tensor& timestamps, const torch::Tensor& tanfovx,
+                                const torch::Tensor& tanfovy, const torch::Tensor& dL_dout_color,
+                                const torch::Tensor& dL_dout_depth, const torch::Tensor& dL_dout_mask,
+                                const torch::Tensor& dL_dout_flow, const torch::Tensor& sh, const torch::Tensor& sh_rest,
+                                const int degree, const int degree_t, const float time_duration, const bool rot_4d,
+                                const int gaussian_dim, const bool force_sh_3d, const torch::Tensor& geomBuffer, const int R,
+                                const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer, const bool debug,
+                                const bool raw_params, const torch::Tensor& bg_image, const bool want_dbg) {
+    return backward_batch(background, means3D, out_means3D, radii, flows, opacities, ts, scales, scales_t, rotations,
+                          rotations_r, scale_modifier, prefilter_var, viewmatrix, projmatrix, campos, timestamps, tanfovx,
+                          tanfovy, dL_dout_color, dL_dout_depth, dL_dout_mask, dL_dout_flow, sh, sh_rest, degree, degree_t,
+                          time_duration, rot_4d, gaussian_dim, force_sh_3d, geomBuffer, R, binningBuffer, imageBuffer, debug,
+                          raw_params, bg_image, want_dbg, false);
+}
+
+// rasterize_gaussians_backward_batch's arguments; returns its 11 tensors and then each view's dL_dviewmatrix,
+// dL_dprojmatrix and dL_dcampos, shaped like viewmatrix [B,4,4] | [B,16], projmatrix and campos [B,3]
+// (include/fdgs.h: fdgs_backward_batch_camera)
+std::vector<torch::Tensor>
+RasterizeGaussiansBackwardBatchCamera(const torch::Tensor& background, const torch::Tensor& means3D, const torch::Tensor& out_means3D,
+                                const torch::Tensor& radii, const torch::Tensor& flows, const torch::Tensor& opacities,
+                                const torch::Tensor& ts, const torch::Tensor& scales, const torch::Tensor& scales_t,
+                                const torch::Tensor& rotations, const torch::Tensor& rotations_r, const float scale_modifier,
+                                const float prefilter_var, const torch::Tensor& viewmatrix, const torch::Tensor& projmatrix,
+                                const torch::Tensor& campos, const torch::Tensor& timestamps, const torch::Tensor& tanfovx,
+                                const torch::Tensor& tanfovy, const torch::Tensor& dL_dout_color,
+                                const torch::Tensor& dL_dout_depth, const torch::Tensor& dL_dout_mask,
+                                const torch::Tensor& dL_dout_flow, const torch::Tensor& sh, const torch::Tensor& sh_rest,
+                                const int degree, const int degree_t, const float time_duration, const bool rot_4d,
+                                const int gaussian_dim, const bool force_sh_3d, const torch::Tensor& geomBuffer, const int R,
+                                const torch::Tensor& binningBuffer, const torch::Tensor& imageBuffer, const bool debug,
+                                const bool raw_params, const torch::Tensor& bg_image, const bool want_dbg) {
+    return backward_batch(background, means3D, out_means3D, radii, flows, opacities, ts, scales, scales_t, rotations,
+                          rotations_r, scale_modifier, prefilter_var, viewmatrix, projmatrix, campos, timestamps, tanfovx,
+                          tanfovy, dL_dout_color, dL_dout_depth, dL_dout_mask, dL_dout_flow, sh, sh_rest, degree, degree_t,
+                          time_duration, rot_4d, gaussian_dim, force_sh_3d, geomBuffer, R, binningBuffer, imageBuffer, debug,
+                          raw_params, bg_image, want_dbg, true);
 }
 
 // Test hook: view `view` of a batch's tile ranges [tiles,2] and n_contrib [H,W]
@@ -1381,6 +1524,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("rasterize_gaussians_backward_ext", &RasterizeGaussiansBackwardExtZeroSh);
     m.def("rasterize_gaussians_batch", &RasterizeGaussiansBatch);
     m.def("rasterize_gaussians_backward_batch", &RasterizeGaussiansBackwardBatch);
+    m.def("rasterize_gaussians_backward_camera", &RasterizeGaussiansBackwardCamera);
+    m.def("rasterize_gaussians_backward_batch_camera", &RasterizeGaussiansBackwardBatchCamera);
     m.def("rasterize_gaussians_batch_capacity", &RasterizeGaussiansBatchCapacity);
     m.def("debug_export_binning_view", &DebugExportBinningView);
     m.def("sky_forward", &SkyForward);

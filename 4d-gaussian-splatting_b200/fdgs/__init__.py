@@ -36,6 +36,7 @@ ABI_SYMBOLS = (
     "fdgs_backward_batch", "fdgs_debug_export_binning_view", "fdgs_forward_zero_sh", "fdgs_backward_zero_sh",
     "fdgs_forward_batch_capacity", "fdgs_densify_stats_status", "fdgs_adam_scalars", "fdgs_adam_step_staged",
     "fdgs_sky_forward_batch", "fdgs_sky_backward_batch",
+    "fdgs_camera_grad_scratch_bytes", "fdgs_backward_camera", "fdgs_backward_batch_camera",
 )
 
 STAGE_NAMES = ("preprocess_fwd", "bin_count_scan", "bin_scatter", "tile_sort_pack", "reserved", "blend_fwd", "blend_bwd",

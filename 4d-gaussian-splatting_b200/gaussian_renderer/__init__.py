@@ -48,11 +48,28 @@ def _fused_prologue_ok(pc, pipe, override_color):
             and pc._features_dc.dim() == 3 and pc._features_dc.shape[1] == 1)
 
 
+def _check_sky_camera(cams):
+    """The sky sampler has no camera gradient: with an environment map, a camera tensor that requires a gradient would
+    receive only the rasterizer's share of it, so it is refused (ValueError)."""
+    if not torch.is_grad_enabled():
+        return
+    for c in cams:
+        for name in ("world_view_transform", "full_proj_transform", "camera_center"):
+            t = getattr(c, name, None)
+            if isinstance(t, torch.Tensor) and t.requires_grad:
+                raise ValueError("camera %s requires a gradient, but the environment-map sky has no camera gradient: "
+                                 "render without env_map_res, or detach the camera" % name)
+
+
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None):
     """Render the scene from `viewpoint_camera` (background tensor must live on the GPU).
 
     Same contract as the reference's render(): returns {"render", "viewspace_points",
     "visibility_filter", "radii", "depth", "alpha", "flow"}.
+
+    The camera's world_view_transform, full_proj_transform and camera_center receive gradients when they require them
+    (pose refinement, INTEGRATION.md), except with an environment map (pipe.env_map_res): its sky has no camera
+    gradient, and such a call raises ValueError.
     """
     xyz = pc.get_xyz
     dev = xyz.device
@@ -64,6 +81,8 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
         pass
 
     env_map_res = getattr(pipe, "env_map_res", 0)
+    if env_map_res:
+        _check_sky_camera([viewpoint_camera])
     duration = pc.time_duration[1] - pc.time_duration[0]
     settings = GaussianRasterizationSettings(
         image_height=int(viewpoint_camera.image_height),
@@ -215,7 +234,11 @@ def render_batch(viewpoint_cameras, pc, pipe, bg_color: torch.Tensor, scaling_mo
     it synchronises after every stage).  An environment map needs StaticViews(..., sky=True) (ValueError otherwise): the
     sky of every view is then sampled by one batched call on the views' device cameras (fdgs.sky.sample_sky_batch), and
     the result has a ninth key, "sky_miss" (int32 [1] on the device: 1 if a ray missed the sky sphere), which nothing
-    here reads -- the caller asserts on it, as fdgs.graph.GraphedStep does."""
+    here reads -- the caller asserts on it, as fdgs.graph.GraphedStep does.
+
+    Camera tensors that require a gradient receive it as in render(): each camera's world_view_transform,
+    full_proj_transform and camera_center get their view's gradient through the stack of the views' cameras (and, as
+    there, not with an environment map: ValueError)."""
     from fdgs.graph import StaticViews
     views = viewpoint_cameras if isinstance(viewpoint_cameras, StaticViews) else None
     cams = None if views is not None else list(viewpoint_cameras)
@@ -244,6 +267,8 @@ def render_batch(viewpoint_cameras, pc, pipe, bg_color: torch.Tensor, scaling_mo
             if (int(c.image_height), int(c.image_width)) != (H, W):
                 raise ValueError("render_batch views must share the image size: %dx%d and %dx%d"
                                  % (W, H, int(c.image_width), int(c.image_height)))
+        if env_map_res:
+            _check_sky_camera(cams)
 
     xyz = pc.get_xyz
     dev = xyz.device

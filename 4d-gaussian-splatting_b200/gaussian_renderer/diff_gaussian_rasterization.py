@@ -15,6 +15,11 @@ raw-parameter `forward_raw`) run through one autograd Function, which calls `_C.
 and `_C.rasterize_gaussians_backward_ext`: the reference's 30 / 37 positional arguments followed by
 the extensions.  So under `debug` a failing call's snapshot holds that extended argument tuple; its
 first 30 (forward) or 37 (backward) entries are the reference's layout.
+
+The camera tensors of the settings (viewmatrix, projmatrix, campos) are inputs of both autograd Functions.  When one of
+them requires a gradient, the backward calls `_C.rasterize_gaussians_backward_camera` (batched:
+`_C.rasterize_gaussians_backward_batch_camera`), which returns the same gradients plus the camera's
+(include/fdgs.h: fdgs_backward_camera); otherwise it calls exactly what it calls without them.
 """
 from typing import NamedTuple
 
@@ -113,7 +118,8 @@ class GaussianRasterizationSettings(NamedTuple):
 
 class _RasterizeGaussians(torch.autograd.Function):
     """reference: :67-225.  Inputs, in order: means3D, means2D, sh, sh_rest, colors_precomp, flow_2d, opacities, ts,
-    scales, scales_t, rotations, rotations_r, cov3Ds_precomp, prefilter_var, raster_settings, raw, bg_image.
+    scales, scales_t, rotations, rotations_r, cov3Ds_precomp, prefilter_var, raster_settings, raw, bg_image, grad_sh,
+    viewmatrix, projmatrix, campos.
 
     raw: the raw-parameter entry (no reference counterpart; SURVEY.md section 8(f) row 1).  The inputs are then the
     optimiser's RAW parameters -- log-scales, un-normalised quaternions, opacity logits, and the SH row as the two tensors
@@ -122,11 +128,14 @@ class _RasterizeGaussians(torch.autograd.Function):
     (scene/gaussian_model.py:179-219), with their autograd mirror images, disappear from the frame.  Otherwise sh_rest is
     empty.  bg_image: a per-pixel background [3,H,W] behind the Gaussians, or None.  grad_sh: the caller runs under grad
     mode and the SH input requires a gradient -- the forward then allocates the dense SH gradient and its blend writes
-    the zero rows of the Gaussians this view does not render, so that the backward writes only the rendered rows."""
+    the zero rows of the Gaussians this view does not render, so that the backward writes only the rendered rows.
+    viewmatrix, projmatrix, campos: the settings' camera tensors, passed again as inputs so that they can receive a
+    gradient (the forward reads them from the settings)."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, sh_rest, colors_precomp, flow_2d, opacities, ts, scales, scales_t,
-                rotations, rotations_r, cov3Ds_precomp, prefilter_var, raster_settings, raw, bg_image, grad_sh):
+                rotations, rotations_r, cov3Ds_precomp, prefilter_var, raster_settings, raw, bg_image, grad_sh,
+                viewmatrix, projmatrix, campos):
         s = raster_settings
         g_sh = g_sh_rest = _NONE
         if grad_sh and sh.numel() > 0 and colors_precomp.numel() == 0 and not _wants_factors(sh, cov3Ds_precomp):
@@ -183,6 +192,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         # once returned, the tensors belong to autograd: a second backward (retain_graph) allocates its own
         ctx.g_sh = (_NONE, _NONE)
         want_bg = ctx.needs_input_grad[16]
+        want_cam = any(ctx.needs_input_grad[18:21])
         # _C.rasterize_gaussians_backward's positional layout (reference: :154-190, rasterize_points.h:51-89) + the
         # extensions
         args = (s.bg, means3D, out_means3D, radii, colors_precomp, flow_2d, opacities, ts, scales, scales_t,
@@ -192,8 +202,14 @@ class _RasterizeGaussians(torch.autograd.Function):
                 s.force_sh_3d, geom_buf, ctx.num_rendered, binning_buf, img_buf, s.debug,
                 sh_rest, ctx.raw, _NONE if ctx.bg_image is None else ctx.bg_image, bool(factors), bool(want_bg),
                 zeroed_sh, zeroed_sh_rest)
+        g_cam = (None, None, None)
+        if want_cam:
+            out = _invoke(_C.rasterize_gaussians_backward_camera, args, s.debug, "snapshot_bw.dump")
+            g_cam = tuple(g if need else None for g, need in zip(out[15:], ctx.needs_input_grad[18:21]))
+        else:
+            out = _invoke(_C.rasterize_gaussians_backward_ext, args, s.debug, "snapshot_bw.dump")
         (g_means2D, g_colors, g_opacities, g_means3D, g_cov3D, g_sh, g_flows, g_ts, g_scales, g_scales_t, g_rot, g_rot_r,
-         sh_factors, g_sh_rest, g_bg) = _invoke(_C.rasterize_gaussians_backward_ext, args, s.debug, "snapshot_bw.dump")
+         sh_factors, g_sh_rest, g_bg) = out[:15]
         if factors:
             inputs = dict(means3D=means3D, ts=ts, scales=scales, scales_t=scales_t, rotations=rotations,
                           rotations_r=rotations_r)
@@ -210,18 +226,20 @@ class _RasterizeGaussians(torch.autograd.Function):
         return (g_means3D, g_means2D, for_input(g_sh, sh), for_input(g_sh_rest, sh_rest), for_input(g_colors, colors_precomp),
                 for_input(g_flows, flow_2d), g_opacities, for_input(g_ts, ts), for_input(g_scales, scales),
                 for_input(g_scales_t, scales_t), for_input(g_rot, rotations), for_input(g_rot_r, rotations_r),
-                for_input(g_cov3D, cov3Ds_precomp), None, None, None, g_bg if want_bg else None, None)
+                for_input(g_cov3D, cov3Ds_precomp), None, None, None, g_bg if want_bg else None, None) + g_cam
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, flow_2d, opacities, ts, scales, scales_t,
                         rotations, rotations_r, cov3Ds_precomp, prefilter_var, raster_settings, bg_image=None):
     """Functional entry point (reference: :34-65).  bg_image: optional per-pixel background [3,H,W] (float32, on the
     Gaussians' device) behind the Gaussians; the image is then `rendered + (1 - alpha) * bg_image`, bit for bit, and
-    bg_image receives a gradient when it requires one."""
+    bg_image receives a gradient when it requires one.  So do raster_settings.viewmatrix / projmatrix / campos: their
+    gradients have their shapes (see include/fdgs.h: fdgs_backward_camera)."""
     _check_bg_image(bg_image, raster_settings, means3D)
+    s = raster_settings
     return _RasterizeGaussians.apply(means3D, means2D, sh, _NONE, colors_precomp, flow_2d, opacities, ts, scales,
                                      scales_t, rotations, rotations_r, cov3Ds_precomp, prefilter_var,
-                                     raster_settings, False, bg_image, _grad_sh(sh))
+                                     raster_settings, False, bg_image, _grad_sh(sh), s.viewmatrix, s.projmatrix, s.campos)
 
 
 class GaussianRasterizer(nn.Module):
@@ -249,10 +267,11 @@ class GaussianRasterizer(nn.Module):
             return torch.Tensor([]) if t is None else t
 
         _check_bg_image(bg_image, self.raster_settings, means3D)
+        s = self.raster_settings
         return _RasterizeGaussians.apply(means3D, means2D, features_dc, opt(features_rest), _NONE, opt(flow_2d),
                                          opacity_logits, opt(ts), log_scales, opt(log_scales_t), rotations_raw,
                                          opt(rotations_r_raw), _NONE, prefilter_var, self.raster_settings, True, bg_image,
-                                         _grad_sh(features_dc, features_rest))
+                                         _grad_sh(features_dc, features_rest), s.viewmatrix, s.projmatrix, s.campos)
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, flow_2d=None, ts=None,
                 scales=None, scales_t=None, rotations=None, rotations_r=None, cov3D_precomp=None,
@@ -306,18 +325,22 @@ class BatchRasterizationSettings(NamedTuple):
 class _RasterizeGaussiansBatch(torch.autograd.Function):
     """B views of the same Gaussians in one forward and one backward (include/fdgs.h: fdgs_forward_batch).  Inputs, in
     order: means3D, means2D [B,P,3], sh, sh_rest, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
-    prefilter_var, settings (BatchRasterizationSettings), raw, bg_image ([B,3,H,W] or None).  raw and sh / sh_rest as in
+    prefilter_var, settings (BatchRasterizationSettings), raw, bg_image ([B,3,H,W] or None), capacity, viewmatrix,
+    projmatrix, campos.  raw and sh / sh_rest as in
     _RasterizeGaussians.  Returns color [B,3,H,W], radii [B,P], depth [B,1,H,W], alpha [B,1,H,W], flow [B,2,H,W].
     Every per-Gaussian gradient is the sum of the views' gradients in view order; means2D's gradient stays per view.
 
     capacity (an int >= 0) selects the entry sized by an instance capacity (_C.rasterize_gaussians_batch_capacity), which
     never synchronises with the host and can be captured in a CUDA graph: settings.timestamp / tanfovx / tanfovy are then
     float32 CUDA tensors [B], and a sixth output, status (int32 [4] on the device: R, largest tile, overflow, wrap),
-    follows the five images.  On overflow the views render as if no Gaussian were listed, and the gradients are zero."""
+    follows the five images.  On overflow the views render as if no Gaussian were listed, and the gradients are zero.
+
+    viewmatrix, projmatrix, campos: the settings' camera tables, passed again as inputs so that they can receive a
+    gradient, each view its own (rasterize_gaussians_backward_batch_camera)."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, sh_rest, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
-                prefilter_var, settings, raw, bg_image, capacity=None):
+                prefilter_var, settings, raw, bg_image, capacity, viewmatrix, projmatrix, campos):
         s = settings
         if capacity is None:
             cams = (s.viewmatrix, s.projmatrix, s.campos) + tuple(
@@ -368,20 +391,26 @@ class _RasterizeGaussiansBatch(torch.autograd.Function):
         grad_alpha = none if grad_alpha is None else grad_alpha
         grad_flow = none if grad_flow is None else grad_flow
         want_bg = ctx.needs_input_grad[14]
+        want_cam = any(ctx.needs_input_grad[16:19])
         args = (s.bg, means3D, out_means3D, radii, flow_2d, opacities, ts, scales, scales_t, rotations, rotations_r,
                 s.scale_modifier, ctx.prefilter_var) + ctx.cams + (
             grad_color, grad_depth, grad_alpha, grad_flow, sh, sh_rest, s.sh_degree, s.sh_degree_t, s.time_duration,
             s.rot_4d, s.gaussian_dim, s.force_sh_3d, geom_buf, ctx.num_rendered, binning_buf, img_buf, s.debug, ctx.raw,
             _NONE if ctx.bg_image is None else ctx.bg_image, bool(want_bg))
-        (g_means2D, g_opacities, g_means3D, g_sh, g_sh_rest, g_ts, g_scales, g_scales_t, g_rot, g_rot_r,
-         g_bg) = _invoke(_C.rasterize_gaussians_backward_batch, args, s.debug, "snapshot_bw.dump")
+        g_cam = (None, None, None)
+        if want_cam:
+            out = _invoke(_C.rasterize_gaussians_backward_batch_camera, args, s.debug, "snapshot_bw.dump")
+            g_cam = tuple(g if need else None for g, need in zip(out[11:], ctx.needs_input_grad[16:19]))
+        else:
+            out = _invoke(_C.rasterize_gaussians_backward_batch, args, s.debug, "snapshot_bw.dump")
+        (g_means2D, g_opacities, g_means3D, g_sh, g_sh_rest, g_ts, g_scales, g_scales_t, g_rot, g_rot_r, g_bg) = out[:11]
 
         def for_input(grad, inp):
             return grad if inp.numel() > 0 else None
 
         return (g_means3D, g_means2D, g_sh, for_input(g_sh_rest, sh_rest), None, g_opacities, for_input(g_ts, ts),
                 g_scales, for_input(g_scales_t, scales_t), g_rot, for_input(g_rot_r, rotations_r), None, None, None,
-                g_bg if want_bg else None) + ((None,) if ctx.capacity else ())
+                g_bg if want_bg else None, None) + g_cam
 
 
 _HOST_PLACEHOLDERS = {}
@@ -403,7 +432,8 @@ def rasterize_gaussians_batch(means3D, means2D, opacities, sh, scales, rotations
     optimiser's raw parameters (forward_raw's convention: sh = features_dc, sh_rest = features_rest).  bg_image: per-view
     background images [B,3,H,W] behind the Gaussians, or None.  capacity: None, or the instance capacity of the entry
     that does not synchronise (the per-view scalars of `settings` are then CUDA tensors [B] and a sixth output, the
-    device status, is returned)."""
+    device status, is returned).  settings.viewmatrix / projmatrix / campos receive their gradients, one per view, when
+    they require them."""
     B = int(settings.viewmatrix.shape[0])
     P = int(means3D.shape[0])
     if tuple(means2D.shape) != (B, P, 3):
@@ -421,10 +451,7 @@ def rasterize_gaussians_batch(means3D, means2D, opacities, sh, scales, rotations
     def opt(t):
         return _NONE if t is None else t
 
-    if capacity is None:
-        return _RasterizeGaussiansBatch.apply(means3D, means2D, sh, opt(sh_rest), opt(flow_2d), opacities, opt(ts), scales,
-                                              opt(scales_t), rotations, opt(rotations_r), prefilter_var, settings, raw,
-                                              bg_image)
     return _RasterizeGaussiansBatch.apply(means3D, means2D, sh, opt(sh_rest), opt(flow_2d), opacities, opt(ts), scales,
                                           opt(scales_t), rotations, opt(rotations_r), prefilter_var, settings, raw,
-                                          bg_image, int(capacity))
+                                          bg_image, None if capacity is None else int(capacity), settings.viewmatrix,
+                                          settings.projmatrix, settings.campos)

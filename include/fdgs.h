@@ -290,6 +290,34 @@ int fdgs_forward_batch(const fdgs_forward_batch_args* args,
                        fdgs_forward_result* result);
 int fdgs_backward_batch(const fdgs_backward_batch_args* args, void* stream);
 
+/* Camera gradients: the backward also returns dL/dviewmatrix, dL/dprojmatrix and dL/dcampos, for pose refinement,
+ * rig calibration or tracking through the rasterizer.  fdgs_backward_camera is fdgs_backward_zero_sh and
+ * fdgs_backward_batch_camera is fdgs_backward_batch, with every other output the same, plus:
+ *   dL_dviewmatrix / dL_dprojmatrix   [16] ([B,16] batched), in the layout of viewmatrix / projmatrix: element 4c + r
+ *                                     is the gradient of the caller's element 4c + r.  Entries the forward does not
+ *                                     read are exactly 0: 3, 7, 11, 15 of the view matrix (view-space w) and 2, 6, 10,
+ *                                     14 of the projection matrix (clip z).
+ *   dL_dcampos                        [3] ([B,3]); the camera centre enters only the SH view direction, so it is 0 with
+ *                                     colors_precomp.
+ * Each is the sum over the Gaussians the view renders (radii > 0, a tile touched) of the reference backward's own
+ * per-Gaussian terms (backward.cu: the view-space mean's gradient, the W part of the EWA Jacobian product T = J W,
+ * the homogeneous projection and the SH direction), applied to the camera instead of the mean, so that
+ *     sum_i dL/dmeans3D[i] + dL/dcampos = V[0:12] (3x4, row-major) @ dL/dV[12:16] + Pm[0:12] @ dL/dPm[12:16]
+ * (moving world and camera together leaves the image unchanged).  The sums are reduced without floating-point
+ * atomics, per block and then over the blocks in a fixed order in fp64: the camera gradient of a call is deterministic.
+ * scratch: fdgs_camera_grad_scratch_bytes(P, B) bytes of device memory (B = 1 for fdgs_backward_camera).  A NULL output
+ * or scratch, or a bad B, is rejected before any launch. */
+typedef struct fdgs_camera_grad_out {
+    float* dL_dviewmatrix;     /* [B,16] overwritten */
+    float* dL_dprojmatrix;     /* [B,16] overwritten */
+    float* dL_dcampos;         /* [B,3]  overwritten */
+    char* scratch;
+} fdgs_camera_grad_out;
+size_t fdgs_camera_grad_scratch_bytes(int P, int B);
+int fdgs_backward_camera(const fdgs_backward_args* args, const float* bg_image, float* dL_dbg_image, int sh_rows_zeroed,
+                         const fdgs_camera_grad_out* cam, void* stream);
+int fdgs_backward_batch_camera(const fdgs_backward_batch_args* args, const fdgs_camera_grad_out* cam, void* stream);
+
 /* The batched forward sized by an instance capacity instead of the exact count: no host synchronisation, no read of
  * device memory on the host and no upload of host data, so the call can be captured in a CUDA graph and replayed with
  * new cameras.  `batch` as in fdgs_forward_batch, except that its host timestamps / tan_fovx / tan_fovy are ignored: the
