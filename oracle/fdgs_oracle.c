@@ -915,6 +915,106 @@ void oracle_preprocess_backward(const OracleScene* s, const float* means /* shif
     }
 }
 
+/* The camera's per-row gradient terms: the reference backward's own per-Gaussian arithmetic (computeCov2DCUDA,
+ * preprocessCUDA's projection, the SH view direction) applied to the view matrix V, the projection Pm and the camera
+ * position instead of the mean.  terms [P,27], zero-initialised by the caller, row idx written when the row is rendered
+ * (radius > 0 and at least one tile), in this order:
+ *   3c + r (c, r < 3)  dL/dV[4c + r] = m_c g_r + sum_i J[i][r] dL/dT[i][c]   (t = W m + V[12..14], T = J W)
+ *   9 + r              dL/dV[12 + r] = g_r                                   (g: the view-space point's gradient)
+ *   12 + 3c + j        dL/dPm[4c + r_j] = m_c gp_j, m_3 = 1, r_j = 0, 1, 3    (gp = dL/d(clip x, y, w))
+ *   24 + k             dL/dcampos[k] = -(the SH direction part of dL/dmean[k])
+ * Inputs as oracle_preprocess_backward's. */
+void oracle_camera_terms(const OracleScene* s, const float* means /* shifted, [P,3] */, const int* radii,
+                         const uint8_t* clamped, const uint32_t* tiles_touched, const float* cov3Ds,
+                         const float* dL_dmean2D, const float* dL_dconics, const float* dL_dcolor, float* terms) {
+    const float h_y = s->H / (2.0f * s->tan_fovy);
+    const float h_x = s->W / (2.0f * s->tan_fovx);
+    const float* V = s->viewmatrix;
+    const float* proj = s->projmatrix;
+    float* sh_mean = NULL;
+    float* sh_dsh = NULL;
+    float* sh_dts = NULL;
+    if (s->shs) {
+        sh_mean = (float*)calloc((size_t)s->P * 3, sizeof(float));
+        sh_dsh = (float*)calloc((size_t)s->P * (s->M > 0 ? s->M : 1) * 3, sizeof(float));
+        sh_dts = (float*)calloc((size_t)s->P, sizeof(float));
+        if (!sh_mean || !sh_dsh || !sh_dts) abort();
+    }
+    for (int idx = 0; idx < s->P; ++idx) {
+        if (!(radii[idx] > 0) || tiles_touched[idx] == 0) continue;
+        float* out = terms + 27 * (size_t)idx;
+        const float* cov3D = cov3Ds + 6 * idx;
+        const float mean[3] = {means[3 * idx], means[3 * idx + 1], means[3 * idx + 2]};
+        { /* computeCov2DCUDA */
+            const float dcx = dL_dconics[4 * idx], dcy = dL_dconics[4 * idx + 1], dcz = dL_dconics[4 * idx + 3];
+            ProjT Pj;
+            build_T(V, mean[0], mean[1], mean[2], h_x, h_y, s->tan_fovx, s->tan_fovy, &Pj);
+            const float limx = 1.3f * s->tan_fovx, limy = 1.3f * s->tan_fovy;
+            const float x_grad_mul = (Pj.txtz < -limx || Pj.txtz > limx) ? 0.f : 1.f;
+            const float y_grad_mul = (Pj.tytz < -limy || Pj.tytz > limy) ? 0.f : 1.f;
+            float a, b, c;
+            cov2d(&Pj, cov3D, &a, &b, &c);
+            a += 0.3f;
+            c += 0.3f;
+            const float (*T)[3] = Pj.T;
+            const float denom = a * c - b * b;
+            float dL_da = 0, dL_db = 0, dL_dc = 0;
+            const float denom2inv = 1.0f / ((denom * denom) + 0.0000001f);
+            if (denom2inv != 0) {
+                dL_da = denom2inv * (-c * c * dcx + 2 * b * c * dcy + (denom - a * c) * dcz);
+                dL_dc = denom2inv * (-a * a * dcz + 2 * a * b * dcy + (denom - a * c) * dcx);
+                dL_db = denom2inv * 2 * (b * c * dcx - (denom + 2 * b * b) * dcy + a * b * dcz);
+            }
+            const float Vrk[3][3] = {{cov3D[0], cov3D[1], cov3D[2]}, {cov3D[1], cov3D[3], cov3D[4]}, {cov3D[2], cov3D[4], cov3D[5]}};
+            float dL_dT[2][3];
+            for (int j = 0; j < 3; ++j) {
+                const float r0 = T[0][0] * Vrk[j][0] + T[0][1] * Vrk[j][1] + T[0][2] * Vrk[j][2];
+                const float r1 = T[1][0] * Vrk[j][0] + T[1][1] * Vrk[j][1] + T[1][2] * Vrk[j][2];
+                dL_dT[0][j] = 2 * r0 * dL_da + r1 * dL_db;
+                dL_dT[1][j] = 2 * r1 * dL_dc + r0 * dL_db;
+            }
+            const float dL_dJ00 = V[0] * dL_dT[0][0] + V[4] * dL_dT[0][1] + V[8] * dL_dT[0][2];
+            const float dL_dJ02 = V[2] * dL_dT[0][0] + V[6] * dL_dT[0][1] + V[10] * dL_dT[0][2];
+            const float dL_dJ11 = V[1] * dL_dT[1][0] + V[5] * dL_dT[1][1] + V[9] * dL_dT[1][2];
+            const float dL_dJ12 = V[2] * dL_dT[1][0] + V[6] * dL_dT[1][1] + V[10] * dL_dT[1][2];
+            const float tz = 1.f / Pj.tz, tz2 = tz * tz, tz3 = tz2 * tz;
+            const float vx = x_grad_mul * -h_x * tz2 * dL_dJ02;
+            const float vy = y_grad_mul * -h_y * tz2 * dL_dJ12;
+            const float vz = -h_x * tz2 * dL_dJ00 - h_y * tz2 * dL_dJ11 + (2 * h_x * Pj.tx) * tz3 * dL_dJ02 +
+                             (2 * h_y * Pj.ty) * tz3 * dL_dJ12 + dL_dmean2D[3 * idx + 2];
+            /* the Jacobian J of forward.cu:204-223 with the clamped tx, ty */
+            const float j00 = h_x / Pj.tz, j11 = h_y / Pj.tz;
+            const float j02 = (h_x * -Pj.tx) / (Pj.tz * Pj.tz), j12 = (h_y * -Pj.ty) / (Pj.tz * Pj.tz);
+            for (int cc = 0; cc < 3; ++cc) {
+                out[3 * cc + 0] = mean[cc] * vx + j00 * dL_dT[0][cc];
+                out[3 * cc + 1] = mean[cc] * vy + j11 * dL_dT[1][cc];
+                out[3 * cc + 2] = mean[cc] * vz + (j02 * dL_dT[0][cc] + j12 * dL_dT[1][cc]);
+            }
+            out[9] = vx;
+            out[10] = vy;
+            out[11] = vz;
+        }
+        { /* backward.cu:877-894: the homogeneous projection p = Pm [m, 1] */
+            const float m_w = 1.0f / ((proj[3] * mean[0] + proj[7] * mean[1] + proj[11] * mean[2] + proj[15]) + 0.0000001f);
+            const float mul1 = (proj[0] * mean[0] + proj[4] * mean[1] + proj[8] * mean[2] + proj[12]) * m_w * m_w;
+            const float mul2 = (proj[1] * mean[0] + proj[5] * mean[1] + proj[9] * mean[2] + proj[13]) * m_w * m_w;
+            const float gx = dL_dmean2D[3 * idx], gy = dL_dmean2D[3 * idx + 1];
+            const float gp[3] = {gx * m_w, gy * m_w, -(mul1 * gx + mul2 * gy)};
+            const float m4[4] = {mean[0], mean[1], mean[2], 1.f};
+            for (int cc = 0; cc < 4; ++cc)
+                for (int j = 0; j < 3; ++j) out[12 + 3 * cc + j] = m4[cc] * gp[j];
+        }
+        if (s->shs) { /* the view direction is m - campos */
+            const int is4d = !(s->gaussian_dim == 3 || s->force_sh_3d);
+            sh_backward(s, idx, is4d, mean, clamped, dL_dcolor, sh_mean, sh_dsh, sh_dts);
+            for (int k = 0; k < 3; ++k) out[24 + k] = -sh_mean[3 * idx + k];
+        }
+    }
+    free(sh_mean);
+    free(sh_dsh);
+    free(sh_dts);
+}
+
 /* reference: rasterizer_impl.cu:54-67 checkFrustum */
 void oracle_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present) {
     for (int i = 0; i < P; ++i)

@@ -187,6 +187,21 @@ def backward(inp: OracleInputs, fwd, grad_color, grad_depth, grad_alpha, grad_fl
     return g
 
 
+def camera_terms(inp: OracleInputs, fwd, grads):
+    """The camera's 27 per-row gradient terms [P,27] (oracle_camera_terms, zero on the rows not rendered), from the
+    forward's dict and the dict backward() returned (its blend gradients dL_dmeans2D, dL_dconic and dL_dcolors)."""
+    L = lib()
+    u32p = ctypes.POINTER(ctypes.c_uint32)
+    terms = np.zeros((inp.P, 27), np.float32)
+    cov = inp.keep["cov3D_precomp"] if inp.keep["cov3D_precomp"] is not None else fwd["cov3D"]
+    L.oracle_camera_terms(ctypes.byref(inp.c), _f(fwd["out_means3D"]),
+                          fwd["radii"].ctypes.data_as(ctypes.POINTER(ctypes.c_int)),
+                          fwd["clamped"].ctypes.data_as(ctypes.POINTER(ctypes.c_uint8)),
+                          fwd["tiles_touched"].ctypes.data_as(u32p), _f(cov), _f(grads["dL_dmeans2D"]),
+                          _f(grads["dL_dconic"]), _f(grads["dL_dcolors"]), _f(terms))
+    return terms
+
+
 def num_threads():
     return int(lib().oracle_num_threads())
 

@@ -312,33 +312,55 @@ def sh_backward(shs, dcol, clamped, means, campos, ts, timestamp, duration, deg,
 
 
 # ---- EWA part of dL_dmeans3D (geom_bwd_body: computeCov2DCUDA and the projection) -------------------------------------
-def ewa_mean_grad(means, cov3D, dmean2D, dconic, st):
-    """The part of dL_dmeans3D that does not come from the SH colour, from the blend gradients in the form the
-    reference's computeCov2DCUDA consumes: dmean2D [P,3] (x, y and the depth gradient), dconic [P,4] (0, 1, 3 used);
-    means [P,3] the shifted means, cov3D [P,6] the forward's conditional covariances.  Returns (3 E, rows whose view-space
-    x/z or y/z lies within 1e-5 of the 1.3 tan(fov) clamp, where fp32 and float64 may take different branches)."""
-    V = [float(x) for x in st["viewmatrix"].reshape(-1).cpu()]
-    Pm = [float(x) for x in st["projmatrix"].reshape(-1).cpu()]
+def ewa_consts(st, exact=False):
+    """The camera constants of computeCov2DCUDA and the projection: the fp32 values the kernels compute (focal lengths
+    W / (2 tan fov), the clamp limits 1.3 tan fov, the 0.3 low-pass and the 1e-7 guards), or with `exact` the float64
+    values blend_f64 / camera_f64 use, so that a float64 restatement can be compared with their autograd to 1e-12."""
     H, W = np.float32(st["image_height"]), np.float32(st["image_width"])
     tanx, tany = np.float32(st["tanfovx"]), np.float32(st["tanfovy"])
-    fx, fy = float(W / (np.float32(2.0) * tanx)), float(H / (np.float32(2.0) * tany))
-    limx, limy = float(np.float32(1.3) * tanx), float(np.float32(1.3) * tany)
+    if exact:
+        return dict(fx=float(W) / (2.0 * float(tanx)), fy=float(H) / (2.0 * float(tany)), limx=1.3 * float(tanx),
+                    limy=1.3 * float(tany), lowpass=0.3, eps=1e-7)
+    return dict(fx=float(W / (np.float32(2.0) * tanx)), fy=float(H / (np.float32(2.0) * tany)),
+                limx=float(np.float32(1.3) * tanx), limy=float(np.float32(1.3) * tany), lowpass=f32(0.3),
+                eps=f32(0.0000001))
+
+
+def ewa_chain(means, cov3D, dmean2D, dconic, st, exact=False, flip=None):
+    """computeCov2DCUDA and the projection's backward (geom_bwd_body) as E values, from the blend gradients in the form
+    the reference's computeCov2DCUDA consumes: dmean2D [P,3] (x, y and the depth gradient), dconic [P,4] (0, 1, 3 used);
+    means [P,3] the shifted means, cov3D [P,6] the forward's conditional covariances.  flip: None, or two [P] bool masks
+    (x, y) of rows on which the frustum clamp takes the other branch (with a positive field of view only: a negative
+    one clamps every row whatever the value).  Returns a dict of the intermediates: g (the EWA part of dL_dmeans3D, 3 E),
+    near (rows whose view-space x/z or y/z lies within 1e-5 of the 1.3 tan(fov) clamp, where fp32 and float64 may take
+    different branches), nx / ny, and the view-space point's gradient (vx, vy, vz; vz0 without the depth gradient dz),
+    the Jacobian (j00, j11, j02, j12), dL/dT (dT0, dT1), the projection's m_w, mul1, mul2 and d2x, d2y."""
+    V = [float(x) for x in st["viewmatrix"].reshape(-1).cpu()]
+    Pm = [float(x) for x in st["projmatrix"].reshape(-1).cpu()]
+    k = ewa_consts(st, exact)
+    fx, fy, limx, limy = k["fx"], k["fy"], k["limx"], k["limy"]
     m = [col(means, i) for i in range(3)]
     c3 = [col(cov3D, i) for i in range(6)]
     row = lambda a, b, c, d: esum([m[0] * a, m[1] * b, m[2] * c, E(d)])
     tx0, ty0, tz = row(V[0], V[4], V[8], V[12]), row(V[1], V[5], V[9], V[13]), row(V[2], V[6], V[10], V[14])
     txtz, tytz = tx0 / tz, ty0 / tz
 
-    def clamp(r, lim):
+    def clamp(r, lim, f):
         """min(lim, max(-lim, r)) and the gradient mask (lim < 0 with a negative field of view: always clamped)"""
         v = torch.clamp(torch.clamp(r.v, min=-lim), max=lim)
         kept = v == r.v
         out = (r.v < -lim) | (r.v > lim)
+        if f is not None and lim > 0:
+            f = f.to(r.v.device)
+            out = out ^ f
+            one = torch.ones_like(r.v)
+            v = torch.where(f, torch.where(out, torch.where(r.v < 0, -one, one) * lim, r.v), v)
+            kept = torch.where(f, ~out, kept)
         return E(v, torch.where(kept, r.e, torch.zeros_like(r.e))), (~out).double(), \
             (r.v.abs() / abs(lim) - 1.0).abs() <= 1e-5
 
-    cx, xgm, nx = clamp(txtz, limx)
-    cy, ygm, ny = clamp(tytz, limy)
+    cx, xgm, nx = clamp(txtz, limx, None if flip is None else flip[0])
+    cy, ygm, ny = clamp(tytz, limy, None if flip is None else flip[1])
     tx, ty = cx * tz, cy * tz
     tz2 = tz * tz
     j00, j11 = fx / tz, fy / tz
@@ -349,12 +371,12 @@ def ewa_mean_grad(means, cov3D, dmean2D, dconic, st):
     X00, X01 = d3(T00, c3[0], T01, c3[1], T02, c3[2]), d3(T10, c3[0], T11, c3[1], T12, c3[2])
     X10, X11 = d3(T00, c3[1], T01, c3[3], T02, c3[4]), d3(T10, c3[1], T11, c3[3], T12, c3[4])
     X20, X21 = d3(T00, c3[2], T01, c3[4], T02, c3[5]), d3(T10, c3[2], T11, c3[4], T12, c3[5])
-    A = d3(T00, X00, T01, X10, T02, X20) + f32(0.3)
+    A = d3(T00, X00, T01, X10, T02, X20) + k["lowpass"]
     B = d3(T00, X01, T01, X11, T02, X21)
-    C = d3(T10, X01, T11, X11, T12, X21) + f32(0.3)
+    C = d3(T10, X01, T11, X11, T12, X21) + k["lowpass"]
     dcx, dcy, dcz = col(dconic, 0), col(dconic, 1), col(dconic, 3)
     denom = esum([A * C, -(B * B)])
-    d2i = 1.0 / (denom * denom + f32(0.0000001))
+    d2i = 1.0 / (denom * denom + k["eps"])
     dL_da = d2i * esum([-C * C * dcx, 2.0 * B * C * dcy, (denom - A * C) * dcz])
     dL_dc = d2i * esum([-A * A * dcz, 2.0 * A * B * dcy, (denom - A * C) * dcx])
     dL_db = d2i * 2.0 * esum([B * C * dcx, -((denom + 2.0 * B * B) * dcy), A * B * dcz])
@@ -369,17 +391,27 @@ def ewa_mean_grad(means, cov3D, dmean2D, dconic, st):
     t3 = t2 * tzi
     vx = E(xgm) * (-fx * t2 * dJ02)
     vy = E(ygm) * (-fy * t2 * dJ12)
-    vz = esum([-fx * t2 * dJ00, -(fy * t2 * dJ11), (2.0 * fx * tx) * t3 * dJ02, (2.0 * fy * ty) * t3 * dJ12]) + \
-        col(dmean2D, 2)
+    vz0 = esum([-fx * t2 * dJ00, -(fy * t2 * dJ11), (2.0 * fx * tx) * t3 * dJ02, (2.0 * fy * ty) * t3 * dJ12])
+    dz = col(dmean2D, 2)
+    vz = vz0 + dz
     g = [esum([V[0] * vx, V[1] * vy, V[2] * vz]), esum([V[4] * vx, V[5] * vy, V[6] * vz]),
          esum([V[8] * vx, V[9] * vy, V[10] * vz])]
-    m_w = 1.0 / (row(Pm[3], Pm[7], Pm[11], Pm[15]) + f32(0.0000001))
+    m_w = 1.0 / (row(Pm[3], Pm[7], Pm[11], Pm[15]) + k["eps"])
     mul1 = row(Pm[0], Pm[4], Pm[8], Pm[12]) * m_w * m_w
     mul2 = row(Pm[1], Pm[5], Pm[9], Pm[13]) * m_w * m_w
     d2x, d2y = col(dmean2D, 0), col(dmean2D, 1)
     for i in range(3):
         g[i] = esum([g[i], (Pm[4 * i] * m_w - Pm[4 * i + 3] * mul1) * d2x, (Pm[4 * i + 1] * m_w - Pm[4 * i + 3] * mul2) * d2y])
-    return g, nx | ny
+    return dict(g=g, near=nx | ny, nx=nx, ny=ny, m=m, tx=tx, ty=ty, tz=tz, cx=cx, cy=cy, xgm=xgm, ygm=ygm, fx=fx, fy=fy,
+                t2=t2, dJ02=dJ02, dJ12=dJ12, j00=j00, j11=j11, j02=j02, j12=j12, dT0=dT0, dT1=dT1, vx=vx, vy=vy, vz=vz,
+                vz0=vz0, dz=dz, m_w=m_w, mul1=mul1, mul2=mul2, d2x=d2x, d2y=d2y)
+
+
+def ewa_mean_grad(means, cov3D, dmean2D, dconic, st):
+    """The part of dL_dmeans3D that does not come from the SH colour (ewa_chain).  Returns (3 E, rows whose view-space
+    x/z or y/z lies within 1e-5 of the 1.3 tan(fov) clamp, where fp32 and float64 may take different branches)."""
+    r = ewa_chain(means, cov3D, dmean2D, dconic, st)
+    return r["g"], r["near"]
 
 
 # ---- the whole per-Gaussian backward of one view ----------------------------------------------------------------------
